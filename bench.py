@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- LP edges/s on B200 (BASELINE.json metric) for the B200-native label-propagation
+"""bench.py -- LP edges/s on the GPU (BASELINE.json metric) for the CUDA label-propagation
 engine, next to the reference's own CPU path.
 
 A "step" = one ``LPClustering.compute_clustering`` call (5 LP rounds + post passes,
@@ -15,6 +15,7 @@ lp_clusterer.cc:89-109) on the synthetic input, the timed region of the referenc
            stand-in) or, when that library is absent, the oracle port, on a bounded sample
 
 ``--impl reference`` times only the CPU reference arm on the same workload definition.
+``--dump-outputs DIR`` writes, after the timed steps, what the last timed step computed (see dump_outputs).
 """
 from __future__ import annotations
 
@@ -49,6 +50,9 @@ WORKLOADS = {
 # step in about a second (R-MAT 22: ~1.3 s/step on the box's host cores); only the three largest inputs
 # use a smaller graph of the same family so that `--impl reference --steps K --warmup W` (plus the thread
 # sweep) still ends within a few minutes -- the line's config says so ("cpu_sample").
+L2_GATHER_PER_S = 128.6e9
+# L2 of the H100 (50 MB): the config's "l2" field says whether the adjacency array alone exceeds it
+L2_BYTES = 50 << 20
 CPU_SAMPLE = {"rmat24": "rmat22", "grid512": "grid256", "rgg24": "rgg20", "road": "road_small"}
 
 
@@ -57,7 +61,7 @@ def peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (HBM3), not measured"
 
 
 def generate(name, device):
@@ -89,7 +93,7 @@ def generate(name, device):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index):
         self.index = index
@@ -157,6 +161,24 @@ class ClockSampler:
                     reasons.add(nm)
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(smax) if smax else None,
                 "reasons": sorted(reasons), "samples": len(sm), "sampled": where}
+
+
+# --dump-outputs: every array is written as float64 (exact for the 32-bit integers the engine returns); an array
+# longer than its share of this budget is replaced by a fixed, seeded sample of its entries plus their indices
+DUMP_BYTES = 60 << 20
+
+
+def dump_outputs(directory, arrays):
+    """Write `arrays` (name -> 1-D integer array) as DIR/<name>.npy, float64, at most DUMP_BYTES in all."""
+    os.makedirs(directory, exist_ok=True)
+    cap = DUMP_BYTES // 8 // len(arrays)
+    for name, a in arrays.items():
+        a = np.asarray(a).ravel()
+        if a.size > cap:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, cap // 2, replace=False))
+            np.save(os.path.join(directory, f"{name}_sample_index.npy"), idx.astype(np.float64))
+            a = a[idx]
+        np.save(os.path.join(directory, f"{name}.npy"), a.astype(np.float64))
 
 
 def _cpu_worker(name, mode, steps, warmup, host_graph=None):
@@ -228,14 +250,21 @@ def contraction_mode(args, handle, g_host, n, m, k, mcw, dev, local_rank):
     torch.cuda.synchronize()
     sampler.mark_begin()
     tot_ms, launches, last = 0.0, 0, None
+    cg = None
     for _ in range(args.steps):
+        if cg is not None:
+            cg.close()
         cg = KC.contract_on_handle(handle, None)
         tot_ms += cg.stats.device_ms
         launches += cg.stats.kernel_launches
         last = (cg.stats.c_n, cg.stats.c_m, cg.stats.cut_edges, cg.stats.sort_bits)
-        cg.close()
     torch.cuda.synchronize()
     sampler.mark_end()
+    if args.dump_outputs:
+        c = cg.get()
+        dump_outputs(args.dump_outputs, dict(c_xadj=c.xadj, c_adjncy=c.adjncy, c_vwgt=c.vwgt, c_adjwgt=c.adjwgt,
+                                              mapping=cg.mapping()))
+    cg.close()
     clocks = sampler.stop()
     value = m * args.steps / (tot_ms * 1e-3)
     c_n, c_m, cut, bits = last
@@ -271,7 +300,7 @@ def contraction_mode(args, handle, g_host, n, m, k, mcw, dev, local_rank):
         "dtype": "int32", "data": "synthetic",
         "config": {"workload": args.workload, "n": n, "m_directed": m, "k": k, "mode": "contraction",
                    "coarse_n": c_n, "coarse_m": c_m, "inter_cluster_edges": cut, "sort_bits": bits,
-                   "l2": "inputs_larger_than_l2" if m * 4 > 126e6 else "small_input"},
+                   "l2": "inputs_larger_than_l2" if m * 4 > L2_BYTES else "small_input"},
         "clocks": clocks, "e2e": e2e, "gpu_launches": int(launches),
         "roofline": {"bound": "hbm", "kernel": "contract_clustering (key pass + radix sort + reduce-by-key)",
                      "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": None,
@@ -295,14 +324,18 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--workload", default=os.environ.get("KMP_BENCH_WORKLOAD"),
                     help="default: rmat22 (BASELINE config 2) on 1 GPU, rmat24 (config 4: R-MAT scale 24, k=64, "
-                         "2/4/8 x B200) on N > 1")
+                         "2/4/8 GPUs) on N > 1")
     ap.add_argument("--cpu-steps", type=int, default=2)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true", help="profiling runs only: skip the host-buffer arm (e2e = null)")
     ap.add_argument("--mode", default="clustering", choices=["clustering", "refinement", "contraction"],
                     help="refinement: one LabelPropagationRefiner.refine call on a hashed k-way partition (N=1 only); "
                          "contraction: contract_clustering of the LP clustering (SURVEY §8f-1, N=1 only)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what the last timed step computed "
+                    "(the clustering, the refined partition and block weights, or the coarse graph) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.workload is None:
         args.workload = "rmat22" if args.gpus <= 1 else "rmat24"
 
@@ -392,10 +425,14 @@ def main():
 
     sharded_moved = []  # per-round move counts of the last sharded step (identical on every rank)
 
+    last_bw = None  # block weights of the last refinement step
+
     def run_resident():
+        nonlocal last_bw
         if refine_handle is not None:
             refine_handle.upload_partition(part0)
-            return refine_handle.refine(k, mbw, None)[2]
+            _, last_bw, st = refine_handle.refine(k, mbw, None)
+            return st
         return handle.cluster(mcw, fetch=False)[1]
 
     def barrier():
@@ -431,6 +468,11 @@ def main():
         last = st
     barrier()
     sampler.mark_end()
+    if args.dump_outputs and rank == 0:
+        if refine_handle is not None:
+            dump_outputs(args.dump_outputs, {"partition": refine_handle.download_labels(), "block_weights": last_bw})
+        else:
+            dump_outputs(args.dump_outputs, {"clustering": handle.download_labels()})
     # ---- breakdown steps (outside the timed region): per-tier CUDA events, tiers serialised ----------------
     BSTEPS = 2
     (refine_handle or handle).set_timing(True)
@@ -528,15 +570,9 @@ def main():
     b_edges, b_nodes = sum(g_edges), sum(g_nodes)
     all_bytes = 8 * b_edges + 16 * b_nodes
     sweep_ms_total = sum(g_ms)
-    traffic = None
-    try:  # DRAM bytes per launch of this kernel from the committed ncu capture (profiles/), if any
-        with open(os.path.join(ROOT, "profiles", "r2_traffic.json")) as f:
-            traffic = json.load(f).get(wl, {}).get(names[dom], {}).get("traffic_bytes_per_launch")
-    except Exception:
-        traffic = None
     roofline = {
         "bound": "hbm", "kernel": names[dom], "achieved": achieved, "peak": peak, "unit": "GB/s",
-        "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src,
+        "frac": achieved / peak, "traffic": None, "peak_source": peak_src,
         "launches": g_launch[dom], "avg_launch_ms": g_ms[dom] / max(g_launch[dom], 1),
         "algorithmic_bytes_per_launch": alg_bytes / max(g_launch[dom], 1),
         "share_of_step": g_ms[dom] / brk_ms if brk_ms > 0 else None,
@@ -549,10 +585,11 @@ def main():
         "commit_ms": commit_ms / BSTEPS, "apply_ms": apply_ms / BSTEPS, "push_activate_ms": push_ms / BSTEPS,
         "pull_rounds_per_step": pull_rounds / args.steps, "push_rounds_per_step": push_rounds / args.steps,
         "gather_bound": {
-            # scripts/microbench_lsu.cu on this pool's B200: random 4-byte gathers from an L2-resident table
-            # (one per scanned edge is the floor of any LP sweep on a graph without locality) run at 272 G/s
-            "l2_gather_per_s": 272e9,
-            "all_sweeps_frac_of_gather_bound": (b_edges / (sweep_ms_total * 1e-3) / 272e9) if sweep_ms_total > 0 else None,
+            # scripts/microbench_lsu.cu on an H100 SXM (80 GB HBM3, 400 W power limit): random 4-byte gathers from an
+            # L2-resident table (one per scanned edge is the floor of any LP sweep on a graph without locality) run at
+            # 128.6 G/s
+            "l2_gather_per_s": L2_GATHER_PER_S,
+            "all_sweeps_frac_of_gather_bound": (b_edges / (sweep_ms_total * 1e-3) / L2_GATHER_PER_S) if sweep_ms_total > 0 else None,
         },
     }
 
@@ -570,7 +607,7 @@ def main():
         "config": {"workload": wl, "n": n, "m_directed": m, "k": k, "mode": args.mode,
                    "max_cluster_weight": mcw,
                    "iterations": last.iterations, "moved": last.moved_list(),
-                   "num_clusters": last.num_clusters, "l2": "inputs_larger_than_l2" if m * 4 > 126e6 else "small_input",
+                   "num_clusters": last.num_clusters, "l2": "inputs_larger_than_l2" if m * 4 > L2_BYTES else "small_input",
                    "parallelism": "single" if world == 1 else f"frontier-sharded x{world} (replicated labels; ncclAllGather of the proposal buffers per sub-round inside the library)",
                    "subrounds": ctx.engine.sync_subrounds},
         "clocks": clocks,

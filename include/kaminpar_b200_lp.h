@@ -1,4 +1,4 @@
-/* kaminpar_b200 -- C ABI of the B200-native label-propagation engine.
+/* kaminpar_b200 -- C ABI of the CUDA label-propagation engine (H100, sm_90a).
  *
  * This is the drop-in boundary (SURVEY.md §8b). The reference has no FFI below its C++ plugin
  * interfaces; the entry points here are what a binding for those interfaces would call:

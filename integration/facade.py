@@ -2,7 +2,7 @@
 
 This is NOT a re-implementation of the multilevel partitioner. It drives the UNMODIFIED reference partitioner
 (coarsening loop, contraction, initial partitioning, balancers) compiled by `make -C oracle ref_b200` with the
-B200 label-propagation clusterer / refiner swapped in behind `factories.cc` (integration/, INTEGRATION.md §2).
+GPU label-propagation clusterer / refiner swapped in behind `factories.cc` (integration/, INTEGRATION.md §2).
 The library only exists where the reference sources were available at build time; without it the constructor
 fails loudly -- there is no fallback partitioner.
 
@@ -32,7 +32,7 @@ class KaMinPar:
     def __init__(self, num_threads: int = 1):
         if not os.path.exists(_LIB_B200):
             raise RuntimeError(f"{_LIB_B200} is missing: build it with `make -C oracle ref_b200` where the KaMinPar "
-                               "sources are available (it is the reference partitioner with the B200 LP plugged in)")
+                               "sources are available (it is the reference partitioner with the GPU LP plugged in)")
         self._lib = C.CDLL(_LIB_B200)
         self._lib.kmpfull_compute_partition.restype = C.c_longlong
         self._threads = int(num_threads)

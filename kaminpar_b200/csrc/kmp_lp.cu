@@ -1,4 +1,4 @@
-// kaminpar_b200: host side of the B200-native label-propagation engine + its C ABI
+// kaminpar_b200: host side of the CUDA label-propagation engine (H100, sm_90a) + its C ABI
 // (include/kaminpar_b200_lp.h). One handle = one CUDA stream on one device; everything between
 // the H2D copy of the inputs and the D2H copy of the result runs on the device.
 //
@@ -58,7 +58,7 @@ constexpr int kStatTiers = 12; // tier slots of kmp_lp_stats / ctr64 (edges at [
 constexpr int kCtrNodes = 16, kCtrScratch = 40, kCtrSize = 48;
 constexpr uint32_t kHubMinDegree = 8192;       // graphs with edge weights (32-bit ratings in the team tables)
 constexpr uint32_t kHubMinDegreeUnit = 16384;  // unit edge weights: 16-bit ratings, twice the slots
-constexpr int kSMs = 148;
+constexpr int kSMs = 132; // H100 SXM: caps the grid-stride launches at a few waves of the device
 constexpr uint32_t kMaxHubWaves = 448; // work-queue cursors ctr32[64 .. 512), overflow counters ctr32[512 .. 960)
 constexpr uint32_t kCtr32Size = 1024;
 constexpr int kTagCommit = 12, kTagApply = 13, kTagPush = 14, kTagMisc = 15; // timing slots besides the tiers
@@ -266,8 +266,8 @@ struct GroupSubrounds {
 __global__ void k_list_keys(uint32_t n, const uint32_t *xadj, uint32_t S, GroupSubrounds gs, uint32_t granule_log2,
                             uint32_t base_sr, uint32_t large_degree_threshold, uint32_t hub_min, uint8_t *keys,
                             uint32_t *vals, uint32_t *hist, uint32_t *max_deg) {
-  // list-size histogram privatised per CTA: n global atomics on < 64 addresses serialise in L2 (measured 0.87 ms
-  // for n = 2.4 M in round 1, i.e. ~50 ms for the 512^3 grid)
+  // list-size histogram privatised per CTA: n global atomics on < 64 addresses serialise in L2
+  // (the cost grows with n: the 512^3 grid has 1.3e8 vertices)
   __shared__ uint32_t s_hist[256];
   s_hist[threadIdx.x & 255] = 0;
   __syncthreads();
@@ -650,7 +650,7 @@ template <int MODE, bool EW, bool P64> cudaError_t launch_sweep_t(kmp_lp_handle 
       launch_team<MODE, EW, P64, 32, 512, 8>(h, a, 7);
     }
     break;
-  case 3: // deg 32..255: one warp per vertex, 512 slots (a 64-register sort was measured: 1.5-2x slower here)
+  case 3: // deg 32..255: one warp per vertex, 512 slots (a 64-register sort was slower here: 230 registers, one CTA per SM)
     launch_team<MODE, EW, P64, 32, 512, 8>(h, a, 7);
     break;
   case 4: // deg < 1024: 128 threads per vertex, 2048 slots
@@ -974,8 +974,7 @@ int ensure_lists(kmp_lp_handle *h) {
   h->lists_valid = true;
   // the sort buffers are only needed here
   // The sort buffers stay allocated (grow-only, released by kmp_lp_free_scratch): a cudaFree / cudaMalloc pair per
-  // set_graph synchronises the whole device and cost 8-12 ms per call on the bench box -- up to 0.6 s on another --
-  // while the graph upload was in flight (scripts/e2e_probe.py).
+  // set_graph synchronises the whole device, and waits for the graph upload in flight (scripts/e2e_probe.py).
   tc.lap("lists: done");
   return KMP_OK;
 }

@@ -273,8 +273,7 @@ __global__ void commit_refine_jmin(const CommitArgs a) {
   a.jmin[b] = jm;
 }
 // Block-weight style accumulators are privatised per CTA in shared memory when k is small: millions of
-// proposals hitting k <= a few hundred global addresses serialise in the L2 atomic units (measured:
-// 783 us per launch for 0.7 M moves on k = 64 before, see profiles/README.md).
+// proposals hitting k <= a few hundred global addresses serialise in the L2 atomic units.
 constexpr uint32_t kSmemPrivLimit = 8192; // ints of dynamic shared memory a commit kernel may use
 
 __global__ void commit_refine_decide(const CommitArgs a) {

@@ -64,7 +64,7 @@ __device__ __forceinline__ typename LabG<P64>::word load_labg(const SweepArgs &a
 // (fully unrolled: 19 / 63 / 191 compare-exchanges of two instructions each, no divergence -- empty slots
 // hold 0xFFFFFFFF and sort to the end), and the ratings are the run lengths of the sorted sequence. Per vertex this
 // costs a few hundred to ~1500 thread instructions (20-50 per edge) where a warp-wide hash-map kernel spends
-// ~250 per edge (N = 64 was measured too: 230 registers, 1.5-2x slower than the warp kernel on deg 32..64), and consecutive list entries have consecutive adjacency rows, so the per-thread row reads share
+// ~250 per edge (N = 64 was tried too: 230 registers, slower than the warp kernel on deg 32..64), and consecutive list entries have consecutive adjacency rows, so the per-thread row reads share
 // sectors across the warp.
 // ================================================================================================
 template <int MODE, bool EW, bool P64, int N> __global__ void __launch_bounds__(256) sweep_thread(const SweepArgs a) {

@@ -90,7 +90,7 @@ def load_library():
         if not os.path.exists(_LIB_PATH):
             raise RuntimeError(
                 f"{_LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a). kaminpar_b200 has no CPU fallback."
+                "(nvcc, sm_90a). kaminpar_b200 has no CPU fallback."
             )
         lib = C.CDLL(_LIB_PATH)
         lib.kmp_last_error.restype = C.c_char_p
@@ -138,7 +138,7 @@ class LabelPropagationRefinementContext:  # kaminpar.h:221-228, defaults presets
 
 @dataclass
 class EngineContext:
-    """Knobs of the B200 engine that have no reference counterpart (DESIGN.md "sync schedule")."""
+    """Knobs of the GPU engine that have no reference counterpart (DESIGN.md "sync schedule")."""
 
     seed: int = 0
     sync_subrounds: int = 8

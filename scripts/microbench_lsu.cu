@@ -4,10 +4,12 @@
 //   smem_cas_add      : per edge one atomicCAS + one atomicAdd on a shared-memory hash table
 //   smem_plain        : per edge plain ld/st claims on a shared-memory table (optimistic insertion)
 //   redg / atomg      : per edge one RED / one ATOM.EXCH on a random word of an L2-resident table
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -o microbench_lsu microbench_lsu.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -o microbench_lsu microbench_lsu.cu
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>
+
+constexpr int kSMs = 132; // H100 SXM
 
 #define CK(x)                                                                                              \
   do {                                                                                                     \
@@ -275,11 +277,11 @@ int main() {
   unsigned long long *out;
   CK(cudaMalloc(&adj, m * 4));
   CK(cudaMalloc(&out, 64));
-  k_fill_adj<<<148 * 8, 256>>>(adj, m, 1u << 31);
+  k_fill_adj<<<kSMs * 8, 256>>>(adj, m, 1u << 31);
   CK(cudaDeviceSynchronize());
   printf("{\"m\": %llu", (unsigned long long)m);
   {
-    const float ms = time_ms([&] { k_stream<8><<<148 * 8, 256>>>(adj, m, out); }, 5);
+    const float ms = time_ms([&] { k_stream<8><<<kSMs * 8, 256>>>(adj, m, out); }, 5);
     printf(", \"stream_Gedges_s\": %.1f", m / ms * 1e-6);
   }
   for (uint32_t n : {2400000u, 9000000u, 64000000u}) {
@@ -287,52 +289,52 @@ int main() {
     unsigned long long *t8;
     CK(cudaMalloc(&t4, (size_t)n * 4));
     CK(cudaMalloc(&t8, (size_t)n * 8));
-    k_fill_adj<<<148 * 8, 256>>>(adj, m, n);
-    k_fill_tab<<<148 * 8, 256>>>(t4, n);
-    k_fill_tab<<<148 * 8, 256>>>(t8, n);
+    k_fill_adj<<<kSMs * 8, 256>>>(adj, m, n);
+    k_fill_tab<<<kSMs * 8, 256>>>(t4, n);
+    k_fill_tab<<<kSMs * 8, 256>>>(t8, n);
     CK(cudaDeviceSynchronize());
-    float ms = time_ms([&] { k_gather<uint32_t, 8><<<148 * 8, 256>>>(adj, t4, m, out); }, 5);
+    float ms = time_ms([&] { k_gather<uint32_t, 8><<<kSMs * 8, 256>>>(adj, t4, m, out); }, 5);
     printf(", \"gather4_n%u_G_s\": %.1f", n, m / ms * 1e-6);
-    ms = time_ms([&] { k_gather<unsigned long long, 8><<<148 * 8, 256>>>(adj, t8, m, out); }, 5);
+    ms = time_ms([&] { k_gather<unsigned long long, 8><<<kSMs * 8, 256>>>(adj, t8, m, out); }, 5);
     printf(", \"gather8_n%u_G_s\": %.1f", n, m / ms * 1e-6);
-    ms = time_ms([&] { k_gather<uint32_t, 4><<<148 * 16, 256>>>(adj, t4, m, out); }, 5);
+    ms = time_ms([&] { k_gather<uint32_t, 4><<<kSMs * 16, 256>>>(adj, t4, m, out); }, 5);
     printf(", \"gather4_b4_n%u_G_s\": %.1f", n, m / ms * 1e-6);
-    ms = time_ms([&] { k_gather<uint32_t, 16><<<148 * 4, 256>>>(adj, t4, m, out); }, 5);
+    ms = time_ms([&] { k_gather<uint32_t, 16><<<kSMs * 4, 256>>>(adj, t4, m, out); }, 5);
     printf(", \"gather4_b16_n%u_G_s\": %.1f", n, m / ms * 1e-6);
     if (n == 2400000u) {
-      ms = time_ms([&] { k_gatom<8, false><<<148 * 8, 256>>>(adj, (int *)t4, m, out); }, 3);
+      ms = time_ms([&] { k_gatom<8, false><<<kSMs * 8, 256>>>(adj, (int *)t4, m, out); }, 3);
       printf(", \"redg_G_s\": %.1f", m / ms * 1e-6);
-      ms = time_ms([&] { k_gatom<8, true><<<148 * 8, 256>>>(adj, (int *)t4, m, out); }, 3);
+      ms = time_ms([&] { k_gatom<8, true><<<kSMs * 8, 256>>>(adj, (int *)t4, m, out); }, 3);
       printf(", \"atomg_exch_G_s\": %.1f", m / ms * 1e-6);
     }
     cudaFree(t4);
     cudaFree(t8);
   }
   // shared-memory aggregation: labels drawn from 2^22 values (mostly distinct within 8192)
-  k_fill_adj<<<148 * 8, 256>>>(adj, m, 1u << 22);
+  k_fill_adj<<<kSMs * 8, 256>>>(adj, m, 1u << 22);
   CK(cudaDeviceSynchronize());
   {
     constexpr int T = 512, EPT = 16, C = 16384;
     const size_t smem = C * 8;
     CK(cudaFuncSetAttribute(k_smem_cas_add<T, EPT, C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    float ms = time_ms([&] { k_smem_cas_add<T, EPT, C><<<148 * 1, T, smem>>>(adj, m, out); }, 3);
+    float ms = time_ms([&] { k_smem_cas_add<T, EPT, C><<<kSMs * 1, T, smem>>>(adj, m, out); }, 3);
     printf(", \"smem_cas_add_1cta_G_s\": %.1f", m / ms * 1e-6);
-    ms = time_ms([&] { k_smem_cas_add<T, EPT, C><<<148 * 2, T, smem>>>(adj, m, out); }, 3);
+    ms = time_ms([&] { k_smem_cas_add<T, EPT, C><<<kSMs * 2, T, smem>>>(adj, m, out); }, 3);
     printf(", \"smem_cas_add_2cta_G_s\": %.1f", m / ms * 1e-6);
     const size_t smem2 = (C + 2 * T * EPT) * 4;
     CK(cudaFuncSetAttribute(k_smem_plain<T, EPT, C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
-    ms = time_ms([&] { k_smem_plain<T, EPT, C><<<148 * 1, T, smem2>>>(adj, m, out); }, 3);
+    ms = time_ms([&] { k_smem_plain<T, EPT, C><<<kSMs * 1, T, smem2>>>(adj, m, out); }, 3);
     printf(", \"smem_plain_1cta_G_s\": %.1f", m / ms * 1e-6);
-    ms = time_ms([&] { k_smem_plain<T, EPT, C><<<148 * 2, T, smem2>>>(adj, m, out); }, 3);
+    ms = time_ms([&] { k_smem_plain<T, EPT, C><<<kSMs * 2, T, smem2>>>(adj, m, out); }, 3);
     printf(", \"smem_plain_2cta_G_s\": %.1f", m / ms * 1e-6);
   }
   {
     constexpr int T = 128, EPT = 8, C = 2048;
     const size_t smem = C * 8;
-    float ms = time_ms([&] { k_smem_cas_add<T, EPT, C><<<148 * 8, T, smem>>>(adj, m, out); }, 3);
+    float ms = time_ms([&] { k_smem_cas_add<T, EPT, C><<<kSMs * 8, T, smem>>>(adj, m, out); }, 3);
     printf(", \"smem_cas_add_t128_G_s\": %.1f", m / ms * 1e-6);
     const size_t smem2 = (C + 2 * T * EPT) * 4;
-    ms = time_ms([&] { k_smem_plain<T, EPT, C><<<148 * 8, T, smem2>>>(adj, m, out); }, 3);
+    ms = time_ms([&] { k_smem_plain<T, EPT, C><<<kSMs * 8, T, smem2>>>(adj, m, out); }, 3);
     printf(", \"smem_plain_t128_G_s\": %.1f", m / ms * 1e-6);
   }
   printf("}\n");

@@ -4,10 +4,12 @@ For the graphs and reference LP clusterings already stored in tests/golden/ref_<
 UNMODIFIED reference's contract_clustering returns (default algorithm UNBUFFERED; raw, i.e. with the
 reference's own coarse numbering and adjacency order) -> tests/golden/contract_<case>.npz. The oracle
 (oracle/contraction_oracle.py) must reproduce every one of them after canonicalize()
-(tests/test_contraction_oracle.py); that is what pins it.
+(tests/test_contraction_oracle.py); that is what pins it. For the generated graphs of that test (live_cases,
+multigraph_cases) the digests of the reference's canonical results go to tests/golden/contract_live_digests.json.
 
     python tests/golden/make_contraction_golden.py
 """
+import json
 import os
 import sys
 
@@ -35,6 +37,22 @@ def main():
                             c_n=np.array([r["c_n"]]), c_xadj=r["c_xadj"], c_adjncy=r["c_adjncy"], c_vwgt=r["c_vwgt"],
                             c_adjwgt=r["c_adjwgt"], mapping=r["mapping"])
         print("wrote", name, g.n, g.m, "->", r["c_n"], len(r["c_adjncy"]))
+    write_live_digests()
+
+
+def write_live_digests():
+    from oracle import contraction_oracle as CO
+    from tests import test_contraction_oracle as T
+
+    def ref_digest(g, cl, algorithm):
+        return T.digest(CO.canonicalize(**B.ref_contract(g, cl, algorithm), clustering=cl))
+
+    assert B.have_reference(), "build oracle/_ref first: make -C oracle ref"
+    live = {"algorithm": {str(a): [ref_digest(g, cl, a) for g, cl in T.live_cases(a)] for a in (0, 1, 2)},
+            "multigraphs": [ref_digest(g, cl, 1) for g, cl in T.multigraph_cases()]}
+    with open(os.path.join(OUT, "contract_live_digests.json"), "w") as f:
+        json.dump(live, f, indent=1)
+    print("wrote contract_live_digests.json")
 
 
 if __name__ == "__main__":

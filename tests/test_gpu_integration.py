@@ -1,5 +1,5 @@
 """-m gpu: the drop-in claim, compiled and run. oracle/_ref/libkaminpar_ref_b200.so is the UNMODIFIED reference
-partitioner (every kaminpar-shm / kaminpar-common translation unit) whose factories.cc returns the B200 glue
+partitioner (every kaminpar-shm / kaminpar-common translation unit) whose factories.cc returns the GPU glue
 classes for the two LABEL_PROPAGATION cases (integration/, INTEGRATION.md §2; `make -C oracle ref_b200`), linked
 against libkaminpar_b200.so. KaMinPar::compute_partition then coarsens with the GPU LP clusterer and refines with
 the GPU LP refiner on every level, everything else (contraction, initial partitioning, balancers) is the reference.
@@ -57,7 +57,7 @@ def test_compute_partition_through_swapped_factories(name, k, cut_bound):
     cut3, p3 = partition(lib, g, k, seed=1)
     assert not np.array_equal(p, p3)                             # :219-247 different seed, different partition
     ref_cut, _ = partition(_load(LIB_FULL), g, k)
-    print(f"{name} k={k}: cut with the B200 LP {cut}, pure reference {ref_cut}")
+    print(f"{name} k={k}: cut with the GPU LP {cut}, pure reference {ref_cut}")
     assert cut <= 1.25 * ref_cut + 16
 
 

@@ -89,8 +89,6 @@ def test_t0_cluster_selection(name):
 @pytest.mark.parametrize("k", [2, 16, 600])
 def test_t0_refine_selection(name, k):
     g = get_graph(name)
-    if k > max(2, g.n // 2):
-        pytest.skip("k too large for this graph")
     ctx, _ = ctx_for(g, k, seed=11)
     h = lp.LPHandle(lp._refine_config(ctx.refinement.lp, ctx.engine))
     h.set_graph(g)
@@ -239,8 +237,6 @@ def test_t1_long_refinement_switches_to_push_activation(name):
 @pytest.mark.parametrize("k", [2, 4, 64])
 def test_t1_refinement_matches_oracle_sync(name, k):
     g = get_graph(name)
-    if k > max(2, g.n // 4):
-        pytest.skip("k too large for this graph")
     ctx, _ = ctx_for(g, k, seed=2)
     rng = np.random.default_rng(7)
     part = rng.integers(0, k, g.n).astype(np.uint32)

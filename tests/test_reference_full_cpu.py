@@ -1,6 +1,6 @@
 """CPU: the whole UNMODIFIED reference partitioner (oracle/_ref/libkaminpar_ref_full.so: every kaminpar-shm /
 kaminpar-common translation unit on the serial oneTBB stand-in, `make -C oracle ref_full`) through the same C entry
-point the B200-integrated build exports (integration/partition_driver.cc). Pins the harness of
+point the GPU-integrated build exports (integration/partition_driver.cc). Pins the harness of
 tests/test_gpu_integration.py against the reference's own end-to-end properties
 (tests/endtoend/shm_endtoend_test.cc:142-247)."""
 import ctypes as C
