@@ -68,6 +68,8 @@ int kmp_coarse_project_up(const kmp_coarse_graph *g, const uint32_t *coarse, uin
 /* CoarseGraph::project_down: coarse[mapping[u]] = fine[u] (any member's value when they differ). */
 int kmp_coarse_project_down(const kmp_coarse_graph *g, const uint32_t *fine, uint32_t *coarse);
 
+/* Frees the arrays stream-ordered on the stream of the handle that contracted the graph: call it before
+ * kmp_lp_destroy of that handle. */
 void kmp_coarse_destroy(kmp_coarse_graph *g);
 
 #ifdef __cplusplus

@@ -76,7 +76,8 @@ typedef struct {
   int32_t seed;                /* Random::reseed() analogue; enters every hash key */
   uint32_t sync_subrounds;     /* S: hashed sub-rounds per degree group and iteration (8) */
   uint32_t sync_granule_log2;  /* vertices u >> g share a sub-round (4) */
-  uint32_t sync_commit_passes; /* commit passes crediting departures: 1 clusterer, 4 refiner */
+  uint32_t sync_commit_passes; /* commit passes crediting departures: 1 clusterer, 4 refiner. The clusterer's
+                                  commit is single-pass: kmp_lp_cluster refuses > 1 with KMP_ERR_UNSUPPORTED */
   int32_t device;              /* CUDA device ordinal, -1 = current */
   int32_t schedule;            /* KMP_SCHEDULE_SYNC (default) or KMP_SCHEDULE_SEQ_STRICT */
 } kmp_lp_config;
@@ -137,7 +138,10 @@ int kmp_lp_destroy(kmp_lp_handle *h);
 int kmp_lp_set_graph(kmp_lp_handle *h, uint32_t n, uint32_t m, const uint32_t *xadj,
                      const uint32_t *adjncy, const int32_t *vwgt, const int32_t *adjwgt);
 /* Same, but the arrays already live in device memory of the handle's device and stay owned by the
- * caller (must outlive their use by the handle). */
+ * caller (must outlive their use by the handle). Every pointer must be 4-byte aligned (KMP_ERR_INVALID
+ * otherwise); views into a larger allocation are fine. When d_adjncy is also 16-byte aligned the
+ * high-degree tier stages adjacency chunks into shared memory with bulk copies; otherwise it reads them
+ * from global memory (same results, somewhat slower on hubs). */
 int kmp_lp_set_graph_device(kmp_lp_handle *h, uint32_t n, uint32_t m, const uint32_t *d_xadj,
                             const uint32_t *d_adjncy, const int32_t *d_vwgt, const int32_t *d_adjwgt);
 

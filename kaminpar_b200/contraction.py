@@ -61,6 +61,8 @@ class CoarseGraph:
         self._g = handle_ptr
         self.stats = stats
         self._keepalive = keepalive  # the LPHandle whose graph was contracted (owns the stream)
+        if keepalive is not None:
+            keepalive._children += 1  # the handle is destroyed after this graph (see close)
         self._host: Optional[CSRGraph] = None
         self._mapping: Optional[np.ndarray] = None
 
@@ -117,8 +119,13 @@ class CoarseGraph:
 
     def close(self):
         if getattr(self, "_g", None):
-            _lib().kmp_coarse_destroy(self._g)
+            _lib().kmp_coarse_destroy(self._g)  # frees on the handle's stream: the handle must still exist
             self._g = None
+            k = self._keepalive
+            if k is not None:
+                k._children -= 1
+                if k._close_pending and k._children == 0:
+                    k.close()
 
     def __del__(self):
         try:

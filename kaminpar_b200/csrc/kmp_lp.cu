@@ -143,6 +143,7 @@ struct kmp_lp_handle {
   const uint32_t *adjncy = nullptr;
   const int32_t *vwgt = nullptr;
   const int32_t *adjwgt = nullptr;
+  bool adjncy_16b = true; // adjncy starts on a 16-byte boundary: the hub tier may stage it with bulk copies
   DevBuf<uint32_t> own_xadj, own_adjncy;
   DevBuf<int32_t> own_vwgt, own_adjwgt;
   bool have_graph = false;
@@ -678,6 +679,7 @@ template <int MODE, bool EW, bool P64> cudaError_t launch_sweep_t(kmp_lp_handle 
     hb.ovf_cap = static_cast<uint32_t>(std::min<uint64_t>(h->t4_max_wave_edges, 0xFFFFFFFFull));
     hb.bucket_cap = h->hub_bucket_cap;
     hb.sel_limit = h->hub_sel_limit;
+    hb.stage_adjncy = h->adjncy_16b ? 1u : 0u;
     hb.rank = h->rank;
     hb.world = h->world;
     hb.sel_begin = h->t4_sel_begin.p + first;
@@ -2133,6 +2135,7 @@ int kmp_lp_set_graph(kmp_lp_handle *h, uint32_t n, uint32_t m, const uint32_t *x
   }
   h->xadj = h->own_xadj.p;
   h->adjncy = h->own_adjncy.p;
+  h->adjncy_16b = true; // cudaMalloc: 256-byte aligned
   h->vwgt = nullptr;
   h->adjwgt = nullptr;
   if (vwgt != nullptr) {
@@ -2156,9 +2159,15 @@ int kmp_lp_set_graph_device(kmp_lp_handle *h, uint32_t n, uint32_t m, const uint
   if (h == nullptr || d_xadj == nullptr || (m > 0 && d_adjncy == nullptr)) {
     return fail(KMP_ERR_INVALID, "null argument");
   }
+  auto misaligned4 = [](const void *p) { return (reinterpret_cast<uintptr_t>(p) & 3u) != 0; };
+  if (misaligned4(d_xadj) || misaligned4(d_adjncy) || misaligned4(d_vwgt) || misaligned4(d_adjwgt)) {
+    return fail(KMP_ERR_INVALID, "device graph arrays must be 4-byte aligned");
+  }
   KMP_CUDA(cudaSetDevice(h->device));
   h->xadj = d_xadj;
   h->adjncy = d_adjncy;
+  // a view into a larger buffer may start anywhere: the hub tier then reads adjncy from global memory
+  h->adjncy_16b = (reinterpret_cast<uintptr_t>(d_adjncy) & 15u) == 0;
   h->vwgt = d_vwgt;
   h->adjwgt = d_adjwgt;
   return set_graph_common(h, n, m);
@@ -2180,6 +2189,9 @@ int kmp_lp_cluster(kmp_lp_handle *h, int32_t max_cluster_weight, uint32_t desire
   }
   if (h->cfg.schedule == KMP_SCHEDULE_SEQ_STRICT) {
     return strict_cluster(h, max_cluster_weight, desired_num_clusters, communities, clustering_out, stats);
+  }
+  if (h->cfg.sync_commit_passes > 1) { // the cluster commit kernels decide in one pass: no departure credit
+    return fail(KMP_ERR_UNSUPPORTED, "the clusterer's sync commit is single-pass (sync_commit_passes must be 1)");
   }
   if (h->world > 1 && h->comm == nullptr) {
     return fail(KMP_ERR_INVALID, "sharded handle without a communicator: call kmp_lp_dist_init (or drive the "

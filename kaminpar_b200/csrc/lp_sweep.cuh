@@ -605,6 +605,7 @@ struct HubArgs {
   uint32_t ovf_cap;
   uint32_t bucket_cap;                     // entries a region takes (kBucketCap; smaller only in tests: KMP_HUB_BUCKET_CAP)
   uint32_t sel_limit;                      // 0, or a smaller claim limit of the select map (tests: KMP_HUB_SEL_LIMIT)
+  uint32_t stage_adjncy;                   // adjncy is 16-byte aligned: chunks are staged with bulk copies
   // select: one item per (list entry, bucket)
   const uint32_t *__restrict__ sel_entry;
   const uint32_t *__restrict__ sel_piece;
@@ -665,7 +666,8 @@ struct HubItem {
   uint32_t full_deg;
   uint32_t gbeg, gend; // edge range of the chunk (indices into adjncy)
   uint32_t a0;         // first staged element (gbeg rounded down to a 16-byte boundary)
-  uint32_t staged;     // number of staged elements (multiple of 4), may stop short of gend at the array end
+  uint32_t staged;     // number of staged elements (multiple of 4), may stop short of gend at the array end;
+                       // 0 when adjncy itself is not 16-byte aligned
 };
 
 __device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
@@ -754,12 +756,15 @@ __global__ void __launch_bounds__(kHubThreads, 4) sweep_hub_scatter(const SweepA
             d.gbeg = beg0 + cbeg;
             d.gend = beg0 + cend;
             d.a0 = d.gbeg & ~3u;
-            uint32_t a1 = (d.gend + 3u) & ~3u;
-            const uint32_t m4 = m_total & ~3u; // last 16-byte block that lies fully inside adjncy
-            if (a1 > m4) {
-              a1 = m4;
+            d.staged = 0;
+            if (hb.stage_adjncy) { // cp.async.bulk needs a 16-byte aligned source; else the consumers read adjncy
+              uint32_t a1 = (d.gend + 3u) & ~3u;
+              const uint32_t m4 = m_total & ~3u; // last 16-byte block that lies fully inside adjncy
+              if (a1 > m4) {
+                a1 = m4;
+              }
+              d.staged = a1 > d.a0 ? a1 - d.a0 : 0;
             }
-            d.staged = a1 > d.a0 ? a1 - d.a0 : 0;
           }
         }
         s_item[stage] = d;

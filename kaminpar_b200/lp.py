@@ -303,10 +303,18 @@ class LPHandle:
     def __init__(self, cfg: KmpConfig):
         self._lib = load_library()
         self._h = C.c_void_p()
+        # coarse graphs contracted on this handle free their arrays on its stream (kmp_coarse_destroy): while any
+        # is open, close() is deferred to the last one's close -- also when the garbage collector finalises a
+        # reference cycle holding both in arbitrary order
+        self._children = 0
+        self._close_pending = False
         _check(self._lib.kmp_lp_create(C.byref(cfg), C.byref(self._h)))
         self._graph_id = None
 
     def close(self):
+        if getattr(self, "_children", 0) > 0:
+            self._close_pending = True
+            return
         if getattr(self, "_h", None) is not None and self._h:
             self._lib.kmp_lp_destroy(self._h)
             self._h = None

@@ -341,17 +341,22 @@ def oracle_max_block_weights(g, k, eps=0.03) -> np.ndarray:
 
 
 def oracle_sync_select_all(mode, g, labels, weights, max_weights=None, max_cluster_weight=0, min_weights=None,
-                           seed=0, call=0, iteration=0):
+                           seed=0, call=0, iteration=0, params=None):
+    """params (LPParams / OracleParams, optional): its max_num_neighbors and large_degree_threshold apply as in a
+    full call -- a vertex of degree >= the threshold keeps its label and stores no favored cluster."""
     labels = np.ascontiguousarray(labels, np.uint32)
     weights = np.ascontiguousarray(weights, np.int32)
     tgt = np.zeros(g.n, np.uint32)
     fav = np.zeros(g.n, np.uint32)
+    if params is not None and not isinstance(params, OracleParams):
+        params = oracle_params(params)
     oracle().lpo_sync_select_all(
         C.c_int(mode), C.c_uint32(g.n), g.xadj.ctypes.data_as(C.c_void_p), g.adjncy.ctypes.data_as(C.c_void_p),
         _opt(g.vwgt, np.int32), _opt(g.adjwgt, np.int32), labels.ctypes.data_as(C.c_void_p),
         weights.ctypes.data_as(C.c_void_p), C.c_uint32(len(weights)), _opt(max_weights, np.int32),
         C.c_int32(max_cluster_weight), _opt(min_weights, np.int32), C.c_int(seed), C.c_uint32(call),
-        C.c_uint32(iteration), tgt.ctypes.data_as(C.c_void_p), fav.ctypes.data_as(C.c_void_p))
+        C.c_uint32(iteration), tgt.ctypes.data_as(C.c_void_p), fav.ctypes.data_as(C.c_void_p),
+        None if params is None else C.byref(params))
     return tgt, fav
 
 

@@ -98,13 +98,15 @@ int lpo_lp_refine(int schedule, uint32_t n, uint32_t m, const uint32_t *xadj, co
 /* ---- T0: per-vertex decision on frozen state (sync rules), for unit parity tests ---------- */
 /* For every vertex u (regardless of active flags) compute the target the sync selection rule picks
  * against the given frozen labels / weights: out_target[u] (== label[u] if it stays) and, for the
- * clusterer (mode 0), out_favored[u]. mode 1 = refiner (weights = block weights, max = per block). */
+ * clusterer (mode 0), out_favored[u]. mode 1 = refiner (weights = block weights, max = per block).
+ * params (nullable): max_num_neighbors caps the scanned prefix of every adjacency, and a vertex of degree
+ * >= large_degree_threshold is not visited (out_target[u] = label[u], out_favored[u] = UINT32_MAX). */
 int lpo_sync_select_all(int mode, uint32_t n, const uint32_t *xadj, const uint32_t *adjncy,
                         const int32_t *vwgt, const int32_t *adjwgt, const uint32_t *labels,
                         const int32_t *weights, uint32_t num_labels, const int32_t *max_weights,
                         int32_t max_cluster_weight, const int32_t *min_weights, int seed,
                         uint32_t call_index, uint32_t iteration, uint32_t *out_target,
-                        uint32_t *out_favored);
+                        uint32_t *out_favored, const lpo_params *params /*nullable*/);
 
 /* ---- bridge: the reference-pinned `seq` selection code (ClusterPolicy / RefinePolicy::select_best_cluster,
  * the code checked bit-for-bit against the unmodified reference) on the same frozen state. Outputs the

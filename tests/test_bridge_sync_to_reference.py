@@ -15,7 +15,8 @@ import numpy as np
 import pytest
 
 from oracle import bindings as B
-from tests.helpers import golden_cases, load_case
+from tests.helpers import (LABEL_PATTERNS, LADDER_DEGREES, degree_ladder, frozen_cluster_state, frozen_refine_state,
+                           golden_cases, load_case)
 
 
 def cluster_states(g, mcw):
@@ -32,6 +33,29 @@ def cluster_states(g, mcw):
         yield f"sync{rounds}", labels, cw
 
 
+def assert_sync_in_reference_ties(g, mode, labels, weights, max_cluster_weight=0, max_weights=None, min_weights=None,
+                                  seed=1, iteration=0, tag=()):
+    """On one frozen state (graph, labels, weights, limits): the sync rule's target is a member of the reference's
+    tie set and equals the reference's choice where that set is a singleton (or empty); the same for the favored
+    cluster of the clusterer. Returns (vertices checked, vertices with a unique answer)."""
+    lim = dict(max_cluster_weight=max_cluster_weight) if mode == 0 else dict(max_weights=max_weights,
+                                                                             min_weights=min_weights)
+    tgt, fav = B.oracle_sync_select_all(mode, g, labels, weights, seed=seed, iteration=iteration, **lim)
+    fav_chk = np.where(fav == 0xFFFFFFFF, labels, fav).astype(np.uint32) if mode == 0 else None
+    r = B.oracle_seq_select_all(mode, g, labels, weights, check_target=tgt, check_favored=fav_chk, **lim)
+    bad = np.nonzero(r["check_in_ties"] == 0)[0]
+    assert bad.size == 0, (tag, bad[:5], tgt[bad[:5]], r["target"][bad[:5]])
+    single = r["num_ties"] <= 1
+    assert np.array_equal(tgt[single], r["target"][single]), tag
+    if mode == 0:
+        # favored: stored for the same vertices, member of the reference's tie set, equal when unique
+        assert np.array_equal(fav == 0xFFFFFFFF, r["favored"] == 0xFFFFFFFF), tag
+        assert (r["check_fav_in_ties"] == 1).all(), tag
+        fs = (r["num_fav_ties"] <= 1) & (fav != 0xFFFFFFFF)
+        assert np.array_equal(fav[fs], r["favored"][fs]), tag
+    return g.n, int(single.sum())
+
+
 @pytest.mark.parametrize("case", golden_cases())
 def test_sync_cluster_selection_is_the_references(case):
     g, d = load_case(case)
@@ -42,21 +66,10 @@ def test_sync_cluster_selection_is_the_references(case):
     checked = singles = 0
     for name, labels, cw in cluster_states(g, mcw):
         for it in (0, 3):
-            tgt, fav = B.oracle_sync_select_all(0, g, labels, cw, max_cluster_weight=mcw, seed=1, call=0, iteration=it)
-            fav_chk = np.where(fav == 0xFFFFFFFF, labels, fav).astype(np.uint32)
-            r = B.oracle_seq_select_all(0, g, labels, cw, max_cluster_weight=mcw, check_target=tgt,
-                                        check_favored=fav_chk)
-            bad = np.nonzero(r["check_in_ties"] == 0)[0]
-            assert bad.size == 0, (case, name, it, bad[:5], tgt[bad[:5]], r["target"][bad[:5]])
-            single = r["num_ties"] <= 1
-            assert np.array_equal(tgt[single], r["target"][single]), (case, name, it)
-            # favored: stored for the same vertices, member of the reference's tie set, equal when unique
-            assert np.array_equal(fav == 0xFFFFFFFF, r["favored"] == 0xFFFFFFFF), (case, name, it)
-            assert (r["check_fav_in_ties"] == 1).all(), (case, name, it)
-            fs = (r["num_fav_ties"] <= 1) & (fav != 0xFFFFFFFF)
-            assert np.array_equal(fav[fs], r["favored"][fs]), (case, name, it)
-            checked += g.n
-            singles += int(single.sum())
+            c, s = assert_sync_in_reference_ties(g, 0, labels, cw, max_cluster_weight=mcw, iteration=it,
+                                                 tag=(case, name, it))
+            checked += c
+            singles += s
     assert checked > 0 and singles > 0
 
 
@@ -80,9 +93,38 @@ def test_sync_refine_selection_is_the_references(case):
         for name, lab in states:
             bw = np.bincount(lab, weights=w, minlength=k).astype(np.int32)
             for min_w in (None, np.full(k, int(bw.min()), np.int32)):
-                tgt, _ = B.oracle_sync_select_all(1, g, lab, bw, max_weights=mbw, min_weights=min_w, seed=2, iteration=1)
-                r = B.oracle_seq_select_all(1, g, lab, bw, max_weights=mbw, min_weights=min_w, check_target=tgt)
-                bad = np.nonzero(r["check_in_ties"] == 0)[0]
-                assert bad.size == 0, (case, k, name, bad[:5], tgt[bad[:5]], r["target"][bad[:5]])
-                single = r["num_ties"] <= 1
-                assert np.array_equal(tgt[single], r["target"][single]), (case, k, name)
+                assert_sync_in_reference_ties(g, 1, lab, bw, max_weights=mbw, min_weights=min_w, seed=2, iteration=1,
+                                              tag=(case, k, name))
+
+
+# ---- the same on the states of the kernel-edge suite (tests/test_gpu_edges.py): degree ladders with labels that
+# are all one, all distinct, exactly tied or hash-colliding, and weights exactly at a limit or one above it
+LADDERS = {
+    "dense_w": (lambda: degree_ladder(sorted(LADDER_DEGREES), 256, weighted=True, multi=True, seed=2), 256),
+    "wide_unit": (lambda: degree_ladder(sorted(LADDER_DEGREES), 18436, seed=3), 18436),
+}
+
+
+@pytest.mark.parametrize("pattern", LABEL_PATTERNS)
+@pytest.mark.parametrize("name", sorted(LADDERS))
+def test_sync_selection_is_the_references_at_the_kernel_edges(name, pattern):
+    make, pool = LADDERS[name]
+    g = make()
+    rng = np.random.default_rng(len(name) * 10 + LABEL_PATTERNS.index(pattern))
+    singles = 0
+    for nl in (513, 32769) if g.n < 512 else (g.n, 1 << 20):
+        for feas in ("lo", "hi", "mix"):
+            labels, weights = frozen_cluster_state(g, pool, nl, pattern, feas, rng)
+            singles += assert_sync_in_reference_ties(g, 0, labels, weights, max_cluster_weight=1000,
+                                                     tag=(name, pattern, nl, feas))[1]
+        cw = 1 if g.vwgt is None else int(g.vwgt[pool])
+        for regime in ("fit", "over"):
+            labels, bw, maxw, own = frozen_refine_state(g, pool, nl, pattern, regime, "mix", rng)
+            for d in (None, 0, 1):
+                mn = None
+                if d is not None:
+                    mn = np.zeros(nl, np.int32)
+                    mn[own] = int(bw[own]) - cw + d
+                singles += assert_sync_in_reference_ties(g, 1, labels, bw, max_weights=maxw, min_weights=mn,
+                                                         tag=(name, pattern, nl, regime, d))[1]
+    assert singles > 0

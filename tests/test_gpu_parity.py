@@ -41,6 +41,9 @@ def graphs():
     out["complete"] = H.complete_graph(40)
     out["bipartite"] = H.complete_bipartite(30, 50)
     out["with_isolated"] = H.from_edges(40, [(i, i + 1) for i in range(0, 20)])
+    # both sides of every kernel-tier boundary; parallel edges keep n below every direct-indexing size (n = 278)
+    out["ladder_dense_w"] = H.degree_ladder(sorted(H.LADDER_DEGREES), 256, weighted=True, multi=True, seed=2)
+    out["ladder_wide"] = H.degree_ladder(sorted(H.LADDER_DEGREES), 18436, seed=3)  # distinct neighbours
     return out
 
 
@@ -56,7 +59,7 @@ def get_graph(name):
 
 NAMES = ["rgg2d_k4", "walshaw_k16", "walshaw_unsorted", "rmat13_w", "grid12", "road60", "star30000", "rmat15_sorted",
          "rmat14_unsorted_w", "rmat16_hubs", "rmat15_hubs_w", "grid20", "rgg_2e15", "star_hub", "path", "complete",
-         "bipartite", "with_isolated"]
+         "bipartite", "with_isolated", "ladder_dense_w", "ladder_wide"]
 
 
 # ------------------------------------------------------------------------------------------------
