@@ -226,6 +226,9 @@ struct kmp_lp_handle {
   int fused_blocks = 0;      // co-resident CTAs of the fused kernel (0: not available)
   int fused_blocks_refine = 0;
   bool fused_commit = true;
+  // resident CTAs of each sweep_team instantiation on the device, [MODE][EW][P64][team size 32 / 128 / 512 / 1024]:
+  // a larger grid only adds CTAs that start after the work queue is drained
+  uint32_t team_grid[2][2][2][4] = {};
   // stepping API state
   int step_mode = -1;
   uint32_t step_iter = 0; // LP round of the stepping API
@@ -610,26 +613,43 @@ inline uint32_t grid_for(uint64_t threads_needed, uint32_t block, uint32_t max_b
   return static_cast<uint32_t>(std::max<uint64_t>(1, std::min<uint64_t>(b, max_blocks)));
 }
 
-template <int MODE, bool EW, bool P64, int T, int SLOTS, int TEAMS, bool V16 = false>
-void launch_team(kmp_lp_handle *h, const SweepArgs &a, int ctas_per_sm) {
-  const size_t smem = static_cast<size_t>(SLOTS) * TEAMS * (V16 ? 6 : 8);
-  const uint32_t want = (a.list_size + TEAMS - 1) / TEAMS;
-  const uint32_t blocks = std::max<uint32_t>(1, std::min<uint32_t>(want, static_cast<uint32_t>(kSMs * ctas_per_sm)));
-  sweep_team<MODE, EW, P64, T, SLOTS, TEAMS, V16><<<blocks, T * TEAMS, smem, h->sweep_stream>>>(a);
+constexpr int team_size_index(int T) { return T == 32 ? 0 : T == 128 ? 1 : T == 512 ? 2 : 3; }
+template <int SLOTS, int TEAMS, bool V16> constexpr size_t team_smem() {
+  return static_cast<size_t>(SLOTS) * TEAMS * (V16 ? 6 : 8);
 }
 
-// dynamic shared memory opt-in of the team kernels (per device; called from kmp_lp_create)
-template <int MODE, bool EW, bool P64> void configure_team_kernels() {
-  cudaFuncSetAttribute(sweep_team<MODE, EW, P64, 32, 512, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 512 * 8 * 8);
-  cudaFuncSetAttribute(sweep_team<MODE, EW, P64, 128, 2048, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2048 * 4 * 8);
-  cudaFuncSetAttribute(sweep_team<MODE, EW, P64, 512, 8192, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 8);
-  cudaFuncSetAttribute(sweep_hub_scatter<MODE, EW, P64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kHubScatterSmem);
-  if constexpr (EW) {
-    cudaFuncSetAttribute(sweep_team<MODE, EW, P64, 1024, 16384, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 8);
-  } else {
-    cudaFuncSetAttribute(sweep_team<MODE, EW, P64, 1024, 32768, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         32768 * 6);
+template <int MODE, bool EW, bool P64, int T, int SLOTS, int TEAMS, bool V16 = false>
+void launch_team(kmp_lp_handle *h, const SweepArgs &a) {
+  const uint32_t want = (a.list_size + TEAMS - 1) / TEAMS;
+  const uint32_t blocks = std::max<uint32_t>(1, std::min<uint32_t>(want, h->team_grid[MODE][EW][P64][team_size_index(T)]));
+  sweep_team<MODE, EW, P64, T, SLOTS, TEAMS, V16><<<blocks, T * TEAMS, team_smem<SLOTS, TEAMS, V16>(), h->sweep_stream>>>(a);
+}
+
+// dynamic shared memory opt-in of one team kernel and its resident grid (CTAs per SM from the occupancy calculator)
+template <int MODE, bool EW, bool P64, int T, int SLOTS, int TEAMS, bool V16 = false>
+bool configure_team(kmp_lp_handle *h, int sms) {
+  const auto kernel = sweep_team<MODE, EW, P64, T, SLOTS, TEAMS, V16>;
+  constexpr size_t smem = team_smem<SLOTS, TEAMS, V16>();
+  int per_sm = 0;
+  if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)) != cudaSuccess ||
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, T * TEAMS, smem) != cudaSuccess || per_sm < 1) {
+    return false;
   }
+  h->team_grid[MODE][EW][P64][team_size_index(T)] = static_cast<uint32_t>(sms * per_sm);
+  return true;
+}
+
+// per device; called from kmp_lp_create
+template <int MODE, bool EW, bool P64> bool configure_team_kernels(kmp_lp_handle *h, int sms) {
+  cudaFuncSetAttribute(sweep_hub_scatter<MODE, EW, P64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kHubScatterSmem);
+  bool ok = configure_team<MODE, EW, P64, 32, 512, 8>(h, sms) && configure_team<MODE, EW, P64, 128, 2048, 4>(h, sms) &&
+            configure_team<MODE, EW, P64, 512, 8192, 1>(h, sms);
+  if constexpr (EW) {
+    ok = ok && configure_team<MODE, EW, P64, 1024, 16384, 1>(h, sms);
+  } else {
+    ok = ok && configure_team<MODE, EW, P64, 1024, 32768, 1, true>(h, sms);
+  }
+  return ok;
 }
 
 template <int MODE, bool EW, bool P64> cudaError_t launch_sweep_t(kmp_lp_handle *h, int tier, const SweepArgs &a) {
@@ -648,23 +668,23 @@ template <int MODE, bool EW, bool P64> cudaError_t launch_sweep_t(kmp_lp_handle 
     if (h->thread_max_deg >= 32) {
       sweep_thread<MODE, EW, P64, 32><<<tgrid, 256, 0, h->sweep_stream>>>(a);
     } else {
-      launch_team<MODE, EW, P64, 32, 512, 8>(h, a, 7);
+      launch_team<MODE, EW, P64, 32, 512, 8>(h, a);
     }
     break;
   case 3: // deg 32..255: one warp per vertex, 512 slots (a 64-register sort was slower here: 230 registers, one CTA per SM)
-    launch_team<MODE, EW, P64, 32, 512, 8>(h, a, 7);
+    launch_team<MODE, EW, P64, 32, 512, 8>(h, a);
     break;
   case 4: // deg < 1024: 128 threads per vertex, 2048 slots
-    launch_team<MODE, EW, P64, 128, 2048, 4>(h, a, 3);
+    launch_team<MODE, EW, P64, 128, 2048, 4>(h, a);
     break;
   case 5: // deg < 4096: 512 threads per vertex, 8192 slots
-    launch_team<MODE, EW, P64, 512, 8192, 1>(h, a, 3);
+    launch_team<MODE, EW, P64, 512, 8192, 1>(h, a);
     break;
   case 6: // 1024 threads per vertex; deg < 8192: 16384 slots, or (unit edge weights) deg < 16384: 32768 slots
     if constexpr (EW) {
-      launch_team<MODE, EW, P64, 1024, 16384, 1>(h, a, 1);
+      launch_team<MODE, EW, P64, 1024, 16384, 1>(h, a);
     } else {
-      launch_team<MODE, EW, P64, 1024, 32768, 1, true>(h, a, 1);
+      launch_team<MODE, EW, P64, 1024, 32768, 1, true>(h, a);
     }
     break;
   default: {
@@ -2027,14 +2047,15 @@ int kmp_lp_create(const kmp_lp_config *cfg, kmp_lp_handle **out) {
   if (const char *e = std::getenv("KMP_OVERLAP_TIERS")) { // experiments: 0 = launch the tiers of a sub-round serially
     h->overlap_tiers = std::atoi(e) != 0;
   }
-  configure_team_kernels<0, false, false>();
-  configure_team_kernels<0, false, true>();
-  configure_team_kernels<0, true, false>();
-  configure_team_kernels<0, true, true>();
-  configure_team_kernels<1, false, false>();
-  configure_team_kernels<1, false, true>();
-  configure_team_kernels<1, true, false>();
-  configure_team_kernels<1, true, true>();
+  int sms = kSMs;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  if (!(configure_team_kernels<0, false, false>(h, sms) && configure_team_kernels<0, false, true>(h, sms) &&
+        configure_team_kernels<0, true, false>(h, sms) && configure_team_kernels<0, true, true>(h, sms) &&
+        configure_team_kernels<1, false, false>(h, sms) && configure_team_kernels<1, false, true>(h, sms) &&
+        configure_team_kernels<1, true, false>(h, sms) && configure_team_kernels<1, true, true>(h, sms))) {
+    delete h;
+    return fail(KMP_ERR_CUDA, "a sweep_team kernel cannot be resident on this device");
+  }
   *out = h;
   return KMP_OK;
 }

@@ -353,14 +353,22 @@ __device__ __forceinline__ int32_t team_rating(const typename TeamVals<V16>::wor
   return TeamVals<V16>::get(vals, slot) + (EW ? 0 : 1);
 }
 
+// CTAs per SM a team tier is built for. __launch_bounds__ caps the registers so that this many fit
+// (65536 / (threads * CTAs), allocated in steps of 8): tier 3 (256 threads, 32 KiB table + 1 KiB reserved per CTA)
+// is held to 6 by shared memory anyway (7 would need more than the SM's 228 KiB), tiers 4 and 5 (512 threads,
+// 64 KiB) fit 3 with <= 40 registers, tier 6 takes a whole SM. tests/test_team_resources.py checks the build.
+template <int T> constexpr int team_ctas_per_sm() { return T == 32 ? 6 : T == 1024 ? 1 : 3; }
+
 template <int MODE, bool EW, bool P64, int T, int SLOTS, int TEAMS, bool V16 = false>
-__global__ void __launch_bounds__(T *TEAMS) sweep_team(const SweepArgs a) {
+__global__ void __launch_bounds__(T *TEAMS, team_ctas_per_sm<T>()) sweep_team(const SweepArgs a) {
   static_assert((SLOTS & (SLOTS - 1)) == 0, "table size must be a power of two");
   static_assert(!(V16 && EW), "16-bit ratings need unit edge weights");
   using TV = TeamVals<V16>;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   __shared__ Cand s_red_all[TEAMS][T > 32 ? T / 32 : 1];
   __shared__ uint32_t s_next[TEAMS];
+  // the scan counters are written by the team's thread 0 only: kept here, not in four registers of every thread
+  __shared__ unsigned long long s_edges[TEAMS], s_nodes[TEAMS];
   const int team = threadIdx.x / T;
   const int tid = threadIdx.x % T;
   const int bar = 1 + team;
@@ -372,9 +380,10 @@ __global__ void __launch_bounds__(T *TEAMS) sweep_team(const SweepArgs a) {
     keys[s] = kEmpty;
     TV::clear(vals, s);
   }
-  unsigned long long edges = 0, nodes = 0;
   // work queue: the next list index is claimed one vertex ahead
   if (tid == 0) {
+    s_edges[team] = 0;
+    s_nodes[team] = 0;
     s_next[team] = atomicAdd(a.queue, 1u);
   }
   TeamSync<T>::sync(bar);
@@ -540,8 +549,8 @@ __global__ void __launch_bounds__(T *TEAMS) sweep_team(const SweepArgs a) {
       TV::clear(vals, s);
     }
     if (act && tid == 0) {
-      edges += deg;
-      nodes += 1;
+      s_edges[team] += deg;
+      s_nodes[team] += 1;
       if (a.active != nullptr && flag) {
         a.active[u] = 0;
       }
@@ -553,7 +562,10 @@ __global__ void __launch_bounds__(T *TEAMS) sweep_team(const SweepArgs a) {
     }
     TeamSync<T>::sync(bar); // table clean, s_next written
   }
-  block_count_flush(a, edges, nodes);
+  if (tid == 0 && s_nodes[team] != 0) {
+    atomicAdd(&a.counters[0], s_edges[team]);
+    atomicAdd(&a.counters[kCounterNodesOffset], s_nodes[team]);
+  }
 }
 
 // ================================================================================================
