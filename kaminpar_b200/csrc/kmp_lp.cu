@@ -28,6 +28,7 @@
 #include "../../include/kaminpar_b200_lp.h"
 #include "lp_commit.cuh"
 #include "lp_device.cuh"
+#include "lp_lowgroup.cuh"
 #include "lp_strict.cuh"
 #include "lp_sweep.cuh"
 
@@ -226,6 +227,9 @@ struct kmp_lp_handle {
   int fused_blocks = 0;      // co-resident CTAs of the fused kernel (0: not available)
   int fused_blocks_refine = 0;
   bool fused_commit = true;
+  // co-resident CTAs of the persistent kernels of degree groups 0 and 1 (lp_lowgroup.cuh), [group][EW][P64];
+  // 0: no cooperative launch on this device (the per-sub-round path runs instead)
+  uint32_t low_blocks[2][2][2] = {};
   // resident CTAs of each sweep_team instantiation on the device, [MODE][EW][P64][team size 32 / 128 / 512 / 1024]:
   // a larger grid only adds CTAs that start after the work queue is drained
   uint32_t team_grid[2][2][2][4] = {};
@@ -1514,6 +1518,93 @@ int dist_unpack_commit(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32
   return r2;
 }
 
+// ---- degree groups 0 and 1 of a clustering round: one persistent cooperative launch each (lp_lowgroup.cuh) ----
+template <bool EW, bool P64> const void *low_group_kernel_t(int group) {
+  return group == 0 ? reinterpret_cast<const void *>(sweep_commit_low<EW, P64, 8, 8, 4>)
+                    : reinterpret_cast<const void *>(sweep_commit_low<EW, P64, 16, 32, 8>);
+}
+const void *low_group_kernel(bool ew, bool p64, int group) {
+  return ew ? (p64 ? low_group_kernel_t<true, true>(group) : low_group_kernel_t<true, false>(group))
+            : (p64 ? low_group_kernel_t<false, true>(group) : low_group_kernel_t<false, false>(group));
+}
+// per device, from kmp_lp_create on a device with cooperative launches: false if a kernel cannot be resident
+bool configure_low_groups(kmp_lp_handle *h, int sms) {
+  for (int g = 0; g < 2; ++g) {
+    for (int ew = 0; ew < 2; ++ew) {
+      for (int p64 = 0; p64 < 2; ++p64) {
+        int per_sm = 0;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, low_group_kernel(ew, p64, g), 256, 0) != cudaSuccess ||
+            per_sm < 1) {
+          return false;
+        }
+        h->low_blocks[g][ew][p64] = static_cast<uint32_t>(sms * per_sm);
+      }
+    }
+  }
+  return true;
+}
+// The clusterer on one GPU with the register-sort kernels in tiers 0..2; the sharded run, the refiner and the
+// stepping API keep the per-sub-round path (its commit is fused into one cooperative launch as well).
+bool can_run_low_groups(const kmp_lp_handle *h, const RunCtx &rc) {
+  return rc.mode == 0 && h->world == 1 && !h->stepping && h->fused_commit && h->low_blocks[0][0][0] > 0 &&
+         h->thread_max_deg >= 32;
+}
+static_assert((255 - 1) / kNumTiers <= kLowMaxSubrounds, "ensure_lists admits more sub-rounds than LowGroupArgs holds");
+// All sub-rounds of degree group `group` (0: tier 0, 1: tiers 1-2) of LP round `iter`, in sub-round order, with the
+// hashes, stamp windows, move stamps and proposal-counter parities the per-sub-round path uses.
+int run_low_group(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, int group) {
+  const uint32_t S = h->lists_S;
+  const int ta = first_tier_of_group(group), tb = last_tier_of_group(group);
+  SweepArgs sa = make_sweep_args(h, rc);
+  sa.base_tie = sync_base(h->cfg.seed, h->call_counter, iter, SALT_TIE);
+  sa.base_fav = sync_base(h->cfg.seed, h->call_counter, iter, SALT_FAV);
+  sa.accumulate = true;
+  sa.pull = h->pull_this;
+  sa.list = h->order.p;
+  CommitArgs ca = make_commit_args(h, rc);
+  LowGroupArgs g{};
+  g.push = !h->pull_this || !h->pull_next;
+  g.ctr32 = h->ctr32.p;
+  g.counters[0] = h->ctr64.p + ta;
+  g.counters[1] = h->ctr64.p + tb;
+  uint32_t max_total = 0;
+  for (uint32_t s = 0; s < S; ++s) {
+    const uint32_t sg = static_cast<uint32_t>(group) * S + s;
+    const SubRound q = subround_of_sg(h, sg);
+    if (q.total == 0) {
+      continue;
+    }
+    LowSubround &x = g.sub[g.num_sub++];
+    x.off[0] = h->list_off[ta * S + s];
+    x.size[0] = q.size[ta];
+    x.off[1] = h->list_off[tb * S + s];
+    x.size[1] = tb != ta ? q.size[tb] : 0u;
+    const StampWindow w = make_window(iter, sg);
+    x.window_start = w.start;
+    x.window_len = w.len;
+    x.base_commit = sync_base(h->cfg.seed, h->call_counter, iter * 4096 + sg, SALT_COMMIT);
+    x.stamp = h->stamps_ok ? make_stamp(iter, sg) : 0u;
+    x.parity = h->mover_parity;
+    h->mover_parity ^= 1u;
+    max_total = std::max(max_total, q.total);
+  }
+  if (g.num_sub == 0) {
+    return KMP_OK;
+  }
+  const bool ew = h->adjwgt != nullptr;
+  const uint32_t blocks = std::min<uint32_t>(grid_for(max_total, 256), h->low_blocks[group][ew][h->p64]);
+  GridBarrier bar{h->grid_bar.p, h->grid_bar.p + 1};
+  void *args[] = {&sa, &ca, &g, &bar};
+  // timing mode: the group's sweeps AND commits are this one event pair, under the group's first tier
+  const int ev = timed_begin(h, ta);
+  KMP_CUDA(cudaLaunchCooperativeKernel(low_group_kernel(ew, h->p64, group), dim3(blocks), dim3(256), args, 0, h->stream));
+  timed_end(h, ev);
+  ++h->kernel_launches;
+  ++h->sweep_launches;
+  ++h->group_launches[ta];
+  return KMP_OK;
+}
+
 // One LP round over all (group, sub-round) lists. Returns via *moved the accepted moves.
 int run_iteration(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t *moved, uint32_t *proposals) {
   const uint32_t S = h->lists_S;
@@ -1546,6 +1637,14 @@ int run_iteration(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t *m
       if (rc2 != KMP_OK) {
         return rc2;
       }
+      continue;
+    }
+    if (q.group <= 1 && can_run_low_groups(h, rc)) { // every sub-round of the group in one launch
+      rc2 = run_low_group(h, rc, iter, q.group);
+      if (rc2 != KMP_OK) {
+        return rc2;
+      }
+      sg = static_cast<uint32_t>(q.group + 1) * S - 1;
       continue;
     }
     rc2 = sweep_subround(h, rc, iter, sg, q);
@@ -2035,6 +2134,10 @@ int kmp_lp_create(const kmp_lp_config *cfg, kmp_lp_handle **out) {
               cudaSuccess &&
           per_sm_r > 0) {
         h->fused_blocks_refine = sms * per_sm_r;
+      }
+      if (!configure_low_groups(h, sms)) {
+        delete h;
+        return fail(KMP_ERR_CUDA, "a persistent low-degree clustering kernel cannot be resident on this device");
       }
     }
     if (const char *e = std::getenv("KMP_FUSED_COMMIT")) { // experiments / tests: 0 = separate commit kernels

@@ -108,20 +108,25 @@ struct GridBarrier {
   unsigned *count;        // arrivals of the running barrier (returns to 0)
   volatile unsigned *gen; // generation, only ever incremented
 };
+// Thread 0 of each CTA arrives with a release-acquire add (its CTA's writes are ordered before it by the first
+// __syncthreads) and the last arrival publishes the next generation with a release store; the others wait for
+// it with acquire loads. Release / acquire at GPU scope instead of sequentially consistent fences: the barrier
+// runs up to four times per sub-round.
 __device__ __forceinline__ void grid_sync(const GridBarrier &b) {
   __syncthreads();
   if (threadIdx.x == 0) {
-    const unsigned g = *b.gen;
-    __threadfence();
-    if (atomicAdd(b.count, 1u) == gridDim.x - 1) {
+    const unsigned g = *b.gen; // before the arrival: the release add keeps it there
+    unsigned prev;
+    asm volatile("atom.add.acq_rel.gpu.u32 %0, [%1], 1;" : "=r"(prev) : "l"(b.count) : "memory");
+    if (prev == gridDim.x - 1) {
       *b.count = 0;
-      __threadfence();
-      atomicAdd(const_cast<unsigned *>(b.gen), 1u);
+      asm volatile("st.release.gpu.u32 [%0], %1;" ::"l"(b.gen), "r"(g + 1) : "memory");
     } else {
-      while (*b.gen == g) {
-      }
+      unsigned cur;
+      do {
+        asm volatile("ld.acquire.gpu.u32 %0, [%1];" : "=r"(cur) : "l"(b.gen) : "memory");
+      } while (cur == g);
     }
-    __threadfence();
   }
   __syncthreads();
 }
@@ -132,36 +137,11 @@ struct GatheredArgs {              // sharded run: proposal buffers of all ranks
   uint32_t *mover_count_w;         // writable alias of CommitArgs::mover_count
 };
 
-template <bool P64>
-__global__ void __launch_bounds__(256) commit_cluster_fused(const CommitArgs a, const GatheredArgs ga, const GridBarrier bar) {
-  const uint32_t tid = blockIdx.x * blockDim.x + threadIdx.x;
-  const uint32_t nth = gridDim.x * blockDim.x;
-  uint32_t cnt;
-  if (ga.gathered != nullptr) {
-    // ---- unpack (rank order) + accumulate incoming[] over ALL proposals
-    const size_t stride = 4 + 2 * static_cast<size_t>(ga.cap);
-    uint32_t total = 0;
-    uint32_t *mv_u = const_cast<uint32_t *>(a.mv_u), *mv_t = const_cast<uint32_t *>(a.mv_t);
-    for (uint32_t r = 0; r < ga.world; ++r) {
-      const uint32_t c = ga.gathered[r * stride];
-      for (uint32_t i = tid; i < c; i += nth) {
-        const uint32_t u = ga.gathered[r * stride + 4 + i];
-        const uint32_t t = ga.gathered[r * stride + 4 + ga.cap + i];
-        mv_u[total + i] = u;
-        mv_t[total + i] = t;
-        atomicAdd(&a.incoming[t], node_weight(a, u));
-      }
-      total += c;
-    }
-    cnt = total;
-    if (tid == 0) {
-      *ga.mover_count_w = total;
-    }
-    grid_sync(bar);
-  } else {
-    cnt = *a.mover_count;
-  }
-  // ---- classify: uncontended targets accept everything; contended ones get a slot and a level histogram
+// The phases of a grid-wide clusterer commit over the `cnt` proposals (grid_sync between them). Thread `tid` of
+// `nth` takes proposals tid, tid + nth, ... in every phase, so acc[i] / cslot[i] are read back by the thread that
+// wrote them; what other threads accumulated in an earlier phase is read through L2 (__ldcg).
+// (1) classify: uncontended targets accept everything; contended ones get a slot and a level histogram
+__device__ __forceinline__ void cluster_classify(const CommitArgs &a, uint32_t cnt, uint32_t tid, uint32_t nth) {
   for (uint32_t i = tid; i < cnt; i += nth) {
     const uint32_t u = a.mv_u[i];
     const uint32_t t = a.mv_t[i];
@@ -176,8 +156,9 @@ __global__ void __launch_bounds__(256) commit_cluster_fused(const CommitArgs a, 
       a.acc[i] = 2;
     }
   }
-  grid_sync(bar);
-  // ---- decide (contended proposals): accept iff level >= jmin(target); weights are still the frozen ones
+}
+// (2) decide (contended proposals): accept iff level >= jmin(target); weights are still the frozen ones
+__device__ __forceinline__ void cluster_decide(const CommitArgs &a, uint32_t cnt, uint32_t tid, uint32_t nth) {
   for (uint32_t i = tid; i < cnt; i += nth) {
     if (a.acc[i] != 2) {
       continue;
@@ -198,8 +179,10 @@ __global__ void __launch_bounds__(256) commit_cluster_fused(const CommitArgs a, 
     const uint32_t lvl = ladder_level(bijective32(u, a.base_commit));
     a.acc[i] = static_cast<int>(lvl) >= jm ? 1 : 0;
   }
-  grid_sync(bar);
-  // ---- apply
+}
+// (3) apply the accepted moves, clean the contended-target scratch, zero the next sub-round's proposal counter
+template <bool P64>
+__device__ __forceinline__ void cluster_apply(const CommitArgs &a, uint32_t cnt, uint32_t tid, uint32_t nth) {
   if (tid == 0) {
     *a.next_mover_count = 0;
     if (a.also_zero != nullptr) {
@@ -237,6 +220,42 @@ __global__ void __launch_bounds__(256) commit_cluster_fused(const CommitArgs a, 
   if ((threadIdx.x & 31) == 0 && moved != 0) {
     atomicAdd(a.moved_count, moved);
   }
+}
+
+template <bool P64>
+__global__ void __launch_bounds__(256) commit_cluster_fused(const CommitArgs a, const GatheredArgs ga, const GridBarrier bar) {
+  const uint32_t tid = blockIdx.x * blockDim.x + threadIdx.x;
+  const uint32_t nth = gridDim.x * blockDim.x;
+  uint32_t cnt;
+  if (ga.gathered != nullptr) {
+    // ---- unpack (rank order) + accumulate incoming[] over ALL proposals
+    const size_t stride = 4 + 2 * static_cast<size_t>(ga.cap);
+    uint32_t total = 0;
+    uint32_t *mv_u = const_cast<uint32_t *>(a.mv_u), *mv_t = const_cast<uint32_t *>(a.mv_t);
+    for (uint32_t r = 0; r < ga.world; ++r) {
+      const uint32_t c = ga.gathered[r * stride];
+      for (uint32_t i = tid; i < c; i += nth) {
+        const uint32_t u = ga.gathered[r * stride + 4 + i];
+        const uint32_t t = ga.gathered[r * stride + 4 + ga.cap + i];
+        mv_u[total + i] = u;
+        mv_t[total + i] = t;
+        atomicAdd(&a.incoming[t], node_weight(a, u));
+      }
+      total += c;
+    }
+    cnt = total;
+    if (tid == 0) {
+      *ga.mover_count_w = total;
+    }
+    grid_sync(bar);
+  } else {
+    cnt = *a.mover_count;
+  }
+  cluster_classify(a, cnt, tid, nth);
+  grid_sync(bar);
+  cluster_decide(a, cnt, tid, nth);
+  grid_sync(bar);
+  cluster_apply<P64>(a, cnt, tid, nth);
 }
 
 // ---- refiner ------------------------------------------------------------------------------------
@@ -649,11 +668,10 @@ template <int MODE, bool P64> __global__ void __launch_bounds__(256) commit_appl
 // ---- push activation (only in rounds with few movers, see kmp_lp.cu choose_activation) ---------
 // A team of LANES threads (by the degree group of the sub-round) flags the neighbours of one accepted
 // mover as active (label_propagation.h:848-870).
-template <int LANES> __global__ void __launch_bounds__(256) commit_activate(const CommitArgs a) {
-  const uint32_t cnt = *a.mover_count;
-  const uint32_t tid = blockIdx.x * blockDim.x + threadIdx.x;
+template <int LANES>
+__device__ __forceinline__ void activate_neighbours(const CommitArgs &a, uint32_t cnt, uint32_t tid, uint32_t nth) {
   const uint32_t sub = tid % LANES;
-  const uint32_t nteams = (gridDim.x * blockDim.x) / LANES;
+  const uint32_t nteams = nth / LANES;
   for (uint32_t i = tid / LANES; i < cnt; i += nteams) {
     if (a.acc[i] != 1) {
       continue;
@@ -674,6 +692,9 @@ template <int LANES> __global__ void __launch_bounds__(256) commit_activate(cons
       }
     }
   }
+}
+template <int LANES> __global__ void __launch_bounds__(256) commit_activate(const CommitArgs a) {
+  activate_neighbours<LANES>(a, *a.mover_count, blockIdx.x * blockDim.x + threadIdx.x, gridDim.x * blockDim.x);
 }
 // acc[] must start at 0 for the refiner's multi-pass decide; clear it and the counters
 __global__ void commit_begin(uint8_t *acc, const uint32_t *mover_count) {
