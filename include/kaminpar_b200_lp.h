@@ -74,7 +74,7 @@ typedef struct {
                                       label_propagation.h:272-319 is not implemented: non-zero = KMP_ERR_UNSUPPORTED */
   /* engine */
   int32_t seed;                /* Random::reseed() analogue; enters every hash key */
-  uint32_t sync_subrounds;     /* S: hashed sub-rounds per degree group and iteration (8) */
+  uint32_t sync_subrounds;     /* S: hashed sub-rounds per degree group and iteration (8; 0 = 8, at most 31) */
   uint32_t sync_granule_log2;  /* vertices u >> g share a sub-round (4) */
   uint32_t sync_commit_passes; /* commit passes crediting departures: 1 clusterer, 4 refiner. The clusterer's
                                   commit is single-pass: kmp_lp_cluster refuses > 1 with KMP_ERR_UNSUPPORTED */
@@ -127,7 +127,9 @@ void kmp_lp_default_config(int mode, kmp_lp_config *cfg);
  * 2 GiB; smaller values process a sub-round's hubs in more waves), KMP_HUB_BUCKET_CAP / KMP_HUB_SEL_LIMIT = smaller
  * bucket capacity / claim limit of the hub tier (force its overflow list and multi-pass selection),
  * KMP_THREAD_MAX_DEG = 16 sends degrees 17..31 to the warp kernel instead of the register-sort kernel,
- * KMP_FUSED_COMMIT=0, KMP_OVERLAP_TIERS=0, KMP_FORCE_P64=1, KMP_UPLOAD_OVERLAP=0 (launch structure / word width).
+ * KMP_FUSED_COMMIT=0, KMP_OVERLAP_TIERS=0, KMP_FORCE_P64=1, KMP_UPLOAD_OVERLAP=0 (launch structure / word width),
+ * KMP_GRID_CAP = N caps the CTA count of every launch inside an LP round at N (small inputs then take every
+ * grid-stride loop and work-queue refill several times).
  * Read per call: KMP_ACTIVATION=push|pull, KMP_TRACE=1 (set_graph stage times on stderr). */
 int kmp_lp_create(const kmp_lp_config *cfg, kmp_lp_handle **out);
 int kmp_lp_destroy(kmp_lp_handle *h);

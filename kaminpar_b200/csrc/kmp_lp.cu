@@ -54,6 +54,8 @@ int fail(int code, const std::string &msg) {
 
 constexpr int kNumGroups = 4; // degree groups of the schedule
 constexpr int kNumTiers = 8;  // kernel tiers: group 1 is split in two, group 3 (deg >= 256) in four
+// sync_subrounds: the work-list keys (tier * S + sub-round, plus one key for unvisited vertices) are 8 bits wide
+constexpr uint32_t kMaxSubrounds = (255 - 1) / kNumTiers;
 constexpr int kHubTier = 7;   // deg >= kHubMinDegree: edge-parallel kernels, label-partitioned buckets (lp_sweep.cuh)
 constexpr int kStatTiers = 12; // tier slots of kmp_lp_stats / ctr64 (edges at [tier], nodes at [kCtrNodes + tier])
 constexpr int kCtrNodes = 16, kCtrScratch = 40, kCtrSize = 48;
@@ -124,6 +126,7 @@ struct kmp_lp_handle {
   std::vector<int> sweep_event_group;
   uint64_t group_launches[kStatTiers] = {};
   uint32_t thread_max_deg = 32; // KMP_THREAD_MAX_DEG: 16 / 32 (which tiers run the register-sort kernel)
+  uint32_t grid_cap = 0;        // KMP_GRID_CAP: most CTAs of any launch inside an LP round (0: no cap)
   // packed (label, stamp) gather array of the sweeps (lp_device.cuh): 4 B per vertex while labels fit 24 bits
   // (n <= 2^24 clusterer / k <= 2^24 refiner), else 8 B
   DevBuf<unsigned char> labg;
@@ -616,6 +619,12 @@ inline uint32_t grid_for(uint64_t threads_needed, uint32_t block, uint32_t max_b
   const uint64_t b = (threads_needed + block - 1) / block;
   return static_cast<uint32_t>(std::max<uint64_t>(1, std::min<uint64_t>(b, max_blocks)));
 }
+// CTA count of a launch inside an LP round under KMP_GRID_CAP (tests): with a tiny grid, small inputs take every
+// grid-stride loop, work-queue refill and persistent-kernel iteration many times. A capped cooperative grid stays
+// co-resident.
+inline uint32_t capped(const kmp_lp_handle *h, uint32_t blocks) {
+  return h->grid_cap != 0 && blocks > h->grid_cap ? h->grid_cap : blocks;
+}
 
 constexpr int team_size_index(int T) { return T == 32 ? 0 : T == 128 ? 1 : T == 512 ? 2 : 3; }
 template <int SLOTS, int TEAMS, bool V16> constexpr size_t team_smem() {
@@ -625,7 +634,7 @@ template <int SLOTS, int TEAMS, bool V16> constexpr size_t team_smem() {
 template <int MODE, bool EW, bool P64, int T, int SLOTS, int TEAMS, bool V16 = false>
 void launch_team(kmp_lp_handle *h, const SweepArgs &a) {
   const uint32_t want = (a.list_size + TEAMS - 1) / TEAMS;
-  const uint32_t blocks = std::max<uint32_t>(1, std::min<uint32_t>(want, h->team_grid[MODE][EW][P64][team_size_index(T)]));
+  const uint32_t blocks = capped(h, std::max<uint32_t>(1, std::min<uint32_t>(want, h->team_grid[MODE][EW][P64][team_size_index(T)])));
   sweep_team<MODE, EW, P64, T, SLOTS, TEAMS, V16><<<blocks, T * TEAMS, team_smem<SLOTS, TEAMS, V16>(), h->sweep_stream>>>(a);
 }
 
@@ -660,7 +669,7 @@ template <int MODE, bool EW, bool P64> cudaError_t launch_sweep_t(kmp_lp_handle 
   if (a.list_size == 0) {
     return cudaSuccess;
   }
-  const uint32_t tgrid = grid_for(a.list_size, 256);
+  const uint32_t tgrid = capped(h, grid_for(a.list_size, 256));
   switch (tier) {
   case 0: // deg <= 7: thread per vertex, labels sorted in registers
     sweep_thread<MODE, EW, P64, 8><<<tgrid, 256, 0, h->sweep_stream>>>(a);
@@ -719,18 +728,18 @@ template <int MODE, bool EW, bool P64> cudaError_t launch_sweep_t(kmp_lp_handle 
       hb.num_items = wv.item_hi - wv.item_lo;
       hb.queue = h->ctr32.p + 64 + w; // zeroed with the other per-round counters
       hb.ovf_count = h->ctr32.p + 512 + w;
-      sweep_hub_scatter<MODE, EW, P64><<<std::min<uint32_t>(hb.num_items, kSMs * 4), kHubThreads, kHubScatterSmem, h->sweep_stream>>>(a, hb, h->m);
+      sweep_hub_scatter<MODE, EW, P64><<<capped(h, std::min<uint32_t>(hb.num_items, kSMs * 4)), kHubThreads, kHubScatterSmem, h->sweep_stream>>>(a, hb, h->m);
       hb.sel_entry = h->t4_sel_entry.p + wv.sel_lo;
       hb.sel_piece = h->t4_sel_piece.p + wv.sel_lo;
       hb.num_sel_items = wv.sel_hi - wv.sel_lo;
       hb.part_best = h->t4_part_best.p + (wv.sel_lo - h->t4_sel_off[s_idx]);
       hb.part_fav = h->t4_part_fav.p + (wv.sel_lo - h->t4_sel_off[s_idx]);
-      sweep_hub_select<MODE><<<std::min<uint32_t>((hb.num_sel_items + kSelWarps - 1) / kSelWarps, kSMs * 6), kSelWarps * 32, 0, h->sweep_stream>>>(a, hb);
+      sweep_hub_select<MODE><<<capped(h, std::min<uint32_t>((hb.num_sel_items + kSelWarps - 1) / kSelWarps, kSMs * 6)), kSelWarps * 32, 0, h->sweep_stream>>>(a, hb);
       h->kernel_launches += 2;
     }
     hb.part_best = h->t4_part_best.p;
     hb.part_fav = h->t4_part_fav.p;
-    sweep_hub_final<MODE><<<grid_for(static_cast<uint64_t>(a.list_size) * 32, 256), 256, 0, h->sweep_stream>>>(a, hb);
+    sweep_hub_final<MODE><<<capped(h, grid_for(static_cast<uint64_t>(a.list_size) * 32, 256)), 256, 0, h->sweep_stream>>>(a, hb);
     break;
   }
   }
@@ -815,8 +824,8 @@ int ensure_lists(kmp_lp_handle *h) {
       h->lists_thr == h->cfg.large_degree_threshold && h->lists_seed == h->cfg.seed) {
     return KMP_OK;
   }
-  if (kNumTiers * S + 1 > 255) {
-    return fail(KMP_ERR_INVALID, "sync_subrounds too large (max 36)");
+  if (S > kMaxSubrounds) {
+    return fail(KMP_ERR_INVALID, "sync_subrounds too large (max " + std::to_string(kMaxSubrounds) + ")");
   }
   h->stamps_ok = kNumGroups * S <= kMaxStampSubrounds; // else: push activation only
   const uint32_t n = h->n;
@@ -1231,10 +1240,10 @@ void launch_push_activation(kmp_lp_handle *h, const CommitArgs &ca, const SubRou
   const uint32_t size = q.total;
   const int ev = timed_begin(h, kTagPush);
   switch (q.group) {
-  case 0: commit_activate<4><<<grid_for(static_cast<uint64_t>(size) * 4, 256, kSMs * 6), 256, 0, h->stream>>>(ca); break;
-  case 1: commit_activate<8><<<grid_for(static_cast<uint64_t>(size) * 8, 256, kSMs * 6), 256, 0, h->stream>>>(ca); break;
-  case 2: commit_activate<32><<<grid_for(static_cast<uint64_t>(size) * 32, 256, kSMs * 6), 256, 0, h->stream>>>(ca); break;
-  default: commit_activate<256><<<grid_for(static_cast<uint64_t>(size) * 256, 256, kSMs * 6), 256, 0, h->stream>>>(ca); break;
+  case 0: commit_activate<4><<<capped(h, grid_for(static_cast<uint64_t>(size) * 4, 256, kSMs * 6)), 256, 0, h->stream>>>(ca); break;
+  case 1: commit_activate<8><<<capped(h, grid_for(static_cast<uint64_t>(size) * 8, 256, kSMs * 6)), 256, 0, h->stream>>>(ca); break;
+  case 2: commit_activate<32><<<capped(h, grid_for(static_cast<uint64_t>(size) * 32, 256, kSMs * 6)), 256, 0, h->stream>>>(ca); break;
+  default: commit_activate<256><<<capped(h, grid_for(static_cast<uint64_t>(size) * 256, 256, kSMs * 6)), 256, 0, h->stream>>>(ca); break;
   }
   timed_end(h, ev);
   ++h->kernel_launches;
@@ -1253,8 +1262,8 @@ int commit_subround_fused(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uin
     const uint32_t k = rc.num_labels;
     const size_t smem = 4 * std::max<size_t>(k * kLadderLevels <= kSmemPrivLimit ? static_cast<size_t>(k) * kLadderLevels : 0,
                                              k <= kSmemPrivLimit ? k : 0);
-    const uint32_t blocks = std::min<uint32_t>(grid_for(std::max<uint32_t>(q.total, k), 256),
-                                               static_cast<uint32_t>(h->fused_blocks_refine));
+    const uint32_t blocks = capped(h, std::min<uint32_t>(grid_for(std::max<uint32_t>(q.total, k), 256),
+                                                         static_cast<uint32_t>(h->fused_blocks_refine)));
     void *rargs[] = {&ca, &ga, &bar, &passes};
     if (h->p64) {
       KMP_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void *>(commit_refine_fused<true>), dim3(blocks), dim3(256), rargs,
@@ -1271,7 +1280,7 @@ int commit_subround_fused(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uin
     h->mover_parity ^= 1u;
     return KMP_OK;
   }
-  const uint32_t blocks = std::min<uint32_t>(grid_for(q.total, 256), static_cast<uint32_t>(h->fused_blocks));
+  const uint32_t blocks = capped(h, std::min<uint32_t>(grid_for(q.total, 256), static_cast<uint32_t>(h->fused_blocks)));
   void *args[] = {&ca, &ga, &bar};
   if (h->p64) {
     KMP_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void *>(commit_cluster_fused<true>), dim3(blocks), dim3(256), args, 0,
@@ -1299,14 +1308,14 @@ int commit_subround(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t 
   ca.stamp = h->stamps_ok ? make_stamp(iter, sg) : 0;
   const uint32_t size = q.total;
   const uint32_t passes = std::max<uint32_t>(1, h->cfg.sync_commit_passes);
-  const uint32_t cgrid = grid_for(size, 256, kSMs * 8);
+  const uint32_t cgrid = capped(h, grid_for(size, 256, kSMs * 8));
   int ev = timed_begin(h, kTagCommit);
   if (rc.mode == 0) {
     commit_cluster_classify<<<cgrid, 256, 0, h->stream>>>(ca);
     commit_cluster_decide<<<cgrid, 256, 0, h->stream>>>(ca);
     h->kernel_launches += 2;
   } else {
-    const uint32_t kgrid = grid_for(rc.num_labels, 128);
+    const uint32_t kgrid = capped(h, grid_for(rc.num_labels, 128));
     const size_t smem_k = rc.num_labels <= kSmemPrivLimit ? static_cast<size_t>(rc.num_labels) * 4 : 0;
     if (!h->step_accumulated) { // level histograms over all proposals (the stepping path did it already)
       const size_t smem_h = rc.num_labels * kLadderLevels <= kSmemPrivLimit ? static_cast<size_t>(rc.num_labels) * kLadderLevels * 4 : 0;
@@ -1327,7 +1336,7 @@ int commit_subround(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t 
       commit_refine_othin<<<cgrid, 256, 0, h->stream>>>(ca);
       h->kernel_launches += 3;
     }
-    commit_refine_reset<<<grid_for(static_cast<uint64_t>(rc.num_labels) * kLadderLevels, 128), 128, 0, h->stream>>>(ca);
+    commit_refine_reset<<<capped(h, grid_for(static_cast<uint64_t>(rc.num_labels) * kLadderLevels, 128)), 128, 0, h->stream>>>(ca);
     h->kernel_launches += 1;
   }
   timed_end(h, ev);
@@ -1337,7 +1346,7 @@ int commit_subround(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t 
   ev = timed_begin(h, kTagApply);
   {
     const size_t smem_k = (rc.mode == 1 && rc.num_labels <= kSmemPrivLimit) ? static_cast<size_t>(rc.num_labels) * 4 : 0;
-    const uint32_t agrid = grid_for(size, 256, kSMs * 4);
+    const uint32_t agrid = capped(h, grid_for(size, 256, kSMs * 4));
     if (rc.mode == 0) {
       if (h->p64) {
         commit_apply<0, true><<<agrid, 256, 0, h->stream>>>(ca);
@@ -1483,7 +1492,7 @@ int dist_sweep_pack(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t 
   if (direct) {
     return KMP_OK;
   }
-  k_pack_movers<<<grid_for(cap, 256, kSMs * 4), 256, 0, h->stream>>>(h->mv_u.p, h->mv_t.p,
+  k_pack_movers<<<capped(h, grid_for(cap, 256, kSMs * 4)), 256, 0, h->stream>>>(h->mv_u.p, h->mv_t.p,
                                                                       h->ctr32.p + (h->mover_parity ? 3 : 0), cap, d_send);
   ++h->kernel_launches;
   KMP_CUDA(cudaGetLastError());
@@ -1499,9 +1508,9 @@ int dist_unpack_commit(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32
   }
   const uint32_t cap = subround_cap(h, q);
   const uint32_t base_commit = sync_base(h->cfg.seed, h->call_counter, iter * 4096 + sg, SALT_COMMIT);
-  k_unpack_movers<<<grid_for(cap, 256, kSMs * 4), 256, 0, h->stream>>>(d_gathered, h->world, cap, h->mv_u.p, h->mv_t.p,
+  k_unpack_movers<<<capped(h, grid_for(cap, 256, kSMs * 4)), 256, 0, h->stream>>>(d_gathered, h->world, cap, h->mv_u.p, h->mv_t.p,
                                                                         h->ctr32.p + (h->mover_parity ? 3 : 0));
-  const uint32_t agrid = grid_for(q.total, 256, kSMs * 8);
+  const uint32_t agrid = capped(h, grid_for(q.total, 256, kSMs * 8));
   if (rc.mode == 0) {
     k_accumulate_movers<0><<<agrid, 256, 0, h->stream>>>(h->mv_u.p, h->mv_t.p, h->ctr32.p + (h->mover_parity ? 3 : 0), h->vwgt,
                                                           base_commit, h->incoming.p, h->hist.p, rc.num_labels);
@@ -1549,7 +1558,7 @@ bool can_run_low_groups(const kmp_lp_handle *h, const RunCtx &rc) {
   return rc.mode == 0 && h->world == 1 && !h->stepping && h->fused_commit && h->low_blocks[0][0][0] > 0 &&
          h->thread_max_deg >= 32;
 }
-static_assert((255 - 1) / kNumTiers <= kLowMaxSubrounds, "ensure_lists admits more sub-rounds than LowGroupArgs holds");
+static_assert(kMaxSubrounds <= kLowMaxSubrounds, "ensure_lists admits more sub-rounds than LowGroupArgs holds");
 // All sub-rounds of degree group `group` (0: tier 0, 1: tiers 1-2) of LP round `iter`, in sub-round order, with the
 // hashes, stamp windows, move stamps and proposal-counter parities the per-sub-round path uses.
 int run_low_group(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, int group) {
@@ -1592,7 +1601,7 @@ int run_low_group(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, int group) 
     return KMP_OK;
   }
   const bool ew = h->adjwgt != nullptr;
-  const uint32_t blocks = std::min<uint32_t>(grid_for(max_total, 256), h->low_blocks[group][ew][h->p64]);
+  const uint32_t blocks = capped(h, std::min<uint32_t>(grid_for(max_total, 256), h->low_blocks[group][ew][h->p64]));
   GridBarrier bar{h->grid_bar.p, h->grid_bar.p + 1};
   void *args[] = {&sa, &ca, &g, &bar};
   // timing mode: the group's sweeps AND commits are this one event pair, under the group's first tier
@@ -2088,6 +2097,9 @@ int kmp_lp_create(const kmp_lp_config *cfg, kmp_lp_handle **out) {
   }
   if (const char *e = std::getenv("KMP_HUB_WAVE_SLOTS")) {
     h->hub_wave_slots = static_cast<uint64_t>(std::max(32ll, std::atoll(e)));
+  }
+  if (const char *e = std::getenv("KMP_GRID_CAP")) {
+    h->grid_cap = static_cast<uint32_t>(std::max(1, std::atoi(e)));
   }
   if (h->cfg.sync_subrounds == 0) {
     h->cfg.sync_subrounds = 8;

@@ -259,37 +259,35 @@ __global__ void __launch_bounds__(256) commit_cluster_fused(const CommitArgs a, 
 }
 
 // ---- refiner ------------------------------------------------------------------------------------
-// suffix sums of the level histograms + reset of the pass state (k threads)
+// The per-block kernels below loop over the k blocks (k * 16 histogram entries) grid-stride: their launches are
+// capped (grid_for), so one thread per block would leave the blocks beyond the grid untouched at large k.
+// suffix sums of the level histograms + reset of the pass state
 __global__ void commit_refine_prepare(const CommitArgs a) {
-  const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= a.k) {
-    return;
-  }
-  int32_t cum = 0;
-  for (int j = kLadderLevels - 1; j >= 0; --j) {
-    cum += a.hist[b * kLadderLevels + j];
-    a.hist[b * kLadderLevels + j] = cum;
-  }
-  a.out_cur[b] = 0;
-  a.out_delta[b] = 0;
-}
-// jmin per block for the running pass; folds the previous pass' departures into out_cur (k threads)
-__global__ void commit_refine_jmin(const CommitArgs a) {
-  const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= a.k) {
-    return;
-  }
-  const int32_t credit = a.out_cur[b] + a.out_delta[b];
-  a.out_cur[b] = credit;
-  a.out_delta[b] = 0;
-  int jm = kLadderLevels;
-  for (int j = 0; j < kLadderLevels; ++j) {
-    if (a.weight[b] + a.hist[b * kLadderLevels + j] - credit <= a.max_w[b]) {
-      jm = j;
-      break;
+  for (uint32_t b = blockIdx.x * blockDim.x + threadIdx.x; b < a.k; b += gridDim.x * blockDim.x) {
+    int32_t cum = 0;
+    for (int j = kLadderLevels - 1; j >= 0; --j) {
+      cum += a.hist[b * kLadderLevels + j];
+      a.hist[b * kLadderLevels + j] = cum;
     }
+    a.out_cur[b] = 0;
+    a.out_delta[b] = 0;
   }
-  a.jmin[b] = jm;
+}
+// jmin per block for the running pass; folds the previous pass' departures into out_cur
+__global__ void commit_refine_jmin(const CommitArgs a) {
+  for (uint32_t b = blockIdx.x * blockDim.x + threadIdx.x; b < a.k; b += gridDim.x * blockDim.x) {
+    const int32_t credit = a.out_cur[b] + a.out_delta[b];
+    a.out_cur[b] = credit;
+    a.out_delta[b] = 0;
+    int jm = kLadderLevels;
+    for (int j = 0; j < kLadderLevels; ++j) {
+      if (a.weight[b] + a.hist[b * kLadderLevels + j] - credit <= a.max_w[b]) {
+        jm = j;
+        break;
+      }
+    }
+    a.jmin[b] = jm;
+  }
 }
 // Block-weight style accumulators are privatised per CTA in shared memory when k is small: millions of
 // proposals hitting k <= a few hundred global addresses serialise in the L2 atomic units.
@@ -347,25 +345,23 @@ __global__ void commit_refine_ohist(const CommitArgs a) {
   }
 }
 __global__ void commit_refine_ojmin(const CommitArgs a) {
-  const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= a.k) {
-    return;
-  }
-  int32_t cum[kLadderLevels];
-  int32_t c = 0;
-  for (int j = kLadderLevels - 1; j >= 0; --j) {
-    c += a.ohist[b * kLadderLevels + j];
-    cum[j] = c;
-    a.ohist[b * kLadderLevels + j] = 0; // reset for the next sub-round
-  }
-  int jm = kLadderLevels;
-  for (int j = 0; j < kLadderLevels; ++j) {
-    if (a.weight[b] - cum[j] >= a.min_w[b]) {
-      jm = j;
-      break;
+  for (uint32_t b = blockIdx.x * blockDim.x + threadIdx.x; b < a.k; b += gridDim.x * blockDim.x) {
+    int32_t cum[kLadderLevels];
+    int32_t c = 0;
+    for (int j = kLadderLevels - 1; j >= 0; --j) {
+      c += a.ohist[b * kLadderLevels + j];
+      cum[j] = c;
+      a.ohist[b * kLadderLevels + j] = 0; // reset for the next sub-round
     }
+    int jm = kLadderLevels;
+    for (int j = 0; j < kLadderLevels; ++j) {
+      if (a.weight[b] - cum[j] >= a.min_w[b]) {
+        jm = j;
+        break;
+      }
+    }
+    a.ojmin[b] = jm;
   }
-  a.ojmin[b] = jm;
 }
 __global__ void commit_refine_othin(const CommitArgs a) {
   const uint32_t cnt = *a.mover_count;
@@ -379,10 +375,9 @@ __global__ void commit_refine_othin(const CommitArgs a) {
     }
   }
 }
-// reset the refiner histograms after the sub-round (k*16 threads)
+// reset the refiner histograms after the sub-round
 __global__ void commit_refine_reset(const CommitArgs a) {
-  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < a.k * kLadderLevels) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < a.k * kLadderLevels; i += gridDim.x * blockDim.x) {
     a.hist[i] = 0;
   }
 }

@@ -83,10 +83,11 @@ def handle(g, mode, max_num_neighbors=UINT32_MAX, large_degree_threshold=UINT32_
     return h
 
 
-def oracle_params(mode, max_num_neighbors=UINT32_MAX, large_degree_threshold=UINT32_MAX, commit_passes=None):
+def oracle_params(mode, max_num_neighbors=UINT32_MAX, large_degree_threshold=UINT32_MAX, commit_passes=None,
+                  subrounds=B.SYNC_SUBROUNDS_DEFAULT, granule_log2=B.SYNC_GRANULE_LOG2_DEFAULT):
     p = B.default_cluster_params() if mode == 0 else B.default_refine_params()
     p.max_num_neighbors, p.large_degree_threshold = max_num_neighbors, large_degree_threshold
-    return B.oracle_params(p, commit_passes=commit_passes or (1 if mode == 0 else 4))
+    return B.oracle_params(p, subrounds, granule_log2, commit_passes=commit_passes or (1 if mode == 0 else 4))
 
 
 def check_t0(h, g, mode, labels, weights, params=None, **kw):
@@ -207,16 +208,20 @@ def assert_tiers_ran(stats, g, thr=UINT32_MAX):
     assert ran == expect, (ran, expect)
 
 
-def run_cluster(g, seed, mcw, mnn=UINT32_MAX, thr=UINT32_MAX, passes=1):
+def run_cluster(g, seed, mcw, mnn=UINT32_MAX, thr=UINT32_MAX, passes=1, subrounds=8, granule_log2=4,
+                oracle_subrounds=None):
+    """oracle_subrounds: the oracle's sub-round count where it differs from the engine's (default: the same)"""
     ctx, _ = ctx_for(g, 8, seed)
     ctx.coarsening.clustering.lp.max_num_neighbors = mnn
     ctx.coarsening.clustering.lp.large_degree_threshold = thr
     ctx.engine.cluster_commit_passes = passes
+    ctx.engine.sync_subrounds, ctx.engine.sync_granule_log2 = subrounds, granule_log2
     clusterer = lp.LPClustering(ctx.coarsening, ctx.engine)
     clusterer.set_max_cluster_weight(mcw)
     c = clusterer.compute_clustering(g)
-    expect, st = B.oracle_lp_cluster(g, seed, mcw, schedule=B.SYNC, params=oracle_params(0, mnn, thr, passes),
-                                     return_stats=True)
+    params = oracle_params(0, mnn, thr, passes, subrounds if oracle_subrounds is None else oracle_subrounds,
+                           granule_log2)
+    expect, st = B.oracle_lp_cluster(g, seed, mcw, schedule=B.SYNC, params=params, return_stats=True)
     assert np.array_equal(c, expect)
     gs = clusterer.last_stats
     assert gs.moved_list() == list(st[0].moved[: st[0].iterations])
@@ -226,18 +231,26 @@ def run_cluster(g, seed, mcw, mnn=UINT32_MAX, thr=UINT32_MAX, passes=1):
     return gs
 
 
-def run_refine(g, seed, k, part, mbw, mnn=UINT32_MAX, thr=UINT32_MAX, passes=4):
+def run_refine(g, seed, k, part, mbw, mnn=UINT32_MAX, thr=UINT32_MAX, passes=4, subrounds=8, granule_log2=4,
+               min_bw=None, expect=None):
+    """expect: the oracle's (partition, block weights, stats) of this call when the caller already has them"""
     ctx, _ = ctx_for(g, k, seed)
     ctx.refinement.lp.max_num_neighbors = mnn
     ctx.refinement.lp.large_degree_threshold = thr
     ctx.engine.refine_commit_passes = passes
+    ctx.engine.sync_subrounds, ctx.engine.sync_granule_log2 = subrounds, granule_log2
     ctx.partition.setup(g, [int(x) for x in mbw])
+    if min_bw is not None:
+        ctx.partition.setup_min_block_weights([int(x) for x in min_bw])
     p_graph = lp.PartitionedGraph(g, k, part)
     refiner = lp.LabelPropagationRefiner(ctx)
     refiner.initialize(p_graph)
     refiner.refine(p_graph, ctx.partition)
-    ep, ebw, st = B.oracle_lp_refine(g, seed, k, mbw, part, schedule=B.SYNC, params=oracle_params(1, mnn, thr, passes),
-                                     return_stats=True)
+    if expect is None:
+        expect = B.oracle_lp_refine(g, seed, k, mbw, part, schedule=B.SYNC,
+                                    params=oracle_params(1, mnn, thr, passes, subrounds, granule_log2),
+                                    min_block_weights=min_bw, return_stats=True)
+    ep, ebw, st = expect
     assert np.array_equal(p_graph.partition, ep)
     assert np.array_equal(p_graph.block_weights(), ebw)
     gs = refiner.last_stats
