@@ -108,8 +108,8 @@ typedef struct {
   uint64_t group_edges[12];
   uint64_t group_nodes[12];
   uint64_t group_launches[12];
-  float group_sweep_ms[16];  /* only when timing is enabled: [0..11] sweep tiers, [12] commit-rule kernels,
-                              * [13] apply, [14] push activation, [15] stamp ageing */
+  float group_sweep_ms[16];  /* only when timing is enabled: [0..11] sweep tiers, [12] commits,
+                              * [13] reserved (0), [14] push activation, [15] stamp ageing */
   uint32_t pull_rounds;      /* LP rounds whose sweeps derived the active flags from the move stamps */
   uint32_t push_rounds;      /* LP rounds in which movers flagged their neighbours */
 } kmp_lp_stats;
@@ -126,8 +126,7 @@ void kmp_lp_default_config(int mode, kmp_lp_config *cfg);
  * kmp_lp_create: KMP_HUB_WAVE_SLOTS = 8-byte bucket entries one wave of high-degree vertices may use (default 2^28 =
  * 2 GiB; smaller values process a sub-round's hubs in more waves), KMP_HUB_BUCKET_CAP / KMP_HUB_SEL_LIMIT = smaller
  * bucket capacity / claim limit of the hub tier (force its overflow list and multi-pass selection),
- * KMP_THREAD_MAX_DEG = 16 sends degrees 17..31 to the warp kernel instead of the register-sort kernel,
- * KMP_FUSED_COMMIT=0, KMP_OVERLAP_TIERS=0, KMP_FORCE_P64=1, KMP_UPLOAD_OVERLAP=0 (launch structure / word width),
+ * KMP_FORCE_P64=1 (8-byte gather words at any label count),
  * KMP_GRID_CAP = N caps the CTA count of every launch inside an LP round at N (small inputs then take every
  * grid-stride loop and work-queue refill several times).
  * Read per call: KMP_ACTIVATION=push|pull, KMP_TRACE=1 (set_graph stage times on stderr). */

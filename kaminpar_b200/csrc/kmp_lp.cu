@@ -64,7 +64,7 @@ constexpr uint32_t kHubMinDegreeUnit = 16384;  // unit edge weights: 16-bit rati
 constexpr int kSMs = 132; // H100 SXM: caps the grid-stride launches at a few waves of the device
 constexpr uint32_t kMaxHubWaves = 448; // work-queue cursors ctr32[64 .. 512), overflow counters ctr32[512 .. 960)
 constexpr uint32_t kCtr32Size = 1024;
-constexpr int kTagCommit = 12, kTagApply = 13, kTagPush = 14, kTagMisc = 15; // timing slots besides the tiers
+constexpr int kTagCommit = 12, kTagPush = 14, kTagMisc = 15; // timing slots besides the tiers; 13 is reserved
 
 // kernel tier of a vertex of degree d >= 1
 __host__ __device__ inline uint32_t tier_of(uint32_t d, uint32_t hub_min) {
@@ -118,14 +118,12 @@ struct kmp_lp_handle {
   cudaStream_t sweep_stream = nullptr; // stream the running sweep launch goes to
   cudaStream_t side_stream[3] = {nullptr, nullptr, nullptr};
   cudaEvent_t ev_fork = nullptr, ev_join[3] = {nullptr, nullptr, nullptr};
-  bool overlap_tiers = true;
   cudaEvent_t ev_begin = nullptr, ev_end = nullptr;
   cudaEvent_t ev_ct0 = nullptr, ev_ct1 = nullptr; // contraction timing (kmp_contract.cuh), created on first use
   bool timing = false;
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> sweep_events;
   std::vector<int> sweep_event_group;
   uint64_t group_launches[kStatTiers] = {};
-  uint32_t thread_max_deg = 32; // KMP_THREAD_MAX_DEG: 16 / 32 (which tiers run the register-sort kernel)
   uint32_t grid_cap = 0;        // KMP_GRID_CAP: most CTAs of any launch inside an LP round (0: no cap)
   // packed (label, stamp) gather array of the sweeps (lp_device.cuh): 4 B per vertex while labels fit 24 bits
   // (n <= 2^24 clusterer / k <= 2^24 refiner), else 8 B
@@ -225,13 +223,11 @@ struct kmp_lp_handle {
   DevBuf<uint32_t> dist_send, dist_recv;
   uint32_t *direct_send = nullptr; // set while the sweeps of a sharded sub-round write into the send buffer
   uint32_t direct_cap = 0;
-  // cooperative single-launch commit of the clusterer (lp_commit.cuh commit_cluster_fused)
+  // cooperative single-launch commit of a sub-round (lp_commit.cuh commit_cluster_fused / commit_refine_fused)
   DevBuf<unsigned> grid_bar; // [0] arrivals, [1] generation
-  int fused_blocks = 0;      // co-resident CTAs of the fused kernel (0: not available)
-  int fused_blocks_refine = 0;
-  bool fused_commit = true;
-  // co-resident CTAs of the persistent kernels of degree groups 0 and 1 (lp_lowgroup.cuh), [group][EW][P64];
-  // 0: no cooperative launch on this device (the per-sub-round path runs instead)
+  int fused_blocks = 0;      // co-resident CTAs of the clusterer's kernel
+  int fused_blocks_refine = 0; // of the refiner's kernel with its largest dynamic shared memory
+  // co-resident CTAs of the persistent kernels of degree groups 0 and 1 (lp_lowgroup.cuh), [group][EW][P64]
   uint32_t low_blocks[2][2][2] = {};
   // resident CTAs of each sweep_team instantiation on the device, [MODE][EW][P64][team size 32 / 128 / 512 / 1024]:
   // a larger grid only adds CTAs that start after the work queue is drained
@@ -243,7 +239,6 @@ struct kmp_lp_handle {
   int32_t step_mcw = 0;
   bool step_has_min = false, step_has_comm = false;
   uint32_t mover_parity = 0; // proposal counter in use: ctr32[0] (parity 0) or ctr32[3] (parity 1)
-  bool step_accumulated = false; // kmp_lp_step_commit already ran k_accumulate_movers for this sub-round
   bool stepping = false; // proposals are accumulated by kmp_lp_step_commit, not by the sweep kernels
 };
 
@@ -553,60 +548,6 @@ __global__ void k_pack_movers(const uint32_t *mv_u, const uint32_t *mv_t, const 
     buf[4 + cap + i] = mv_t[i];
   }
 }
-// concatenate the proposals of all ranks (rank order) into mv_u / mv_t
-__global__ void k_unpack_movers(const uint32_t *gathered, uint32_t world, uint32_t cap, uint32_t *mv_u, uint32_t *mv_t,
-                                uint32_t *count) {
-  const uint32_t stride = 4 + 2 * cap;
-  uint32_t total = 0;
-  for (uint32_t r = 0; r < world; ++r) {
-    const uint32_t cnt = gathered[static_cast<size_t>(r) * stride];
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < cnt; i += gridDim.x * blockDim.x) {
-      mv_u[total + i] = gathered[static_cast<size_t>(r) * stride + 4 + i];
-      mv_t[total + i] = gathered[static_cast<size_t>(r) * stride + 4 + cap + i];
-    }
-    total += cnt;
-  }
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
-    *count = total;
-  }
-}
-// incoming[] / hist[] over the gathered proposals (the sweep kernels skip it when world > 1)
-template <int MODE>
-__global__ void k_accumulate_movers(const uint32_t *mv_u, const uint32_t *mv_t, const uint32_t *count,
-                                    const int32_t *vwgt, uint32_t base_commit, int32_t *incoming, int32_t *hist,
-                                    uint32_t k) {
-  extern __shared__ int32_t s_hist[];
-  const bool priv = (MODE == 1) && k * kLadderLevels <= kSmemPrivLimit;
-  if (priv) {
-    for (uint32_t b = threadIdx.x; b < k * kLadderLevels; b += blockDim.x) {
-      s_hist[b] = 0;
-    }
-    __syncthreads();
-  }
-  const uint32_t cnt = *count;
-  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < cnt; i += gridDim.x * blockDim.x) {
-    const uint32_t u = mv_u[i];
-    const int32_t w = vwgt != nullptr ? vwgt[u] : 1;
-    if (MODE == 0) {
-      atomicAdd(&incoming[mv_t[i]], w);
-    } else {
-      const uint32_t slot = mv_t[i] * kLadderLevels + ladder_level(bijective32(u, base_commit));
-      if (priv) {
-        atomicAdd(&s_hist[slot], w);
-      } else {
-        atomicAdd(&hist[slot], w);
-      }
-    }
-  }
-  if (priv) {
-    __syncthreads();
-    for (uint32_t b = threadIdx.x; b < k * kLadderLevels; b += blockDim.x) {
-      if (s_hist[b] != 0) {
-        atomicAdd(&hist[b], s_hist[b]);
-      }
-    }
-  }
-}
 // favored fix-up across ranks: only the owner of u ever writes favored[u] (initially u)
 __global__ void k_xor_iota(uint32_t n, const uint32_t *in, uint32_t *out) {
   for (uint32_t u = blockIdx.x * blockDim.x + threadIdx.x; u < n; u += gridDim.x * blockDim.x) {
@@ -677,12 +618,8 @@ template <int MODE, bool EW, bool P64> cudaError_t launch_sweep_t(kmp_lp_handle 
   case 1: // deg 8..16
     sweep_thread<MODE, EW, P64, 16><<<tgrid, 256, 0, h->sweep_stream>>>(a);
     break;
-  case 2: // deg 17..31 (KMP_THREAD_MAX_DEG=16 sends them to the warp-team kernel instead: experiments)
-    if (h->thread_max_deg >= 32) {
-      sweep_thread<MODE, EW, P64, 32><<<tgrid, 256, 0, h->sweep_stream>>>(a);
-    } else {
-      launch_team<MODE, EW, P64, 32, 512, 8>(h, a);
-    }
+  case 2: // deg 17..31
+    sweep_thread<MODE, EW, P64, 32><<<tgrid, 256, 0, h->sweep_stream>>>(a);
     break;
   case 3: // deg 32..255: one warp per vertex, 512 slots (a 64-register sort was slower here: 230 registers, one CTA per SM)
     launch_team<MODE, EW, P64, 32, 512, 8>(h, a);
@@ -747,7 +684,7 @@ template <int MODE, bool EW, bool P64> cudaError_t launch_sweep_t(kmp_lp_handle 
 }
 
 // timing mode: bracket a section of the stream with an event pair tagged with a stats slot
-// (0..4 sweep tiers, 5 commit-rule kernels, 6 apply + activate)
+// (0..7 sweep tiers, kTagCommit commits, kTagPush push activation, kTagMisc stamp ageing)
 int timed_begin(kmp_lp_handle *h, int tag, cudaStream_t st = nullptr) {
   if (!h->timing) {
     return -1;
@@ -1185,7 +1122,7 @@ int sweep_subround(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t s
   sa.base_tie = sync_base(h->cfg.seed, h->call_counter, iter, SALT_TIE);
   sa.base_fav = sync_base(h->cfg.seed, h->call_counter, iter, SALT_FAV);
   sa.base_commit = sync_base(h->cfg.seed, h->call_counter, iter * 4096 + sg, SALT_COMMIT);
-  sa.accumulate = !h->stepping && rc.mode == 0; // refiner: accumulated by k_accumulate_movers (privatised)
+  sa.accumulate = !h->stepping && rc.mode == 0; // refiner: commit_refine_fused builds the level histograms
   sa.pull = h->pull_this;
   sa.window = make_window(iter, sg);
   h->cur_subround = q.sr;
@@ -1196,7 +1133,7 @@ int sweep_subround(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t s
   }
   // several tiers in this sub-round: fork them onto side streams (per-tier timing mode keeps them serial so
   // that every tier's CUDA-event time is its own)
-  const bool fork = live > 1 && h->overlap_tiers && !h->timing;
+  const bool fork = live > 1 && !h->timing;
   if (fork) {
     KMP_CUDA(cudaEventRecord(h->ev_fork, h->stream));
   }
@@ -1230,11 +1167,6 @@ int sweep_subround(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t s
   return KMP_OK;
 }
 
-// clusterer, pull activation: the whole commit in one cooperative launch (gathered != nullptr: the sharded run's
-// all-gathered proposal buffers are unpacked and accumulated by the same launch)
-bool can_fuse_commit(const kmp_lp_handle *h, const RunCtx &rc) {
-  return h->fused_commit && (rc.mode == 0 ? h->fused_blocks : h->fused_blocks_refine) > 0;
-}
 // push activation (rounds with few movers): flags for the neighbours of the accepted movers; reads acc[] / mv_u[]
 void launch_push_activation(kmp_lp_handle *h, const CommitArgs &ca, const SubRound &q) {
   const uint32_t size = q.total;
@@ -1248,8 +1180,12 @@ void launch_push_activation(kmp_lp_handle *h, const CommitArgs &ca, const SubRou
   timed_end(h, ev);
   ++h->kernel_launches;
 }
-int commit_subround_fused(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t sg, const SubRound &q,
-                          const uint32_t *gathered) {
+// The whole commit of sub-round sg in one cooperative launch, over the proposals in mv_u / mv_t -- or, with
+// gathered != nullptr, over the all-gathered proposal buffers (world * (4 + 2 * cap) words) of a sharded run or of
+// the stepping API, which the same launch unpacks and accumulates first. Every rank runs the same
+// order-independent commit on the same proposals, so the replicas stay bit-identical.
+int commit_subround(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t sg, const SubRound &q,
+                    const uint32_t *gathered) {
   CommitArgs ca = make_commit_args(h, rc);
   ca.base_commit = sync_base(h->cfg.seed, h->call_counter, iter * 4096 + sg, SALT_COMMIT);
   ca.stamp = h->stamps_ok ? make_stamp(iter, sg) : 0;
@@ -1272,99 +1208,23 @@ int commit_subround_fused(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uin
       KMP_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void *>(commit_refine_fused<false>), dim3(blocks), dim3(256), rargs,
                                            smem, h->stream));
     }
-    timed_end(h, ev);
-    ++h->kernel_launches;
-    if (!h->pull_this || !h->pull_next) {
-      launch_push_activation(h, ca, q); // acc[] / mv_u[] still hold this sub-round's verdicts
-    }
-    h->mover_parity ^= 1u;
-    return KMP_OK;
-  }
-  const uint32_t blocks = capped(h, std::min<uint32_t>(grid_for(q.total, 256), static_cast<uint32_t>(h->fused_blocks)));
-  void *args[] = {&ca, &ga, &bar};
-  if (h->p64) {
-    KMP_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void *>(commit_cluster_fused<true>), dim3(blocks), dim3(256), args, 0,
-                                         h->stream));
   } else {
-    KMP_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void *>(commit_cluster_fused<false>), dim3(blocks), dim3(256), args,
-                                         0, h->stream));
+    const uint32_t blocks = capped(h, std::min<uint32_t>(grid_for(q.total, 256), static_cast<uint32_t>(h->fused_blocks)));
+    void *args[] = {&ca, &ga, &bar};
+    if (h->p64) {
+      KMP_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void *>(commit_cluster_fused<true>), dim3(blocks), dim3(256), args, 0,
+                                           h->stream));
+    } else {
+      KMP_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void *>(commit_cluster_fused<false>), dim3(blocks), dim3(256), args,
+                                           0, h->stream));
+    }
   }
   timed_end(h, ev);
   ++h->kernel_launches;
   if (!h->pull_this || !h->pull_next) {
-    launch_push_activation(h, ca, q);
+    launch_push_activation(h, ca, q); // acc[] / mv_u[] still hold this sub-round's verdicts
   }
   h->mover_parity ^= 1u;
-  return KMP_OK;
-}
-
-// commit kernels of one sub-round over the proposals in mv_u / mv_t (count in ctr32[0])
-int commit_subround(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t sg, const SubRound &q) {
-  if (!h->step_accumulated && can_fuse_commit(h, rc)) {
-    return commit_subround_fused(h, rc, iter, sg, q, nullptr);
-  }
-  CommitArgs ca = make_commit_args(h, rc);
-  ca.base_commit = sync_base(h->cfg.seed, h->call_counter, iter * 4096 + sg, SALT_COMMIT);
-  ca.stamp = h->stamps_ok ? make_stamp(iter, sg) : 0;
-  const uint32_t size = q.total;
-  const uint32_t passes = std::max<uint32_t>(1, h->cfg.sync_commit_passes);
-  const uint32_t cgrid = capped(h, grid_for(size, 256, kSMs * 8));
-  int ev = timed_begin(h, kTagCommit);
-  if (rc.mode == 0) {
-    commit_cluster_classify<<<cgrid, 256, 0, h->stream>>>(ca);
-    commit_cluster_decide<<<cgrid, 256, 0, h->stream>>>(ca);
-    h->kernel_launches += 2;
-  } else {
-    const uint32_t kgrid = capped(h, grid_for(rc.num_labels, 128));
-    const size_t smem_k = rc.num_labels <= kSmemPrivLimit ? static_cast<size_t>(rc.num_labels) * 4 : 0;
-    if (!h->step_accumulated) { // level histograms over all proposals (the stepping path did it already)
-      const size_t smem_h = rc.num_labels * kLadderLevels <= kSmemPrivLimit ? static_cast<size_t>(rc.num_labels) * kLadderLevels * 4 : 0;
-      k_accumulate_movers<1><<<cgrid, 256, smem_h, h->stream>>>(h->mv_u.p, h->mv_t.p, h->ctr32.p + (h->mover_parity ? 3 : 0),
-                                                               h->vwgt, ca.base_commit, h->incoming.p, h->hist.p, rc.num_labels);
-      ++h->kernel_launches;
-    }
-    commit_begin<<<cgrid, 256, 0, h->stream>>>(h->acc.p, h->ctr32.p + (h->mover_parity ? 3 : 0));
-    commit_refine_prepare<<<kgrid, 128, 0, h->stream>>>(ca);
-    for (uint32_t p = 0; p < passes; ++p) {
-      commit_refine_jmin<<<kgrid, 128, 0, h->stream>>>(ca);
-      commit_refine_decide<<<cgrid, 256, smem_k, h->stream>>>(ca);
-    }
-    h->kernel_launches += 2 + 2 * passes;
-    if (rc.has_min) {
-      commit_refine_ohist<<<cgrid, 256, 0, h->stream>>>(ca);
-      commit_refine_ojmin<<<kgrid, 128, 0, h->stream>>>(ca);
-      commit_refine_othin<<<cgrid, 256, 0, h->stream>>>(ca);
-      h->kernel_launches += 3;
-    }
-    commit_refine_reset<<<capped(h, grid_for(static_cast<uint64_t>(rc.num_labels) * kLadderLevels, 128)), 128, 0, h->stream>>>(ca);
-    h->kernel_launches += 1;
-  }
-  timed_end(h, ev);
-  if (!h->pull_this || !h->pull_next) {
-    launch_push_activation(h, ca, q);
-  }
-  ev = timed_begin(h, kTagApply);
-  {
-    const size_t smem_k = (rc.mode == 1 && rc.num_labels <= kSmemPrivLimit) ? static_cast<size_t>(rc.num_labels) * 4 : 0;
-    const uint32_t agrid = capped(h, grid_for(size, 256, kSMs * 4));
-    if (rc.mode == 0) {
-      if (h->p64) {
-        commit_apply<0, true><<<agrid, 256, 0, h->stream>>>(ca);
-      } else {
-        commit_apply<0, false><<<agrid, 256, 0, h->stream>>>(ca);
-      }
-    } else {
-      if (h->p64) {
-        commit_apply<1, true><<<agrid, 256, smem_k, h->stream>>>(ca);
-      } else {
-        commit_apply<1, false><<<agrid, 256, smem_k, h->stream>>>(ca);
-      }
-    }
-  }
-  timed_end(h, ev);
-  h->kernel_launches += 1;
-  h->mover_parity ^= 1u;
-  KMP_CUDA(cudaGetLastError());
   return KMP_OK;
 }
 
@@ -1499,34 +1359,6 @@ int dist_sweep_pack(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t 
   return KMP_OK;
 }
 
-// Commit sub-round sg from the all-gathered proposal buffers (world * (4 + 2 * cap) words): every rank runs
-// the same order-independent commit on the same proposals, so the replicas stay bit-identical.
-int dist_unpack_commit(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t sg, const SubRound &q,
-                       const uint32_t *d_gathered) {
-  if (can_fuse_commit(h, rc)) {
-    return commit_subround_fused(h, rc, iter, sg, q, d_gathered);
-  }
-  const uint32_t cap = subround_cap(h, q);
-  const uint32_t base_commit = sync_base(h->cfg.seed, h->call_counter, iter * 4096 + sg, SALT_COMMIT);
-  k_unpack_movers<<<capped(h, grid_for(cap, 256, kSMs * 4)), 256, 0, h->stream>>>(d_gathered, h->world, cap, h->mv_u.p, h->mv_t.p,
-                                                                        h->ctr32.p + (h->mover_parity ? 3 : 0));
-  const uint32_t agrid = capped(h, grid_for(q.total, 256, kSMs * 8));
-  if (rc.mode == 0) {
-    k_accumulate_movers<0><<<agrid, 256, 0, h->stream>>>(h->mv_u.p, h->mv_t.p, h->ctr32.p + (h->mover_parity ? 3 : 0), h->vwgt,
-                                                          base_commit, h->incoming.p, h->hist.p, rc.num_labels);
-  } else {
-    const size_t smem_h = rc.num_labels * kLadderLevels <= kSmemPrivLimit ? static_cast<size_t>(rc.num_labels) * kLadderLevels * 4 : 0;
-    k_accumulate_movers<1><<<agrid, 256, smem_h, h->stream>>>(h->mv_u.p, h->mv_t.p, h->ctr32.p + (h->mover_parity ? 3 : 0), h->vwgt,
-                                                               base_commit, h->incoming.p, h->hist.p, rc.num_labels);
-  }
-  h->kernel_launches += 2;
-  KMP_CUDA(cudaGetLastError());
-  h->step_accumulated = true;
-  const int r2 = commit_subround(h, rc, iter, sg, q);
-  h->step_accumulated = false;
-  return r2;
-}
-
 // ---- degree groups 0 and 1 of a clustering round: one persistent cooperative launch each (lp_lowgroup.cuh) ----
 template <bool EW, bool P64> const void *low_group_kernel_t(int group) {
   return group == 0 ? reinterpret_cast<const void *>(sweep_commit_low<EW, P64, 8, 8, 4>)
@@ -1536,7 +1368,7 @@ const void *low_group_kernel(bool ew, bool p64, int group) {
   return ew ? (p64 ? low_group_kernel_t<true, true>(group) : low_group_kernel_t<true, false>(group))
             : (p64 ? low_group_kernel_t<false, true>(group) : low_group_kernel_t<false, false>(group));
 }
-// per device, from kmp_lp_create on a device with cooperative launches: false if a kernel cannot be resident
+// per device, from kmp_lp_create: false if a kernel cannot be resident
 bool configure_low_groups(kmp_lp_handle *h, int sms) {
   for (int g = 0; g < 2; ++g) {
     for (int ew = 0; ew < 2; ++ew) {
@@ -1552,11 +1384,10 @@ bool configure_low_groups(kmp_lp_handle *h, int sms) {
   }
   return true;
 }
-// The clusterer on one GPU with the register-sort kernels in tiers 0..2; the sharded run, the refiner and the
-// stepping API keep the per-sub-round path (its commit is fused into one cooperative launch as well).
+// The clusterer on one GPU; the sharded run, the refiner and the stepping API keep the per-sub-round path (a sweep
+// launch and a commit launch per sub-round).
 bool can_run_low_groups(const kmp_lp_handle *h, const RunCtx &rc) {
-  return rc.mode == 0 && h->world == 1 && !h->stepping && h->fused_commit && h->low_blocks[0][0][0] > 0 &&
-         h->thread_max_deg >= 32;
+  return rc.mode == 0 && h->world == 1 && !h->stepping;
 }
 static_assert(kMaxSubrounds <= kLowMaxSubrounds, "ensure_lists admits more sub-rounds than LowGroupArgs holds");
 // All sub-rounds of degree group `group` (0: tier 0, 1: tiers 1-2) of LP round `iter`, in sub-round order, with the
@@ -1642,7 +1473,7 @@ int run_iteration(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t *m
         return rc2;
       }
       KMP_NCCL(g_nccl.AllGather(h->dist_send.p, h->dist_recv.p, words, ncclUint32, h->comm, h->stream));
-      rc2 = dist_unpack_commit(h, rc, iter, sg, q, h->dist_recv.p);
+      rc2 = commit_subround(h, rc, iter, sg, q, h->dist_recv.p);
       if (rc2 != KMP_OK) {
         return rc2;
       }
@@ -1660,7 +1491,7 @@ int run_iteration(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t *m
     if (rc2 != KMP_OK) {
       return rc2;
     }
-    rc2 = commit_subround(h, rc, iter, sg, q);
+    rc2 = commit_subround(h, rc, iter, sg, q, nullptr);
     if (rc2 != KMP_OK) {
       return rc2;
     }
@@ -2092,9 +1923,6 @@ int kmp_lp_create(const kmp_lp_config *cfg, kmp_lp_handle **out) {
   if (const char *e = std::getenv("KMP_HUB_SEL_LIMIT")) {
     h->hub_sel_limit = static_cast<uint32_t>(std::max(0, std::atoi(e)));
   }
-  if (const char *e = std::getenv("KMP_THREAD_MAX_DEG")) {
-    h->thread_max_deg = static_cast<uint32_t>(std::max(16, std::atoi(e)));
-  }
   if (const char *e = std::getenv("KMP_HUB_WAVE_SLOTS")) {
     h->hub_wave_slots = static_cast<uint64_t>(std::max(32ll, std::atoll(e)));
   }
@@ -2130,40 +1958,39 @@ int kmp_lp_create(const kmp_lp_config *cfg, kmp_lp_handle **out) {
     delete h;
     return fail(KMP_ERR_CUDA, "failed to create events");
   }
-  {
-    int coop = 0, per_sm = 0;
-    cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
-    if (coop != 0 &&
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, commit_cluster_fused<false>, 256, 0) == cudaSuccess &&
-        per_sm > 0 && h->grid_bar.ensure(2) == cudaSuccess && cudaMemset(h->grid_bar.p, 0, 2 * sizeof(unsigned)) == cudaSuccess) {
-      int sms = kSMs;
-      cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-      // all co-resident CTAs: a sub-round of a 10^8-vertex graph commits 10^7 proposals, each a short chain of
-      // dependent random accesses -- the grid is sized by the proposal count up to this limit
-      h->fused_blocks = sms * per_sm;
-      int per_sm_r = 0; // refiner kernel with its largest dynamic shared memory (kSmemPrivLimit ints)
-      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_r, commit_refine_fused<false>, 256, kSmemPrivLimit * 4) ==
-              cudaSuccess &&
-          per_sm_r > 0) {
-        h->fused_blocks_refine = sms * per_sm_r;
-      }
-      if (!configure_low_groups(h, sms)) {
-        delete h;
-        return fail(KMP_ERR_CUDA, "a persistent low-degree clustering kernel cannot be resident on this device");
-      }
-    }
-    if (const char *e = std::getenv("KMP_FUSED_COMMIT")) { // experiments / tests: 0 = separate commit kernels
-      h->fused_commit = std::atoi(e) != 0;
-    }
-  }
   if (const char *e = std::getenv("KMP_FORCE_P64")) {
     h->force_p64 = std::atoi(e) != 0;
   }
-  if (const char *e = std::getenv("KMP_OVERLAP_TIERS")) { // experiments: 0 = launch the tiers of a sub-round serially
-    h->overlap_tiers = std::atoi(e) != 0;
-  }
   int sms = kSMs;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  // every commit is a cooperative launch (grid barriers between its phases)
+  int coop = 0, per_sm = 0, per_sm_r = 0;
+  cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
+  if (coop == 0) {
+    delete h;
+    return fail(KMP_ERR_CUDA, "this device does not support cooperative launches");
+  }
+  // co-resident CTAs of both commit kernels, the refiner's with its largest dynamic shared memory (kSmemPrivLimit ints)
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, commit_cluster_fused<false>, 256, 0) != cudaSuccess ||
+      per_sm < 1 ||
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_r, commit_refine_fused<false>, 256, kSmemPrivLimit * 4) !=
+          cudaSuccess ||
+      per_sm_r < 1) {
+    delete h;
+    return fail(KMP_ERR_CUDA, "a fused commit kernel cannot be resident on this device");
+  }
+  if (h->grid_bar.ensure(2) != cudaSuccess || cudaMemset(h->grid_bar.p, 0, 2 * sizeof(unsigned)) != cudaSuccess) {
+    delete h;
+    return fail(KMP_ERR_CUDA, "failed to allocate the grid barrier");
+  }
+  // all co-resident CTAs: a sub-round of a 10^8-vertex graph commits 10^7 proposals, each a short chain of
+  // dependent random accesses -- the grid is sized by the proposal count up to this limit
+  h->fused_blocks = sms * per_sm;
+  h->fused_blocks_refine = sms * per_sm_r;
+  if (!configure_low_groups(h, sms)) {
+    delete h;
+    return fail(KMP_ERR_CUDA, "a persistent low-degree clustering kernel cannot be resident on this device");
+  }
   if (!(configure_team_kernels<0, false, false>(h, sms) && configure_team_kernels<0, false, true>(h, sms) &&
         configure_team_kernels<0, true, false>(h, sms) && configure_team_kernels<0, true, true>(h, sms) &&
         configure_team_kernels<1, false, false>(h, sms) && configure_team_kernels<1, false, true>(h, sms) &&
@@ -2261,11 +2088,7 @@ int kmp_lp_set_graph(kmp_lp_handle *h, uint32_t n, uint32_t m, const uint32_t *x
   // pass, three small host round trips) while the m-sized arrays are still crossing PCIe on a side stream
   KMP_CUDA(cudaStreamSynchronize(h->stream)); // earlier work may still read the old arrays
   KMP_CUDA(cudaMemcpyAsync(h->own_xadj.p, xadj, (static_cast<size_t>(n) + 1) * 4, cudaMemcpyHostToDevice, h->stream));
-  static const bool overlap_upload = [] { // experiments: KMP_UPLOAD_OVERLAP=0 copies everything on the handle's stream
-    const char *e = std::getenv("KMP_UPLOAD_OVERLAP");
-    return e == nullptr || std::atoi(e) != 0;
-  }();
-  cudaStream_t big = overlap_upload ? h->side_stream[0] : h->stream;
+  const cudaStream_t big = h->side_stream[0];
   if (m > 0) {
     KMP_CUDA(cudaMemcpyAsync(h->own_adjncy.p, adjncy, static_cast<size_t>(m) * 4, cudaMemcpyHostToDevice, big));
   }
@@ -2882,7 +2705,7 @@ int kmp_lp_step_commit(kmp_lp_handle *h, uint32_t iter, uint32_t sg, const void 
     return fail(KMP_ERR_INVALID, "bad argument");
   }
   const RunCtx rc{h->step_mode, h->step_labels, h->step_mcw, h->step_has_min, h->step_has_comm};
-  return dist_unpack_commit(h, rc, iter, sg, subround_of_sg(h, sg), static_cast<const uint32_t *>(d_gathered));
+  return commit_subround(h, rc, iter, sg, subround_of_sg(h, sg), static_cast<const uint32_t *>(d_gathered));
 }
 
 int kmp_lp_step_end_iteration(kmp_lp_handle *h, uint32_t *moved) {

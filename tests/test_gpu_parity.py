@@ -188,16 +188,19 @@ def test_t1_activation_mode_does_not_change_results(name, mode, monkeypatch):
     assert np.array_equal(p_graph.partition, ep) and np.array_equal(p_graph.block_weights(), ebw)
 
 
-@pytest.mark.parametrize("knob", ["KMP_FUSED_COMMIT=0", "KMP_OVERLAP_TIERS=0", "KMP_FORCE_P64=1"])
+@pytest.mark.parametrize("knob", ["timing", "KMP_FORCE_P64=1"])
 @pytest.mark.parametrize("name", ["rmat16_hubs", "rmat15_hubs_w", "road60"])
 def test_t1_launch_structure_knobs_do_not_change_results(name, knob, monkeypatch):
-    """The single cooperative commit launch (vs. classify / decide / apply kernels), the side-stream overlap of
-    the tiers of a sub-round and the width of the packed (label, stamp) gather word (8 bytes once n > 2^24, e.g. the
-    512^3 grid; forced here) are implementation choices only."""
-    monkeypatch.setenv(*knob.split("="))
+    """The side-stream overlap of the tiers of a sub-round (timing mode launches them serially, one event pair
+    each) and the width of the packed (label, stamp) gather word (8 bytes once n > 2^24, e.g. the 512^3 grid;
+    forced here) are implementation choices only."""
+    timing = knob == "timing"
+    if not timing:
+        monkeypatch.setenv(*knob.split("="))
     g = get_graph(name)
     ctx, mcw = ctx_for(g, 8, seed=4)
     clusterer = lp.LPClustering(ctx.coarsening, ctx.engine)
+    clusterer._handle.set_timing(timing)
     clusterer.set_max_cluster_weight(mcw)
     c = clusterer.compute_clustering(g)
     assert np.array_equal(c, B.oracle_lp_cluster(g, 4, mcw, schedule=B.SYNC))
@@ -205,6 +208,7 @@ def test_t1_launch_structure_knobs_do_not_change_results(name, knob, monkeypatch
     part = np.random.default_rng(9).integers(0, k, g.n).astype(np.uint32)
     p_graph = lp.PartitionedGraph(g, k, part)
     refiner = lp.LabelPropagationRefiner(ctx)
+    refiner._handle.set_timing(timing)
     refiner.initialize(p_graph)
     refiner.refine(p_graph, ctx.partition)
     rp = B.oracle_params(B.default_refine_params(), commit_passes=4)

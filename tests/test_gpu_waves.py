@@ -5,12 +5,13 @@ pass once a work list outgrows the launch's grid. The inputs of the other parity
 here the grids are made small instead (KMP_GRID_CAP) or the inputs large, and the sub-round count, a public
 setting, is varied. All of it is integer work: the GPU must equal the oracle's `sync` schedule bit for bit.
 
-W1  capped grids (KMP_GRID_CAP = 1, 2, 3 CTAs) on ladders, R-MAT, grid and road graphs; each case asserts from
-    the schedule's work lists that the loops it relies on take more than two passes
+W1  capped grids (KMP_GRID_CAP = 1, 2, 3 CTAs) on ladders, R-MAT, grid and road graphs, clustering through the
+    library and through the stepping API; each case asserts from the schedule's work lists that the loops it
+    relies on take more than two passes
 W2  sync_subrounds in {0, 1, .., 31} (0: the default 8; 32 is refused), granule_log2 in {0, 4, 12}: the small-group
     rule, move stamps only while 4 * S <= 64, the proposal-counter parity carried from group to group
-W3  the refiner's commit at k up to 40000 (shared-memory privatisation limits, per-block kernels at large k),
-    fused and separate commit kernels, the stepping API, min block weights
+W3  the refiner's commit at k up to 40000 (shared-memory privatisation limits, per-block loops at large k),
+    the stepping API, min block weights
 W4  production grids at a scale where lists exceed what an H100 holds resident (132 SMs x 2048 threads)
 """
 import ctypes as C
@@ -84,53 +85,78 @@ def random_refine(g, k, seed, subrounds=8, granule_log2=4):
 # ------------------------------------------------------------------------------------------------
 # W1: capped grids
 # ------------------------------------------------------------------------------------------------
-# graph, KMP_GRID_CAP, sync_subrounds, other knobs, the tiers (or 'g1') whose loops must take > 2 passes
+# graph, KMP_GRID_CAP, sync_subrounds, clustering driver, other knobs, the tiers (or 'g1') whose loops must take
+# > 2 passes. 'library' clusters through LPClustering: degree groups 0 and 1 run as one persistent launch each per
+# round. 'stepping' clusters through the stepping API at world 1: every sub-round is a sweep launch per tier
+# (sweep_thread in tiers 0..2) and a commit that unpacks the gathered proposals.
 W1 = [
-    ("grid20", 1, 8, {}, (0,)),
-    ("grid20", 3, 1, {"KMP_ACTIVATION": "push"}, (0,)),
-    ("road60", 2, 1, {"KMP_FUSED_COMMIT": "0"}, (0,)),
-    ("road60", 3, 1, {"KMP_FORCE_P64": "1"}, (0,)),
-    ("rmat16_hubs", 1, 8, {"KMP_ACTIVATION": "pull"}, (0, "g1", 3)),
-    ("rmat16_hubs", 2, 1, {"KMP_ACTIVATION": "push"}, (0, "g1", 3, 4)),
-    ("rmat16_hubs", 3, 1, {"KMP_FUSED_COMMIT": "0"}, (0, 1, 2, 3, 4)),
-    ("rmat16_hubs", 2, 1, {"KMP_THREAD_MAX_DEG": "16"}, (0, 1, 2, 3)),
-    ("rmat15_hubs_w", 1, 1, {"KMP_FORCE_P64": "1", "KMP_ACTIVATION": "push"}, (0, "g1", 3, 4)),
-    ("rmat15_hubs_w", 3, 1, {}, (0, "g1", 3)),
-    ("rmat15_hubs_w", 3, 1, {"KMP_FUSED_COMMIT": "0", "KMP_ACTIVATION": "pull"}, (0, 1, 2, 3)),
-    ("wide_unit", 2, 1, {"KMP_FUSED_COMMIT": "0", "KMP_ACTIVATION": "push"}, (0, 1)),
-    ("wide_unit", 3, 1, {"KMP_FORCE_P64": "1"}, (0, "g1")),
-    ("dense_w", 1, 8, {"KMP_FUSED_COMMIT": "0"}, (4,)),
-    ("dense_w", 3, 1, {"KMP_ACTIVATION": "push"}, (4,)),
+    ("grid20", 1, 8, "library", {}, (0,)),
+    ("grid20", 3, 1, "library", {"KMP_ACTIVATION": "push"}, (0,)),
+    ("road60", 2, 1, "stepping", {}, (0,)),
+    ("road60", 3, 1, "library", {"KMP_FORCE_P64": "1"}, (0,)),
+    ("rmat16_hubs", 1, 8, "library", {"KMP_ACTIVATION": "pull"}, (0, "g1", 3)),
+    ("rmat16_hubs", 2, 1, "library", {"KMP_ACTIVATION": "push"}, (0, "g1", 3, 4)),
+    ("rmat16_hubs", 3, 1, "stepping", {}, (0, 1, 2, 3, 4)),
+    ("rmat15_hubs_w", 1, 1, "library", {"KMP_FORCE_P64": "1", "KMP_ACTIVATION": "push"}, (0, "g1", 3, 4)),
+    ("rmat15_hubs_w", 3, 1, "library", {}, (0, "g1", 3)),
+    ("rmat15_hubs_w", 3, 1, "stepping", {"KMP_ACTIVATION": "pull"}, (0, 1, 2, 3)),
+    ("wide_unit", 2, 1, "stepping", {"KMP_ACTIVATION": "push"}, (0, 1)),
+    ("wide_unit", 3, 1, "library", {"KMP_FORCE_P64": "1"}, (0, "g1")),
+    ("dense_w", 1, 8, "stepping", {}, (4,)),
+    ("dense_w", 3, 1, "library", {"KMP_ACTIVATION": "push"}, (4,)),
 ]
 
 
 def w1_id(case):
-    name, cap, S, env, _ = case
-    return "-".join([name, f"cap{cap}", f"S{S}"] + [f"{k[4:].lower()}={v}" for k, v in env.items()])
+    name, cap, S, driver, env, _ = case
+    parts = [name, f"cap{cap}", f"S{S}"] + ([driver] if driver != "library" else [])
+    return "-".join(parts + [f"{k[4:].lower()}={v}" for k, v in env.items()])
+
+
+def stepping_cluster(g, seed, mcw, subrounds):
+    """Clustering through the stepping API at world 1 (ShardedLP + CudaBackend): labels, moves per round, edges and
+    vertices scanned equal the oracle's, as run_cluster checks for the library path"""
+    import torch
+
+    from kaminpar_b200.dist import CudaBackend, ShardedLP
+
+    ctx, _ = ctx_for(g, 8, seed)
+    ctx.engine.sync_subrounds = subrounds
+    h = lp.LPHandle(lp._cluster_config(ctx.coarsening.clustering.lp, ctx.engine))
+    try:
+        h.set_graph(g)
+        drv = ShardedLP(CudaBackend(h, torch.device("cuda", 0)), g.n, ctx.coarsening.clustering.lp.num_iterations, 0, 1)
+        c, moved, gs = drv.compute_clustering(mcw)
+    finally:
+        h.close()
+    expect, st = B.oracle_lp_cluster(g, seed, mcw, schedule=B.SYNC, params=oracle_params(0, subrounds=subrounds),
+                                     return_stats=True)
+    assert np.array_equal(c, expect)
+    assert list(moved) == list(st[0].moved[: st[0].iterations])
+    assert gs.edges_scanned == st[0].edges_scanned and gs.nodes_visited == st[0].nodes_visited
 
 
 @pytest.mark.parametrize("case", W1, ids=[w1_id(c) for c in W1])
 def test_w1_capped_grids(case, monkeypatch):
-    name, cap, S, env, relies = case
+    name, cap, S, driver, env, relies = case
     monkeypatch.setenv("KMP_GRID_CAP", str(cap))
     for key, value in env.items():
         monkeypatch.setenv(key, value)
     g = graph(name)
-    team_tier2 = env.get("KMP_THREAD_MAX_DEG") == "16"
     sizes = largest_lists(g, SEED, S, 4)
     for t in relies:
-        thread_loop = t == "g1" or t < 2 or (t == 2 and not team_tier2)
+        thread_loop = t == "g1" or t <= 2
         per_pass = cap * (CTA_THREADS if thread_loop else TEAMS_PER_CTA.get(t, 8))
         assert sizes[t] > 2 * per_pass, (t, sizes[t], per_pass)
     _, mcw = ctx_for(g, 8)
-    gs = run_cluster(g, SEED, mcw, subrounds=S)  # labels, moves per round, edges and vertices scanned
-    rounds = gs.iterations
-    assert rounds > 0
-    if env.get("KMP_FUSED_COMMIT") != "0" and not team_tier2:  # one persistent launch per low group and round
-        launches = [rounds if sizes[0] else 0, rounds if sizes["g1"] else 0]
+    if driver == "stepping":
+        stepping_cluster(g, SEED, mcw, S)
+    else:
+        gs = run_cluster(g, SEED, mcw, subrounds=S)  # labels, moves per round, edges and vertices scanned
+        rounds = gs.iterations
+        assert rounds > 0
+        launches = [rounds if sizes[0] else 0, rounds if sizes["g1"] else 0]  # one persistent launch per group, round
         assert list(gs.group_launches[:2]) == launches, list(gs.group_launches)
-    if team_tier2:
-        assert gs.group_launches[2] > 0 and gs.group_nodes[2] > 0  # tier 2 runs as a warp-team kernel
     random_refine(g, 8, SEED, subrounds=S)
 
 
@@ -206,8 +232,8 @@ def test_w2_more_than_31_subrounds_are_refused():
 # ------------------------------------------------------------------------------------------------
 # W3: the refiner's commit at large k
 # ------------------------------------------------------------------------------------------------
-# 512 / 8192: k * 16 and k ints of shared memory (kSmemPrivLimit); 16896: k * 16 = 2112 CTAs of 128 threads, the
-# largest grid of a per-block commit kernel; 40000: more than twice that
+# 512 / 8192: k * 16 and k ints of shared memory (kSmemPrivLimit); 16896: k * 16 = 2112 x 128 histogram entries;
+# 40000: more than twice that. The commit loops over blocks and histogram entries grid-stride, in several passes here.
 W3_KS = (512, 513, 8192, 8193, 16896, 16897, 40000)
 W3_SEED = 2
 
@@ -251,36 +277,28 @@ def w3_run(k, kind):
     return expect
 
 
-@pytest.mark.parametrize("fused", ["1", "0"])
 @pytest.mark.parametrize("k", W3_KS)
-def test_w3_refiner_at_large_k(k, fused, monkeypatch):
-    monkeypatch.setenv("KMP_FUSED_COMMIT", fused)
+def test_w3_refiner_at_large_k(k):
     w3_run(k, "random")
 
 
-@pytest.mark.parametrize("fused", ["1", "0"])
-def test_w3_blocks_past_the_reset_grid_stay_contended(fused, monkeypatch):
+def test_w3_blocks_past_the_reset_grid_stay_contended():
     """k = 16897: only block 16896 lies past the first 2112 x 128 histogram entries, and it is proposed into in every
     sub-round; a histogram left from an earlier sub-round would lower what it accepts."""
-    monkeypatch.setenv("KMP_FUSED_COMMIT", fused)
     w3_run(16897, "hot")
 
 
-@pytest.mark.parametrize("fused", ["1", "0"])
-def test_w3_min_block_weights_at_large_k(fused, monkeypatch):
-    monkeypatch.setenv("KMP_FUSED_COMMIT", fused)
+def test_w3_min_block_weights_at_large_k():
     w3_run(40000, "min")
 
 
-@pytest.mark.parametrize("fused", ["1", "0"])
-def test_w3_stepping_api_at_large_k(fused, monkeypatch):
-    """The stepping API at world 1 (ShardedLP + CudaBackend): proposals packed, unpacked and accumulated, then
-    committed by the fused kernel or the separate ones"""
+def test_w3_stepping_api_at_large_k():
+    """The stepping API at world 1 (ShardedLP + CudaBackend): proposals packed, then unpacked, accumulated and
+    committed by one cooperative launch"""
     import torch
 
     from kaminpar_b200.dist import CudaBackend, ShardedLP
 
-    monkeypatch.setenv("KMP_FUSED_COMMIT", fused)
     k = 40000
     g = grid64()
     part, mbw, _, (ep, ebw, st) = w3_expect(k, "random")
