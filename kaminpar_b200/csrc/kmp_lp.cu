@@ -240,6 +240,13 @@ struct kmp_lp_handle {
   bool step_has_min = false, step_has_comm = false;
   uint32_t mover_parity = 0; // proposal counter in use: ctr32[0] (parity 0) or ctr32[3] (parity 1)
   bool stepping = false; // proposals are accumulated by kmp_lp_step_commit, not by the sweep kernels
+  // overload balancer (kmp_balance.cuh): its own call counter, so that LP calls hash the same with or without it
+  uint32_t bal_calls = 0;
+  DevBuf<uint32_t> bal_cand, bal_under, bal_ctr32, bal_target, bal_lists, bal_sv_a, bal_sv_b, bal_blk;
+  DevBuf<int32_t> bal_over, bal_pbw, bal_wt, bal_prefix;
+  DevBuf<uint8_t> bal_flag;
+  DevBuf<float> bal_key;
+  DevBuf<unsigned long long> bal_ctrl, bal_sk_a, bal_sk_b;
 };
 
 namespace {
@@ -2459,6 +2466,18 @@ int kmp_lp_free_scratch(kmp_lp_handle *h) {
   h->ct_rank.release();
   h->ct_cl.release();
   h->ct_counter.release();
+  for (DevBuf<uint32_t> *b : {&h->bal_cand, &h->bal_under, &h->bal_ctr32, &h->bal_target, &h->bal_lists, &h->bal_sv_a,
+                              &h->bal_sv_b, &h->bal_blk}) {
+    b->release();
+  }
+  for (DevBuf<int32_t> *b : {&h->bal_over, &h->bal_pbw, &h->bal_wt, &h->bal_prefix}) {
+    b->release();
+  }
+  h->bal_flag.release();
+  h->bal_key.release();
+  h->bal_ctrl.release();
+  h->bal_sk_a.release();
+  h->bal_sk_b.release();
   {
     cudaMemPool_t pool = kmp_private_pool(h->device); // blocks cached for coarse graphs (kmp_contract.cuh)
     if (pool != nullptr) {
@@ -2778,3 +2797,4 @@ int kmp_lp_step_finish(kmp_lp_handle *h, uint32_t *labels_out, int32_t *block_we
 } // extern "C"
 
 #include "kmp_contract.cuh"
+#include "kmp_balance.cuh"

@@ -8,6 +8,8 @@ Same names, argument meaning and error behaviour as the reference:
   (kaminpar-shm/coarsening/clusterer.h:35-46, clustering/lp_clusterer.cc:376-399),
 * ``LabelPropagationRefiner(ctx)`` with ``initialize(p_graph)`` / ``refine(p_graph, p_ctx)``
   (kaminpar-shm/refinement/refiner.h:34-56, refinement/lp/lp_refiner.cc:357-376),
+* ``OverloadBalancer(ctx)`` with ``initialize(p_graph)`` / ``refine(p_graph, p_ctx)``
+  (refinement/balancer/overload_balancer.cc:40-160, include/kaminpar_b200_balancer.h),
 * ``PartitionContext.setup`` (kaminpar-shm/context.cc:27-70), ``compute_max_cluster_weight``
   (kaminpar-shm/coarsening/max_cluster_weights.h:17-46), ``create_default_context``
   (kaminpar-shm/presets.cc:109-450, LP fields only).
@@ -79,6 +81,22 @@ class KmpStats(C.Structure):
         return list(self.moved[: self.iterations])
 
 
+class KmpBalanceStats(C.Structure):  # include/kaminpar_b200_balancer.h
+    _fields_ = [
+        ("rounds", C.c_uint32),
+        ("moved", C.c_uint32 * 64),
+        ("overload_before", C.c_int64),
+        ("overload_after", C.c_int64),
+        ("candidates", C.c_uint64),
+        ("edges_scanned", C.c_uint64),
+        ("kernel_launches", C.c_uint64),
+        ("device_ms", C.c_float),
+    ]
+
+    def moved_list(self):
+        return list(self.moved[: self.rounds])
+
+
 def library_path() -> str:
     return _LIB_PATH
 
@@ -95,6 +113,9 @@ def load_library():
         lib = C.CDLL(_LIB_PATH)
         lib.kmp_last_error.restype = C.c_char_p
         lib.kmp_lp_labels_device.restype = C.c_void_p
+        for sym in ("kmp_overload_balance", "kmp_balance_select_all"):  # include/kaminpar_b200_balancer.h
+            if not hasattr(lib, sym):
+                raise RuntimeError(f"{_LIB_PATH} lacks {sym}; rebuild the library")
         if lib.kmp_lp_abi_version() != ABI_VERSION:  # the ctypes structs below mirror exactly this header version
             raise RuntimeError(f"{_LIB_PATH}: ABI version {lib.kmp_lp_abi_version()} != {ABI_VERSION}; rebuild the library")
         _lib = lib
@@ -228,6 +249,12 @@ class PartitionContext:
 
     def max_block_weights(self) -> np.ndarray:
         return np.asarray(self._max_block_weights, dtype=np.int32)
+
+    def perfectly_balanced_block_weight(self, b: int) -> int:  # kaminpar.h:436-438
+        return int(math.ceil(1.0 * self._unrelaxed[b] / (1 + self.inferred_epsilon())))
+
+    def perfectly_balanced_block_weights(self) -> np.ndarray:
+        return np.asarray([self.perfectly_balanced_block_weight(b) for b in range(self.k)], dtype=np.int32)
 
     def min_block_weight(self, b: int) -> int:
         return self._min_block_weights[b] if self._min_block_weights else 0
@@ -405,6 +432,31 @@ class LPHandle:
                                            _ptr(fav)))
         return tgt, fav
 
+    def overload_balance(self, k, max_block_weights, perfectly_balanced_block_weights, partition: Optional[np.ndarray]):
+        """kmp_overload_balance: partition (uint32, balanced in place) or None = the labels on the device.
+        Returns (improved, block_weights, stats)."""
+        stats = KmpBalanceStats()
+        mbw = np.ascontiguousarray(max_block_weights, np.int32)
+        pbw = np.ascontiguousarray(perfectly_balanced_block_weights, np.int32)
+        bw = np.zeros(k, np.int32)
+        improved = C.c_int(0)
+        if partition is not None:
+            assert partition.dtype == np.uint32 and partition.flags.c_contiguous
+        _check(self._lib.kmp_overload_balance(self._h, C.c_uint32(int(k)), _ptr(mbw), _ptr(pbw), _ptr(partition), _ptr(bw),
+                                              C.byref(improved), C.byref(stats)))
+        return bool(improved.value), bw, stats
+
+    def balance_select_all(self, k, labels, block_weights, max_block_weights, call_index=0, round=0):
+        """kmp_balance_select_all: (target[n] uint32, key[n] float32) against frozen state."""
+        labels = np.ascontiguousarray(labels, np.uint32)
+        bw = np.ascontiguousarray(block_weights, np.int32)
+        mbw = np.ascontiguousarray(max_block_weights, np.int32)
+        tgt = np.empty(self._n, np.uint32)
+        key = np.empty(self._n, np.float32)
+        _check(self._lib.kmp_balance_select_all(self._h, C.c_uint32(int(k)), _ptr(labels), _ptr(bw), _ptr(mbw),
+                                                C.c_uint32(call_index), C.c_uint32(round), _ptr(tgt), _ptr(key)))
+        return tgt, key
+
     def edge_cut(self) -> int:
         cut = C.c_int64(0)
         _check(self._lib.kmp_lp_edge_cut(self._h, C.byref(cut)))
@@ -512,3 +564,39 @@ class LabelPropagationRefiner:
         p_graph._block_weights = bw
         self.last_stats = stats
         return True  # lp_refiner.cc:88
+
+
+class OverloadBalancer:
+    """Drop-in for ``kaminpar::shm::OverloadBalancer : Refiner`` (overload_balancer.h, refiner.h:18-57) on the
+    device. Its selection rule is the reference's without thread order (DESIGN.md §11)."""
+
+    def __init__(self, ctx: Context):
+        self._ctx = ctx
+        self._handle = LPHandle(_refine_config(ctx.refinement.lp, ctx.engine))
+        self._graph = None
+        self.last_stats: Optional[KmpBalanceStats] = None
+
+    def name(self) -> str:
+        return "Overload Balancer"
+
+    def invalidate_graph(self):
+        self._graph = None
+
+    def initialize(self, p_graph: PartitionedGraph):
+        pass  # overload_balancer.cc:40-43: nothing until refine() finds an overloaded block
+
+    def refine(self, p_graph: PartitionedGraph, p_ctx: PartitionContext) -> bool:
+        assert p_graph.k() <= p_ctx.k
+        mbw = p_ctx.max_block_weights()
+        w = p_graph.block_weights().astype(np.int64)
+        if int(np.maximum(w - mbw[: len(w)], 0).sum()) == 0:  # metrics::total_overload == 0: no device work
+            self.last_stats = None
+            return False
+        if self._graph is not p_graph.graph:
+            self._handle.set_graph(p_graph.graph)
+            self._graph = p_graph.graph
+        improved, bw, stats = self._handle.overload_balance(p_ctx.k, mbw, p_ctx.perfectly_balanced_block_weights(),
+                                                            p_graph.partition)
+        p_graph._block_weights = bw
+        self.last_stats = stats
+        return improved
