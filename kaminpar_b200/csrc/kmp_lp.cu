@@ -603,7 +603,7 @@ bool configure_team(kmp_lp_handle *h, int sms) {
 // per device; called from kmp_lp_create
 template <int MODE, bool EW, bool P64> bool configure_team_kernels(kmp_lp_handle *h, int sms) {
   cudaFuncSetAttribute(sweep_hub_scatter<MODE, EW, P64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kHubScatterSmem);
-  bool ok = configure_team<MODE, EW, P64, 32, 512, 8>(h, sms) && configure_team<MODE, EW, P64, 128, 2048, 4>(h, sms) &&
+  bool ok = configure_team<MODE, EW, P64, 32, 512, 8, !EW>(h, sms) && configure_team<MODE, EW, P64, 128, 2048, 4>(h, sms) &&
             configure_team<MODE, EW, P64, 512, 8192, 1>(h, sms);
   if constexpr (EW) {
     ok = ok && configure_team<MODE, EW, P64, 1024, 16384, 1>(h, sms);
@@ -628,8 +628,9 @@ template <int MODE, bool EW, bool P64> cudaError_t launch_sweep_t(kmp_lp_handle 
   case 2: // deg 17..31
     sweep_thread<MODE, EW, P64, 32><<<tgrid, 256, 0, h->sweep_stream>>>(a);
     break;
-  case 3: // deg 32..255: one warp per vertex, 512 slots (a 64-register sort was slower here: 230 registers, one CTA per SM)
-    launch_team<MODE, EW, P64, 32, 512, 8>(h, a);
+  case 3: // deg 32..255: one warp per vertex, 512 slots (a 64-register sort was slower here: 230 registers, one CTA per SM);
+          // 16-bit ratings with unit edge weights (a rating is at most the degree), which leaves room for the claim lists
+    launch_team<MODE, EW, P64, 32, 512, 8, !EW>(h, a);
     break;
   case 4: // deg < 1024: 128 threads per vertex, 2048 slots
     launch_team<MODE, EW, P64, 128, 2048, 4>(h, a);
