@@ -2,6 +2,8 @@
 // error behaviour of the reference's plugin interfaces, so that
 //   kaminpar-shm/factories.cc:66-67   case ClusteringAlgorithm::LABEL_PROPAGATION  -> b200::LPClustering
 //   kaminpar-shm/factories.cc:108-109 case RefinementAlgorithm::LABEL_PROPAGATION  -> b200::LabelPropagationRefiner
+//   the OVERLOAD_BALANCER / UNDERLOAD_BALANCER cases                                 -> b200::OverloadBalancer /
+//                                                                                       b200::UnderloadBalancer
 // become one-line swaps (INTEGRATION.md shows the glue that maps kaminpar::shm::Graph /
 // PartitionedGraph / PartitionContext onto the views below).
 //
@@ -10,6 +12,8 @@
 //   class Refiner    kaminpar-shm/refinement/refiner.h:18-57
 //   LPClustering     kaminpar-shm/coarsening/clustering/lp_clusterer.h:19 / lp_clusterer.cc:376-399
 //   LabelPropagationRefiner  kaminpar-shm/refinement/lp/lp_refiner.h:19 / lp_refiner.cc:357-376
+//   OverloadBalancer   kaminpar-shm/refinement/balancer/overload_balancer.h / overload_balancer.cc:40-160
+//   UnderloadBalancer  kaminpar-shm/refinement/balancer/underload_balancer.h / underload_balancer.cc:27-104
 //   CoarseGraph / contract_clustering  kaminpar-shm/coarsening/contraction/cluster_contraction.h:22-56
 //
 // Error convention: the reference's path has no error codes (KASSERT aborts); here a non-zero
@@ -23,6 +27,7 @@
 #include <string>
 #include <vector>
 
+#include "kaminpar_b200_balancer.h"
 #include "kaminpar_b200_contraction.h"
 #include "kaminpar_b200_lp.h"
 
@@ -60,6 +65,7 @@ struct PartitionContextView {
   BlockID k = 0;
   std::span<const BlockWeight> max_block_weights; // max_block_weight(b)
   std::span<const BlockWeight> min_block_weights; // min_block_weight(b); empty -> 0
+  std::span<const BlockWeight> perfectly_balanced_block_weights; // perfectly_balanced_block_weight(b); OverloadBalancer
 };
 
 struct LabelPropagationCoarseningContext { // kaminpar.h:140-154, defaults presets.cc:140-153
@@ -234,6 +240,110 @@ private:
   detail::Handle _handle;
   std::span<const NodeID> _communities;
   kmp_lp_stats _stats{};
+};
+
+namespace detail {
+inline kmp_lp_config balancer_config(const EngineContext &e) {
+  kmp_lp_config cfg;
+  kmp_lp_default_config(1, &cfg);
+  cfg.seed = e.seed;
+  cfg.sync_subrounds = e.sync_subrounds;
+  cfg.sync_granule_log2 = e.sync_granule_log2;
+  cfg.device = e.device;
+  cfg.schedule = e.schedule;
+  return cfg;
+}
+inline void check_balancer_args(const PartitionedGraphView &p_graph, const PartitionContextView &p_ctx) {
+  if (p_graph.k > p_ctx.k || p_ctx.max_block_weights.size() != p_ctx.k ||
+      (!p_graph.block_weights.empty() && p_graph.block_weights.size() != p_ctx.k)) {
+    throw std::invalid_argument("kaminpar_b200: inconsistent k / max_block_weights / block_weights");
+  }
+}
+} // namespace detail
+
+// Same surface as kaminpar::shm::Refiner (refiner.h:34-56), OverloadBalancer::refine on the device (DESIGN.md §11).
+// Reads p_ctx.perfectly_balanced_block_weights (k entries). Returns false without device work when the block
+// weights (if given) show no overloaded block, like overload_balancer.cc:58-60.
+class OverloadBalancer {
+public:
+  explicit OverloadBalancer(const EngineContext &engine = {}) : _handle(detail::balancer_config(engine)) {}
+
+  [[nodiscard]] std::string name() const { return "Overload Balancer"; }
+  void initialize(const PartitionedGraphView &) {} // overload_balancer.cc:40-43
+
+  bool refine(PartitionedGraphView &p_graph, const PartitionContextView &p_ctx) {
+    detail::check_balancer_args(p_graph, p_ctx);
+    if (p_ctx.perfectly_balanced_block_weights.size() != p_ctx.k) {
+      throw std::invalid_argument("kaminpar_b200: perfectly_balanced_block_weights needs k entries");
+    }
+    if (!p_graph.block_weights.empty()) {
+      bool overloaded = false;
+      for (BlockID b = 0; b < p_ctx.k; ++b) {
+        overloaded = overloaded || p_graph.block_weights[b] > p_ctx.max_block_weights[b];
+      }
+      if (!overloaded) {
+        return false;
+      }
+    }
+    _handle.set_graph(p_graph.graph);
+    int improved = 0;
+    detail::check(kmp_overload_balance(_handle.get(), p_ctx.k, p_ctx.max_block_weights.data(),
+                                       p_ctx.perfectly_balanced_block_weights.data(), p_graph.partition.data(),
+                                       p_graph.block_weights.empty() ? nullptr : p_graph.block_weights.data(),
+                                       &improved, &_stats));
+    return improved != 0;
+  }
+  [[nodiscard]] const kmp_balance_stats &last_stats() const { return _stats; }
+  [[nodiscard]] kmp_lp_handle *handle() const { return _handle.get(); }
+  void invalidate_graph() { _handle.invalidate_graph(); }
+
+private:
+  detail::Handle _handle;
+  kmp_balance_stats _stats{};
+};
+
+// Same surface as kaminpar::shm::Refiner (refiner.h:34-56), UnderloadBalancer::refine on the device (DESIGN.md §12).
+// Returns false without device work when p_ctx has no minimum weights or the block weights (if given) are at or
+// above them, like underload_balancer.cc:47-50.
+class UnderloadBalancer {
+public:
+  explicit UnderloadBalancer(const EngineContext &engine = {}) : _handle(detail::balancer_config(engine)) {}
+
+  [[nodiscard]] std::string name() const { return "Underload Balancer"; }
+  void initialize(const PartitionedGraphView &) {} // underload_balancer.cc:35-37
+
+  bool refine(PartitionedGraphView &p_graph, const PartitionContextView &p_ctx) {
+    detail::check_balancer_args(p_graph, p_ctx);
+    if (p_ctx.min_block_weights.empty()) {
+      return false;
+    }
+    if (p_ctx.min_block_weights.size() != p_ctx.k) {
+      throw std::invalid_argument("kaminpar_b200: min_block_weights needs k entries");
+    }
+    if (!p_graph.block_weights.empty()) {
+      bool underloaded = false;
+      for (BlockID b = 0; b < p_ctx.k; ++b) {
+        underloaded = underloaded || p_graph.block_weights[b] < p_ctx.min_block_weights[b];
+      }
+      if (!underloaded) {
+        return false;
+      }
+    }
+    _handle.set_graph(p_graph.graph);
+    int improved = 0;
+    detail::check(kmp_underload_balance(_handle.get(), p_ctx.k, p_ctx.max_block_weights.data(),
+                                        p_ctx.min_block_weights.data(), p_graph.partition.data(),
+                                        p_graph.block_weights.empty() ? nullptr : p_graph.block_weights.data(),
+                                        &improved, &_stats));
+    return improved != 0;
+  }
+  [[nodiscard]] const kmp_underload_stats &last_stats() const { return _stats; }
+  [[nodiscard]] kmp_lp_handle *handle() const { return _handle.get(); }
+  void invalidate_graph() { _handle.invalidate_graph(); }
+
+private:
+  detail::Handle _handle;
+  kmp_underload_stats _stats{};
 };
 
 // Same surface as kaminpar::shm::CoarseGraph (cluster_contraction.h:22-32). The coarse graph lives on the

@@ -1,4 +1,4 @@
-/* kaminpar_b200 -- C ABI of the overload balancer on the device (H100, sm_90a).
+/* kaminpar_b200 -- C ABI of the overload and underload balancers on the device (H100, sm_90a).
  *
  *   kmp_overload_balance  <->  OverloadBalancer::refine(PartitionedGraph&, const PartitionContext&)
  *                              kaminpar-shm/refinement/balancer/overload_balancer.cc:51-160
@@ -63,6 +63,54 @@ int kmp_overload_balance(kmp_lp_handle *h, uint32_t k, const int32_t *max_block_
 int kmp_balance_select_all(kmp_lp_handle *h, uint32_t k, const uint32_t *labels, const int32_t *block_weights,
                            const int32_t *max_block_weights, uint32_t call_index, uint32_t round,
                            uint32_t *target_out, float *key_out);
+
+/* ---- underload balancer -------------------------------------------------------------------------------------
+ *
+ *   kmp_underload_balance  <->  UnderloadBalancer::refine(PartitionedGraph&, const PartitionContext&)
+ *                               kaminpar-shm/refinement/balancer/underload_balancer.cc:39-104
+ *
+ * The last stage of the default refinement chain: it moves vertices into blocks below their minimum weight
+ * (PartitionContext::min_block_weight), so that upload -> kmp_overload_balance -> kmp_lp_refine ->
+ * kmp_underload_balance -> download runs without a host copy between the stages.
+ *
+ * The rule is the reference's, restated without thread order (DESIGN.md §12): synchronous rounds against the block
+ * weights and underloaded flags frozen at the start of the round; a vertex may leave its block b iff b is not
+ * underloaded and W[b] - w(u) >= min[b]; its target is the best adjacent underloaded block with room; per target
+ * block the candidates are taken by (relative gain desc, vertex id asc) until its deficit min - W is covered; the
+ * moves are committed by the LP refiner's ladder with the minimum weights (one pass), so no block ends above its
+ * maximum and no block ends below its minimum because a vertex left it. Rounds stop when every block is at or above
+ * its minimum, when a round proposes no move, or after KMP_BALANCE_MAX_ROUNDS.
+ *
+ * Refused like kmp_overload_balance: seq_strict, sharded, NCCL and stepping handles (KMP_ERR_UNSUPPORTED); labels
+ * >= k (KMP_ERR_INVALID; checked before any label indexes a [k] array). */
+typedef struct kmp_underload_stats {
+  uint32_t rounds;           /* rounds executed (the last one may have accepted no move) */
+  uint32_t moved[64];        /* accepted moves per round */
+  int64_t underload_before;  /* sum over the blocks of max(0, min[b] - W[b]) before / after the call */
+  int64_t underload_after;
+  uint64_t candidates;       /* sum over the rounds of the vertices that may leave their block */
+  uint64_t edges_scanned;    /* their adjacency entries */
+  uint64_t kernel_launches;
+  float device_ms;           /* CUDA-event time of the whole call on the handle's stream */
+} kmp_underload_stats;
+
+/* UnderloadBalancer::refine on the graph the handle holds. partition_inout: HOST buffer of n BlockIDs, balanced in
+ * place, or NULL = the labels on the device (they stay there). max_block_weights[k], min_block_weights[k]
+ * (PartitionContext::min_block_weight). min_block_weights = NULL means the context has no minimum weights: then
+ * *improved_out = 0 and nothing runs on the device (block_weights_out is not written). block_weights_out[k]
+ * nullable, stats nullable. *improved_out = the reference's return value: 0 when every block is at or above its
+ * minimum (nothing is touched then), else 1. */
+int kmp_underload_balance(kmp_lp_handle *h, uint32_t k, const int32_t *max_block_weights,
+                          const int32_t *min_block_weights, uint32_t *partition_inout, int32_t *block_weights_out,
+                          int *improved_out, kmp_underload_stats *stats);
+
+/* T0 parity hook: target and key of EVERY vertex against frozen labels / block weights, as round `round` of call
+ * `call_index` would compute them; no moves. target_out[u] = labels[u] (key from gain INT32_MIN) when u may not
+ * leave its block or no adjacent underloaded block has room for it. HOST buffers. Like kmp_balance_select_all it
+ * overwrites the labels, block weights and maximum weights held on the device. */
+int kmp_underload_select_all(kmp_lp_handle *h, uint32_t k, const uint32_t *labels, const int32_t *block_weights,
+                             const int32_t *max_block_weights, const int32_t *min_block_weights, uint32_t call_index,
+                             uint32_t round, uint32_t *target_out, float *key_out);
 
 #ifdef __cplusplus
 }

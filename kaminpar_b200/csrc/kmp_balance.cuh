@@ -57,6 +57,7 @@ struct BalArgs {
   const uint32_t *__restrict__ label;
   const int32_t *__restrict__ weight; // [k], frozen
   const int32_t *__restrict__ max_w;  // [k]
+  const uint8_t *__restrict__ tmask;  // nullable: [k] the blocks a vertex may move to (underload balancer: W < min)
   uint32_t k;
   uint32_t base_tie;
   const uint32_t *__restrict__ cand;  // candidate i is vertex cand[i]
@@ -89,7 +90,7 @@ __device__ __forceinline__ bool bal_better(const BalBest &a, const BalBest &b) {
 }
 __device__ __forceinline__ void bal_offer(const BalArgs &a, uint32_t u, uint32_t own, int32_t uw, int32_t conn_own,
                                           uint32_t c, int32_t conn, BalBest &best) {
-  if (c == own || a.weight[c] + uw > a.max_w[c]) {
+  if (c == own || a.weight[c] + uw > a.max_w[c] || (a.tmask != nullptr && a.tmask[c] == 0)) {
     return;
   }
   const BalBest x{conn - conn_own, tie_hash(a.base_tie, u, c), c};
@@ -383,15 +384,16 @@ namespace {
 
 using namespace kmp;
 
-int bal_refuse(kmp_lp_handle *h) {
+int bal_refuse(kmp_lp_handle *h, const char *what = "the overload balancer", const char *section = "§11") {
   if (h == nullptr || !h->have_graph) {
     return fail(KMP_ERR_INVALID, "no graph set");
   }
   if (h->cfg.schedule == KMP_SCHEDULE_SEQ_STRICT) {
-    return fail(KMP_ERR_UNSUPPORTED, "the overload balancer has no seq_strict schedule (DESIGN.md §11)");
+    return fail(KMP_ERR_UNSUPPORTED, std::string(what) + " has no seq_strict schedule (DESIGN.md " + section + ")");
   }
   if (h->world > 1 || h->comm != nullptr || h->stepping || h->step_mode >= 0) {
-    return fail(KMP_ERR_UNSUPPORTED, "the overload balancer runs on one GPU: sharded, NCCL and stepping handles are refused");
+    return fail(KMP_ERR_UNSUPPORTED,
+                std::string(what) + " runs on one GPU: sharded, NCCL and stepping handles are refused");
   }
   return KMP_OK;
 }
@@ -420,8 +422,9 @@ int bal_ensure(kmp_lp_handle *h, uint32_t k, uint32_t nc) {
 }
 
 // Target and key of candidates cand[0 .. nc) against the frozen labels / weights on the device: three launches,
-// the thread tier hands the higher degrees to the warp and CTA tiers.
-int bal_evaluate(kmp_lp_handle *h, uint32_t k, uint32_t nc, uint32_t base_tie, bool sort_keys) {
+// the thread tier hands the higher degrees to the warp and CTA tiers. tmask (nullable, [k]): the allowed targets.
+int bal_evaluate(kmp_lp_handle *h, uint32_t k, uint32_t nc, uint32_t base_tie, bool sort_keys,
+                 const uint8_t *tmask = nullptr) {
   BalArgs a{};
   a.xadj = h->xadj;
   a.adjncy = h->adjncy;
@@ -430,6 +433,7 @@ int bal_evaluate(kmp_lp_handle *h, uint32_t k, uint32_t nc, uint32_t base_tie, b
   a.label = h->label.p;
   a.weight = h->weight.p;
   a.max_w = h->maxw.p;
+  a.tmask = tmask;
   a.k = k;
   a.base_tie = base_tie;
   a.cand = h->bal_cand.p;

@@ -247,6 +247,10 @@ struct kmp_lp_handle {
   DevBuf<uint8_t> bal_flag;
   DevBuf<float> bal_key;
   DevBuf<unsigned long long> bal_ctrl, bal_sk_a, bal_sk_b;
+  // underload balancer (kmp_underload.cuh): its own call counter; shares the overload balancer's scratch
+  uint32_t ubal_calls = 0;
+  DevBuf<int32_t> ubal_deficit;
+  DevBuf<uint8_t> ubal_tmask;
 };
 
 namespace {
@@ -2479,6 +2483,8 @@ int kmp_lp_free_scratch(kmp_lp_handle *h) {
   h->bal_ctrl.release();
   h->bal_sk_a.release();
   h->bal_sk_b.release();
+  h->ubal_deficit.release();
+  h->ubal_tmask.release();
   {
     cudaMemPool_t pool = kmp_private_pool(h->device); // blocks cached for coarse graphs (kmp_contract.cuh)
     if (pool != nullptr) {
@@ -2799,3 +2805,4 @@ int kmp_lp_step_finish(kmp_lp_handle *h, uint32_t *labels_out, int32_t *block_we
 
 #include "kmp_contract.cuh"
 #include "kmp_balance.cuh"
+#include "kmp_underload.cuh"

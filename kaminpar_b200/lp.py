@@ -10,6 +10,8 @@ Same names, argument meaning and error behaviour as the reference:
   (kaminpar-shm/refinement/refiner.h:34-56, refinement/lp/lp_refiner.cc:357-376),
 * ``OverloadBalancer(ctx)`` with ``initialize(p_graph)`` / ``refine(p_graph, p_ctx)``
   (refinement/balancer/overload_balancer.cc:40-160, include/kaminpar_b200_balancer.h),
+* ``UnderloadBalancer(ctx)`` with ``initialize(p_graph)`` / ``refine(p_graph, p_ctx)``
+  (refinement/balancer/underload_balancer.cc:35-104, include/kaminpar_b200_balancer.h),
 * ``PartitionContext.setup`` (kaminpar-shm/context.cc:27-70), ``compute_max_cluster_weight``
   (kaminpar-shm/coarsening/max_cluster_weights.h:17-46), ``create_default_context``
   (kaminpar-shm/presets.cc:109-450, LP fields only).
@@ -97,6 +99,22 @@ class KmpBalanceStats(C.Structure):  # include/kaminpar_b200_balancer.h
         return list(self.moved[: self.rounds])
 
 
+class KmpUnderloadStats(C.Structure):  # include/kaminpar_b200_balancer.h
+    _fields_ = [
+        ("rounds", C.c_uint32),
+        ("moved", C.c_uint32 * 64),
+        ("underload_before", C.c_int64),
+        ("underload_after", C.c_int64),
+        ("candidates", C.c_uint64),
+        ("edges_scanned", C.c_uint64),
+        ("kernel_launches", C.c_uint64),
+        ("device_ms", C.c_float),
+    ]
+
+    def moved_list(self):
+        return list(self.moved[: self.rounds])
+
+
 def library_path() -> str:
     return _LIB_PATH
 
@@ -113,7 +131,8 @@ def load_library():
         lib = C.CDLL(_LIB_PATH)
         lib.kmp_last_error.restype = C.c_char_p
         lib.kmp_lp_labels_device.restype = C.c_void_p
-        for sym in ("kmp_overload_balance", "kmp_balance_select_all"):  # include/kaminpar_b200_balancer.h
+        for sym in ("kmp_overload_balance", "kmp_balance_select_all",  # include/kaminpar_b200_balancer.h
+                    "kmp_underload_balance", "kmp_underload_select_all"):
             if not hasattr(lib, sym):
                 raise RuntimeError(f"{_LIB_PATH} lacks {sym}; rebuild the library")
         if lib.kmp_lp_abi_version() != ABI_VERSION:  # the ctypes structs below mirror exactly this header version
@@ -457,6 +476,35 @@ class LPHandle:
                                                 C.c_uint32(call_index), C.c_uint32(round), _ptr(tgt), _ptr(key)))
         return tgt, key
 
+    def underload_balance(self, k, max_block_weights, min_block_weights, partition: Optional[np.ndarray]):
+        """kmp_underload_balance: partition (uint32, balanced in place) or None = the labels on the device;
+        min_block_weights None = no minimum weights (no device work, block weights None).
+        Returns (improved, block_weights, stats)."""
+        stats = KmpUnderloadStats()
+        mbw = np.ascontiguousarray(max_block_weights, np.int32)
+        mnw = None if min_block_weights is None else np.ascontiguousarray(min_block_weights, np.int32)
+        bw = np.zeros(k, np.int32)
+        improved = C.c_int(0)
+        if partition is not None:
+            assert partition.dtype == np.uint32 and partition.flags.c_contiguous
+        _check(self._lib.kmp_underload_balance(self._h, C.c_uint32(int(k)), _ptr(mbw), _ptr(mnw), _ptr(partition),
+                                               _ptr(bw), C.byref(improved), C.byref(stats)))
+        return bool(improved.value), (bw if mnw is not None else None), stats
+
+    def underload_select_all(self, k, labels, block_weights, max_block_weights, min_block_weights, call_index=0,
+                             round=0):
+        """kmp_underload_select_all: (target[n] uint32, key[n] float32) against frozen state."""
+        labels = np.ascontiguousarray(labels, np.uint32)
+        bw = np.ascontiguousarray(block_weights, np.int32)
+        mbw = np.ascontiguousarray(max_block_weights, np.int32)
+        mnw = np.ascontiguousarray(min_block_weights, np.int32)
+        tgt = np.empty(self._n, np.uint32)
+        key = np.empty(self._n, np.float32)
+        _check(self._lib.kmp_underload_select_all(self._h, C.c_uint32(int(k)), _ptr(labels), _ptr(bw), _ptr(mbw),
+                                                  _ptr(mnw), C.c_uint32(call_index), C.c_uint32(round), _ptr(tgt),
+                                                  _ptr(key)))
+        return tgt, key
+
     def edge_cut(self) -> int:
         cut = C.c_int64(0)
         _check(self._lib.kmp_lp_edge_cut(self._h, C.byref(cut)))
@@ -597,6 +645,44 @@ class OverloadBalancer:
             self._graph = p_graph.graph
         improved, bw, stats = self._handle.overload_balance(p_ctx.k, mbw, p_ctx.perfectly_balanced_block_weights(),
                                                             p_graph.partition)
+        p_graph._block_weights = bw
+        self.last_stats = stats
+        return improved
+
+
+class UnderloadBalancer:
+    """Drop-in for ``kaminpar::shm::UnderloadBalancer : Refiner`` (underload_balancer.h, refiner.h:18-57) on the
+    device. Its selection rule is the reference's without thread order (DESIGN.md §12)."""
+
+    def __init__(self, ctx: Context):
+        self._ctx = ctx
+        self._handle = LPHandle(_refine_config(ctx.refinement.lp, ctx.engine))
+        self._graph = None
+        self.last_stats: Optional[KmpUnderloadStats] = None
+
+    def name(self) -> str:
+        return "Underload Balancer"
+
+    def invalidate_graph(self):
+        self._graph = None
+
+    def initialize(self, p_graph: PartitionedGraph):
+        pass  # underload_balancer.cc:35-37: nothing to do
+
+    def refine(self, p_graph: PartitionedGraph, p_ctx: PartitionContext) -> bool:
+        assert p_graph.k() <= p_ctx.k
+        mnw = p_ctx.min_block_weights()
+        if mnw is None:  # underload_balancer.cc:47: no minimum weights
+            self.last_stats = None
+            return False
+        w = p_graph.block_weights().astype(np.int64)
+        if bool(np.all(w >= mnw[: len(w)])):  # metrics::is_min_balanced: no device work
+            self.last_stats = None
+            return False
+        if self._graph is not p_graph.graph:
+            self._handle.set_graph(p_graph.graph)
+            self._graph = p_graph.graph
+        improved, bw, stats = self._handle.underload_balance(p_ctx.k, p_ctx.max_block_weights(), mnw, p_graph.partition)
         p_graph._block_weights = bw
         self.last_stats = stats
         return improved
