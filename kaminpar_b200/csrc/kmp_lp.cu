@@ -56,7 +56,7 @@ constexpr int kNumGroups = 4; // degree groups of the schedule
 constexpr int kNumTiers = 8;  // kernel tiers: group 1 is split in two, group 3 (deg >= 256) in four
 // sync_subrounds: the work-list keys (tier * S + sub-round, plus one key for unvisited vertices) are 8 bits wide
 constexpr uint32_t kMaxSubrounds = (255 - 1) / kNumTiers;
-constexpr int kHubTier = 7;   // deg >= kHubMinDegree: edge-parallel kernels, label-partitioned buckets (lp_sweep.cuh)
+constexpr int kHubTier = 7;   // deg >= kHubMinDegree: label-partitioned hub kernels (lp_sweep.cuh)
 constexpr int kStatTiers = 12; // tier slots of kmp_lp_stats / ctr64 (edges at [tier], nodes at [kCtrNodes + tier])
 constexpr int kCtrNodes = 16, kCtrScratch = 40, kCtrSize = 48;
 constexpr uint32_t kHubMinDegree = 8192;       // graphs with edge weights (32-bit ratings in the team tables)
@@ -190,6 +190,12 @@ struct kmp_lp_handle {
   DevBuf<unsigned long long> hub_tab; // bucket regions: kBucketCap packed (key << 32 | rating) entries each
   DevBuf<uint32_t> hub_cursor;        // per bucket: entries appended in the running sub-round
   DevBuf<HubOverflow> hub_ovf;
+  // clusterer hub path (gather + rate): per list entry the start of its row in hub_lab (sub-round-relative) and its
+  // first rate item result; the (entry, hash class) rate items of each sub-round, largest degree first
+  DevBuf<uint32_t> t4_lab_off, t4_rate_begin, t4_rate_entry, t4_rate_cls;
+  std::vector<uint32_t> t4_rate_off; // S + 1
+  uint64_t t4_max_subround_edges = 0;
+  DevBuf<uint32_t> hub_lab; // staged neighbour labels of the running sub-round's hubs (4 B per edge)
   uint32_t mover_cap = 0;
   uint32_t cur_subround = 0; // hashed class of the running sub-round
   uint32_t cur_sg = 0;       // running sub-round index in [0, 4 * S): queue cursor and stamp code
@@ -606,7 +612,13 @@ bool configure_team(kmp_lp_handle *h, int sms) {
 
 // per device; called from kmp_lp_create
 template <int MODE, bool EW, bool P64> bool configure_team_kernels(kmp_lp_handle *h, int sms) {
-  cudaFuncSetAttribute(sweep_hub_scatter<MODE, EW, P64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kHubScatterSmem);
+  if constexpr (MODE == 0) {
+    if (cudaFuncSetAttribute(sweep_hub_rate<EW>, cudaFuncAttributeMaxDynamicSharedMemorySize, rate_smem<EW>()) != cudaSuccess) {
+      return false;
+    }
+  } else {
+    cudaFuncSetAttribute(sweep_hub_scatter<MODE, EW, P64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kHubScatterSmem);
+  }
   bool ok = configure_team<MODE, EW, P64, 32, 512, 8, !EW>(h, sms) && configure_team<MODE, EW, P64, 128, 2048, 4>(h, sms) &&
             configure_team<MODE, EW, P64, 512, 8192, 1>(h, sms);
   if constexpr (EW) {
@@ -654,37 +666,61 @@ template <int MODE, bool EW, bool P64> cudaError_t launch_sweep_t(kmp_lp_handle 
     const uint32_t s_idx = h->cur_subround;
     const uint32_t S = h->lists_S;
     const uint32_t first = h->list_off[kHubTier * S + s_idx] - h->list_off[kHubTier * S];
-    hb.table_off = h->t4_table_off.p + first;
-    hb.g_tab = h->hub_tab.p;
-    hb.cursor = h->hub_cursor.p;
-    hb.ovf = h->hub_ovf.p;
-    hb.ovf_cap = static_cast<uint32_t>(std::min<uint64_t>(h->t4_max_wave_edges, 0xFFFFFFFFull));
-    hb.bucket_cap = h->hub_bucket_cap;
     hb.sel_limit = h->hub_sel_limit;
-    hb.stage_adjncy = h->adjncy_16b ? 1u : 0u;
     hb.rank = h->rank;
     hb.world = h->world;
-    hb.sel_begin = h->t4_sel_begin.p + first;
     hb.hit = h->t4_hit.p + first;
-    // one scatter + select pair per wave; all waves share the bucket memory (cursors reset by the select)
-    for (uint32_t w = h->t4_wave_off[s_idx]; w < h->t4_wave_off[s_idx + 1]; ++w) {
-      const kmp_lp_handle::HubWave &wv = h->t4_waves[w];
-      hb.item_entry = h->t4_item_entry.p + wv.item_lo;
-      hb.item_chunk = h->t4_item_chunk.p + wv.item_lo;
-      hb.item_u = h->t4_item_u.p + wv.item_lo;
-      hb.item_beg = h->t4_item_beg.p + wv.item_lo;
-      hb.item_deg = h->t4_item_deg.p + wv.item_lo;
-      hb.num_items = wv.item_hi - wv.item_lo;
-      hb.queue = h->ctr32.p + 64 + w; // zeroed with the other per-round counters
-      hb.ovf_count = h->ctr32.p + 512 + w;
-      sweep_hub_scatter<MODE, EW, P64><<<capped(h, std::min<uint32_t>(hb.num_items, kSMs * 4)), kHubThreads, kHubScatterSmem, h->sweep_stream>>>(a, hb, h->m);
-      hb.sel_entry = h->t4_sel_entry.p + wv.sel_lo;
-      hb.sel_piece = h->t4_sel_piece.p + wv.sel_lo;
-      hb.num_sel_items = wv.sel_hi - wv.sel_lo;
-      hb.part_best = h->t4_part_best.p + (wv.sel_lo - h->t4_sel_off[s_idx]);
-      hb.part_fav = h->t4_part_fav.p + (wv.sel_lo - h->t4_sel_off[s_idx]);
-      sweep_hub_select<MODE><<<capped(h, std::min<uint32_t>((hb.num_sel_items + kSelWarps - 1) / kSelWarps, kSMs * 6)), kSelWarps * 32, 0, h->sweep_stream>>>(a, hb);
+    if constexpr (MODE == 0) {
+      // gather the labels of the sub-round's hub edges once, then rate every (hub, hash class) item in one CTA
+      const uint32_t ilo = h->t4_item_off[s_idx], ihi = h->t4_item_off[s_idx + 1];
+      hb.item_entry = h->t4_item_entry.p + ilo;
+      hb.item_chunk = h->t4_item_chunk.p + ilo;
+      hb.item_u = h->t4_item_u.p + ilo;
+      hb.item_beg = h->t4_item_beg.p + ilo;
+      hb.item_deg = h->t4_item_deg.p + ilo;
+      hb.num_items = ihi - ilo;
+      hb.lab = h->hub_lab.p;
+      hb.lab_off = h->t4_lab_off.p + first;
+      sweep_hub_gather<P64><<<capped(h, std::min<uint32_t>(hb.num_items, kSMs * 8)), 256, 0, h->sweep_stream>>>(a, hb);
+      const uint32_t rlo = h->t4_rate_off[s_idx], rhi = h->t4_rate_off[s_idx + 1];
+      hb.item_entry = h->t4_rate_entry.p + rlo;
+      hb.item_cls = h->t4_rate_cls.p + rlo;
+      hb.num_items = rhi - rlo;
+      hb.sel_begin = h->t4_rate_begin.p + first;
+      hb.part_best = h->t4_part_best.p;
+      hb.part_fav = h->t4_part_fav.p;
+      hb.queue = h->ctr32.p + 64 + s_idx; // zeroed with the other per-round counters
+      sweep_hub_rate<EW><<<capped(h, std::min<uint32_t>(hb.num_items, kSMs)), kRateThreads, rate_smem<EW>(), h->sweep_stream>>>(a, hb);
       h->kernel_launches += 2;
+    } else {
+      hb.table_off = h->t4_table_off.p + first;
+      hb.g_tab = h->hub_tab.p;
+      hb.cursor = h->hub_cursor.p;
+      hb.ovf = h->hub_ovf.p;
+      hb.ovf_cap = static_cast<uint32_t>(std::min<uint64_t>(h->t4_max_wave_edges, 0xFFFFFFFFull));
+      hb.bucket_cap = h->hub_bucket_cap;
+      hb.stage_adjncy = h->adjncy_16b ? 1u : 0u;
+      hb.sel_begin = h->t4_sel_begin.p + first;
+      // one scatter + select pair per wave; all waves share the bucket memory (cursors reset by the select)
+      for (uint32_t w = h->t4_wave_off[s_idx]; w < h->t4_wave_off[s_idx + 1]; ++w) {
+        const kmp_lp_handle::HubWave &wv = h->t4_waves[w];
+        hb.item_entry = h->t4_item_entry.p + wv.item_lo;
+        hb.item_chunk = h->t4_item_chunk.p + wv.item_lo;
+        hb.item_u = h->t4_item_u.p + wv.item_lo;
+        hb.item_beg = h->t4_item_beg.p + wv.item_lo;
+        hb.item_deg = h->t4_item_deg.p + wv.item_lo;
+        hb.num_items = wv.item_hi - wv.item_lo;
+        hb.queue = h->ctr32.p + 64 + w; // zeroed with the other per-round counters
+        hb.ovf_count = h->ctr32.p + 512 + w;
+        sweep_hub_scatter<MODE, EW, P64><<<capped(h, std::min<uint32_t>(hb.num_items, kSMs * 4)), kHubThreads, kHubScatterSmem, h->sweep_stream>>>(a, hb, h->m);
+        hb.sel_entry = h->t4_sel_entry.p + wv.sel_lo;
+        hb.sel_piece = h->t4_sel_piece.p + wv.sel_lo;
+        hb.num_sel_items = wv.sel_hi - wv.sel_lo;
+        hb.part_best = h->t4_part_best.p + (wv.sel_lo - h->t4_sel_off[s_idx]);
+        hb.part_fav = h->t4_part_fav.p + (wv.sel_lo - h->t4_sel_off[s_idx]);
+        sweep_hub_select<MODE><<<capped(h, std::min<uint32_t>((hb.num_sel_items + kSelWarps - 1) / kSelWarps, kSMs * 6)), kSelWarps * 32, 0, h->sweep_stream>>>(a, hb);
+        h->kernel_launches += 2;
+      }
     }
     hb.part_best = h->t4_part_best.p;
     hb.part_fav = h->t4_part_fav.p;
@@ -848,6 +884,7 @@ int ensure_lists(kmp_lp_handle *h) {
     h->t4_waves.clear();
     h->t4_max_slots = 0;
     h->t4_max_wave_edges = 0;
+    h->t4_max_subround_edges = 0;
     if (t4_cnt > 0) {
       DevBuf<uint32_t> &d_deg = h->t4_tmp_deg, &d_beg = h->t4_tmp_beg, &d_ids = h->t4_tmp_ids; // grow-only
       KMP_CUDA(d_deg.ensure(t4_cnt));
@@ -925,6 +962,43 @@ int ensure_lists(kmp_lp_handle *h) {
       if (h->t4_waves.size() > kMaxHubWaves) {
         return fail(KMP_ERR_UNSUPPORTED, "too many high-degree table waves (raise KMP_HUB_WAVE_SLOTS)");
       }
+      // clusterer: per entry its row in the staged labels and its first result slot, and the (entry, hash class)
+      // rate items of every sub-round, largest degree first (the longest items start first)
+      std::vector<uint32_t> loff(t4_cnt), rbeg(t4_cnt), rent, rcls, ord;
+      h->t4_rate_off.assign(S + 1, 0);
+      size_t max_rate = 0;
+      for (uint32_t sr = 0; sr < S; ++sr) {
+        const uint32_t lo = h->list_off[kHubTier * S + sr] - t4_begin, hi = h->list_off[kHubTier * S + sr + 1] - t4_begin;
+        uint64_t edges = 0; // <= m < 2^32
+        uint32_t res = 0;
+        ord.clear();
+        for (uint32_t i = lo; i < hi; ++i) {
+          loff[i] = static_cast<uint32_t>(edges);
+          edges += deg[i];
+          rbeg[i] = res;
+          res += hub_classes(deg[i]);
+          ord.push_back(i);
+        }
+        std::stable_sort(ord.begin(), ord.end(), [&](uint32_t x, uint32_t y) { return deg[x] > deg[y]; });
+        for (const uint32_t i : ord) {
+          for (uint32_t c = 0; c < hub_classes(deg[i]); ++c) {
+            rent.push_back(i - lo);
+            rcls.push_back(c);
+          }
+        }
+        h->t4_rate_off[sr + 1] = static_cast<uint32_t>(rent.size());
+        max_rate = std::max<size_t>(max_rate, res);
+        h->t4_max_subround_edges = std::max(h->t4_max_subround_edges, edges);
+      }
+      max_sel = std::max(max_sel, max_rate);
+      KMP_CUDA(h->t4_lab_off.ensure(t4_cnt));
+      KMP_CUDA(h->t4_rate_begin.ensure(t4_cnt));
+      KMP_CUDA(h->t4_rate_entry.ensure(rent.size()));
+      KMP_CUDA(h->t4_rate_cls.ensure(rcls.size()));
+      KMP_CUDA(cudaMemcpyAsync(h->t4_lab_off.p, loff.data(), t4_cnt * 4, cudaMemcpyHostToDevice, h->stream));
+      KMP_CUDA(cudaMemcpyAsync(h->t4_rate_begin.p, rbeg.data(), t4_cnt * 4, cudaMemcpyHostToDevice, h->stream));
+      KMP_CUDA(cudaMemcpyAsync(h->t4_rate_entry.p, rent.data(), rent.size() * 4, cudaMemcpyHostToDevice, h->stream));
+      KMP_CUDA(cudaMemcpyAsync(h->t4_rate_cls.p, rcls.data(), rcls.size() * 4, cudaMemcpyHostToDevice, h->stream));
       KMP_CUDA(h->t4_table_off.ensure(t4_cnt));
       KMP_CUDA(h->t4_hit.ensure(t4_cnt));
       KMP_CUDA(cudaMemsetAsync(h->t4_hit.p, 0, static_cast<size_t>(t4_cnt) * 4, h->stream));
@@ -995,8 +1069,12 @@ int ensure_scratch(kmp_lp_handle *h, int mode, uint32_t num_labels) {
     KMP_CUDA(cudaMemsetAsync(h->hist.p, 0, kk * kLadderLevels * sizeof(int32_t), h->stream));
     KMP_CUDA(cudaMemsetAsync(h->ohist.p, 0, kk * kLadderLevels * sizeof(int32_t), h->stream));
   }
-  // bucket regions, cursors and overflow list of the hub tier
-  if (h->t4_max_slots > 0) {
+  // hub tier scratch: the clusterer stages 4 B per hub edge of the largest sub-round; the refiner has bucket
+  // regions, cursors and an overflow list
+  if (mode == 0 && h->t4_max_subround_edges > 0) {
+    KMP_CUDA(h->hub_lab.ensure(h->t4_max_subround_edges));
+  }
+  if (mode == 1 && h->t4_max_slots > 0) {
     KMP_CUDA(h->hub_tab.ensure(h->t4_max_slots)); // no initialisation: the cursors say how much of a region is valid
     KMP_CUDA(h->hub_cursor.ensure(h->t4_max_slots / kBucketCap));
     KMP_CUDA(h->hub_ovf.ensure(std::max<uint64_t>(h->t4_max_wave_edges, 1)));
@@ -2455,6 +2533,7 @@ int kmp_lp_free_scratch(kmp_lp_handle *h) {
   h->hub_tab.release();
   h->hub_cursor.release();
   h->hub_ovf.release();
+  h->hub_lab.release();
   h->labg.release();
   h->sort_keys_in.release();
   h->sort_keys_out.release();

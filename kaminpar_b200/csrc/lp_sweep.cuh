@@ -8,7 +8,8 @@
 //   tier 5 (deg 1024..4095) sweep_team<T=512> : one 512-thread CTA per vertex, 8192 slots
 //   tier 6 (deg 4096..8191, or ..16383 with unit edge weights: 16-bit ratings) sweep_team<T=1024>: one
 //                          1024-thread CTA per vertex, 16384 / 32768 slots
-//   tier 7 (deg >= 8192 / 16384) sweep_hub_*  : edge-parallel chunks, label-partitioned bucket appends (see below)
+//   tier 7 (deg >= 8192 / 16384) sweep_hub_*  : clusterer: staged labels rated per hash class, one CTA per class;
+//                          refiner: edge-parallel chunks, label-partitioned bucket appends (see below)
 //   (tiers 1-2 are degree group 1 of the schedule, tiers 4..7 group 3)
 //
 // Each of them restates label_propagation.h:460-541 (find_best_cluster): accumulate
@@ -663,8 +664,20 @@ __global__ void __launch_bounds__(T *TEAMS, team_ctas_per_sm<T>()) sweep_team(co
 }
 
 // ================================================================================================
-// tier 7 (deg >= 8192 / 16384): edge-parallel, label-partitioned two-pass aggregation. No random access ever
-// touches a table outside shared memory, and after the chunk is staged every warp works on its own:
+// tier 7 (deg >= 8192 / 16384), clusterer (MODE 0): label-partitioned rating with final results per CTA.
+//   gather : edge-parallel over the 2048-edge chunks of the sub-round's hubs: every neighbour label is gathered
+//            once and written, coalesced, to a scratch row per hub (4 B per edge); the stamps mark pull activation.
+//   rate   : one 1024-thread CTA per work item (hub u, hash class c of K_u = hub_classes(deg) classes, taken from a
+//            queue in order of decreasing degree). It streams all staged labels of u from L2 and inserts only those
+//            with lowbias32(label) & (K_u - 1) == c -- compacted per warp first, so a class costs inserts only for
+//            its own labels -- into a 16384-slot shared-memory table with a claim list, then selects as the team
+//            kernels do. Classes of a hub hold disjoint labels, so each result is final for its class: no merge.
+//            A class that claims more than the list holds is split by the next hash bit and streamed again, until
+//            every sub-class fits (lowbias32 is a bijection, so this terminates).
+//   final  : as below: the arg-max over the K_u class results of each hub.
+// tier 7, refiner (MODE 1): edge-parallel, label-partitioned two-pass aggregation (a refiner hub sees at most k
+// labels, so the slice maps compress 256 edges to <= k appends). No random access ever touches a table outside
+// shared memory, and after the chunk is staged every warp works on its own:
 //   scatter : a CTA takes 2048-edge chunks of hub adjacencies from a work queue. The producer warp stages each
 //             chunk with one 1-D bulk TMA copy; each of the 8 consumer warps gathers the labels of its 256-edge
 //             slice, aggregates them in its private 512-slot shared-memory hash map (slice-local ratings: a label
@@ -722,6 +735,11 @@ struct HubArgs {
   uint32_t rank, world;                   // hub entry i is owned by rank i % world
   uint32_t *__restrict__ queue;           // work-queue cursor of this launch (zeroed per LP round)
   uint32_t *__restrict__ hit;             // per list entry: a neighbour moved since the last visit (pull); reset by final
+  // clusterer (gather + rate): the staged neighbour labels of the sub-round and, per list entry, where its row
+  // starts in them; rate items are (item_entry, item_cls) pairs, their results go to part_*[sel_begin[entry] + cls]
+  uint32_t *__restrict__ lab;
+  const uint32_t *__restrict__ lab_off;
+  const uint32_t *__restrict__ item_cls;
 };
 
 // buckets of a hub: a power of two with <= kBucketTargetFill expected distinct labels per bucket
@@ -984,8 +1002,9 @@ __global__ void __launch_bounds__(kHubThreads, 4) sweep_hub_scatter(const SweepA
   }
 }
 
-// select: one warp per (hub, bucket): best candidates of the bucket's labels
+// select (refiner): one warp per (hub, bucket): best candidate of the bucket's labels
 template <int MODE> __global__ void __launch_bounds__(kSelWarps * 32) sweep_hub_select(const SweepArgs a, const HubArgs hb) {
+  static_assert(MODE == 1, "the clusterer rates its hubs with sweep_hub_rate");
   __shared__ uint32_t s_keys[kSelWarps][kSelTableSlots];
   __shared__ int32_t s_vals[kSelWarps][kSelTableSlots];
   __shared__ uint32_t s_claims_all[kSelWarps];
@@ -1006,7 +1025,7 @@ template <int MODE> __global__ void __launch_bounds__(kSelWarps * 32) sweep_hub_
   for (uint32_t it = blockIdx.x * kSelWarps + wib; it < hb.num_sel_items; it += nwarps) {
     const uint32_t entry = hb.sel_entry[it];
     const uint32_t u = a.list[entry];
-    Cand c = cand_none(), f = cand_none();
+    Cand c = cand_none();
     // a bucket is read (and its cursor reset) whenever the scatter pass may have filled it; activity is decided
     // by sweep_hub_final
     const bool act = (entry % hb.world == hb.rank) && (a.active == nullptr || a.pull || a.active[u] != 0);
@@ -1018,7 +1037,6 @@ template <int MODE> __global__ void __launch_bounds__(kSelWarps * 32) sweep_hub_
       const uint32_t own = a.label[u];
       const int32_t uw = a.vwgt != nullptr ? a.vwgt[u] : 1;
       const int32_t own_w = a.weight[own];
-      const bool store_fav = (MODE == 0) && (uw == own_w) && (own_w <= a.max_cluster_weight / 2);
       const uint32_t n_reg = appended < hb.bucket_cap ? appended : hb.bucket_cap;
       const uint32_t n_ovf = appended > hb.bucket_cap ? min(__ldcg(hb.ovf_count), hb.ovf_cap) : 0u;
       // The map is sized for the entries at hand. A bucket without overflow entries holds <= kBucketCap =
@@ -1048,7 +1066,6 @@ template <int MODE> __global__ void __launch_bounds__(kSelWarps * 32) sweep_hub_
       uint32_t K = 1;
       while (true) {
         c = cand_none();
-        f = cand_none();
         bool overflowed = false;
         for (uint32_t cls = 0; cls < K && !overflowed; ++cls) {
           // ---- insert the entries of hash class `cls`
@@ -1090,44 +1107,7 @@ template <int MODE> __global__ void __launch_bounds__(kSelWarps * 32) sweep_hub_
           }
           __syncwarp(); // the class is inserted (or abandoned)
           // ---- evaluate + clear
-          bool lazy_done = false;
-          if (MODE == 0 && K == 1 && !overflowed) {
-            // Clusterer, single class: rank the labels WITHOUT their cluster weights (the team kernels do the
-            // same): if the bucket's top label is feasible it is the bucket's best; the favored label never needs
-            // weights. Only a full top label costs the second scan with one weight gather per label.
-            Cand ct = cand_none();
-            for (uint32_t s = lane; s < tcap; s += 32) {
-              const uint32_t kx = keys[s];
-              if (kx != kEmpty) {
-                const int32_t r = vals[s];
-                if (r >= ct.gain && r > 0) {
-                  const Cand x{r, 0, tie_hash(a.base_tie, u, kx), kx};
-                  if (cand_better<0>(x, ct)) {
-                    ct = x;
-                  }
-                }
-                if (store_fav && r >= f.gain && r > 0) {
-                  const Cand y{r, 0, tie_hash(a.base_fav, u, kx), kx};
-                  if (cand_better<0>(y, f)) {
-                    f = y;
-                  }
-                }
-              }
-            }
-            const Cand top = warp_argmax<0>(kFull, ct);
-            bool top_ok = true;
-            if (top.gain > 0) {
-              top_ok = (a.weight[top.key] + uw <= a.max_cluster_weight) || (top.key == own);
-              if (a.communities != nullptr) {
-                top_ok = top_ok && (a.communities[top.key] == a.communities[own]);
-              }
-            }
-            if (top_ok) {
-              c = top;
-              lazy_done = true;
-            }
-          }
-          const bool evaluate = !overflowed && !lazy_done;
+          const bool evaluate = !overflowed;
           for (uint32_t s0 = 0; s0 < tcap; s0 += 32 * B) {
             uint32_t kk[B];
             int32_t rr[B], ww[B];
@@ -1149,14 +1129,9 @@ template <int MODE> __global__ void __launch_bounds__(kSelWarps * 32) sweep_hub_
                 vals[s] = 0;
                 if (evaluate) {
                   Cand ff;
-                  // (the favored candidate of the lazy pass is final: no second evaluation)
-                  const Cand cc = eval_candidate_w<MODE>(a, u, own, uw, own_w, kk[j], rr[j], ww[j],
-                                                         store_fav && !(MODE == 0 && K == 1), ff);
-                  if (cand_better<MODE>(cc, c)) {
+                  const Cand cc = eval_candidate_w<1>(a, u, own, uw, own_w, kk[j], rr[j], ww[j], false, ff);
+                  if (cand_better<1>(cc, c)) {
                     c = cc;
-                  }
-                  if (MODE == 0 && cand_better<0>(ff, f)) {
-                    f = ff;
                   }
                 }
               }
@@ -1177,16 +1152,322 @@ template <int MODE> __global__ void __launch_bounds__(kSelWarps * 32) sweep_hub_
         hb.cursor[b] = 0;
       }
     }
-    const Cand best = warp_argmax<MODE>(kFull, c);
-    const Cand fav = (MODE == 0) ? warp_argmax<0>(kFull, f) : cand_none();
+    const Cand best = warp_argmax<1>(kFull, c);
     if (lane == 0) {
       hb.part_best[it] = best;
-      hb.part_fav[it] = fav;
     }
   }
 }
 
-// final: one warp per hub: reduce its buckets' candidates, then propose / store the favored cluster.
+// ---- clusterer: gather + rate ---------------------------------------------------------------------------------
+constexpr int kRateThreads = 1024;
+constexpr uint32_t kRateSlots = 16384;            // table of the rate kernel: 128 KiB of keys + 32-bit ratings
+constexpr uint32_t kRateListCap = kRateSlots / 2; // claim list (16-bit slot indices); the table load stays <= 0.5
+constexpr uint32_t kHubClassEdges = 8192;         // edges per hash class: a class fits the list even if all distinct
+constexpr uint32_t kRateStage = 64;               // per-warp staging ring: < 32 pending + 32 new labels
+// dynamic shared memory of the rate kernel: keys + ratings, the claim list, the staging buffers (labels, weights)
+template <bool EW> constexpr int rate_smem() {
+  return static_cast<int>(kRateSlots * 8 + kRateListCap * 2 + (kRateThreads / 32) * kRateStage * (EW ? 8 : 4));
+}
+
+// hash classes of a hub: a power of two with <= kHubClassEdges edges per class (the low bits of lowbias32(label),
+// the same bits as the bucket index of the refiner's path)
+__host__ __device__ __forceinline__ uint32_t hub_classes(uint32_t full_degree) {
+  const uint32_t need = (full_degree + kHubClassEdges - 1) / kHubClassEdges;
+  uint32_t p = 1;
+  while (p < need) {
+    p <<= 1;
+  }
+  return p;
+}
+
+// gather: one 256-thread CTA per (hub, 2048-edge chunk) item, 8 independent label gathers per thread
+template <bool P64> __global__ void __launch_bounds__(256) sweep_hub_gather(const SweepArgs a, const HubArgs hb) {
+  constexpr int B = kChunkEdges / 256;
+  const int lane = threadIdx.x & 31;
+  for (uint32_t it = blockIdx.x; it < hb.num_items; it += gridDim.x) {
+    const uint32_t entry = hb.item_entry[it];
+    const uint32_t u = hb.item_u[it];
+    if (entry % hb.world != hb.rank || !(a.active == nullptr || a.pull || a.active[u] != 0)) {
+      continue;
+    }
+    const uint32_t deg = min(hb.item_deg[it], a.max_num_neighbors);
+    const uint32_t cbeg = hb.item_chunk[it] * kChunkEdges;
+    if (cbeg >= deg) {
+      continue;
+    }
+    const uint32_t cend = min(cbeg + kChunkEdges, deg);
+    const uint32_t *adj = a.adjncy + hb.item_beg[it];
+    uint32_t *out = hb.lab + hb.lab_off[entry];
+    uint32_t v[B];
+#pragma unroll
+    for (int j = 0; j < B; ++j) {
+      const uint32_t e = cbeg + j * 256 + threadIdx.x;
+      v[j] = e < cend ? adj[e] : kEmpty;
+    }
+    bool hit = false;
+#pragma unroll
+    for (int j = 0; j < B; ++j) {
+      if (v[j] != kEmpty) {
+        const typename LabG<P64>::word g = load_labg<P64>(a, v[j]);
+        hit = hit || stamp_hit(LabG<P64>::stamp(g), a.window);
+        out[cbeg + j * 256 + threadIdx.x] = LabG<P64>::label(g);
+      }
+    }
+    if (a.pull && __any_sync(kFull, hit) && lane == 0) {
+      atomicOr(&hb.hit[entry], 1u);
+    }
+  }
+}
+
+// One warp inserts up to 32 staged labels (one per lane where `valid`) into the rate table and appends the slots
+// it claims to the list. With unit edge weights the claimer does not add its 1 (see team_table_add). Returns, in
+// every lane, whether the claims of the running class have passed `limit`.
+template <bool EW>
+__device__ __forceinline__ bool rate_insert(uint32_t *keys, int32_t *vals, uint16_t *list, uint32_t *s_claims,
+                                            uint32_t limit, uint32_t key, int32_t w, bool valid, int lane) {
+  uint32_t slot = 0;
+  bool claimed = false;
+  if (valid) {
+    // the class fixes the low bits of lowbias32(key): the slot comes from another hash of the key
+    slot = lowbias32(key ^ 0x9E3779B9u) & (kRateSlots - 1);
+    while (true) {
+      const uint32_t prev = atomicCAS(&keys[slot], kEmpty, key);
+      if (prev == kEmpty || prev == key) {
+        claimed = prev == kEmpty;
+        if (EW || !claimed) {
+          atomicAdd(&vals[slot], w);
+        }
+        break;
+      }
+      slot = (slot + 1) & (kRateSlots - 1);
+    }
+  }
+  const unsigned mask = __ballot_sync(kFull, claimed);
+  if (mask == 0) {
+    return false;
+  }
+  const uint32_t n = __popc(mask);
+  uint32_t base = 0;
+  if (lane == 0) {
+    base = atomicAdd(s_claims, n);
+  }
+  base = __shfl_sync(kFull, base, 0);
+  const uint32_t idx = base + __popc(mask & ((1u << lane) - 1u));
+  if (claimed && idx < kRateListCap) {
+    list[idx] = static_cast<uint16_t>(slot);
+  }
+  return base + n > limit;
+}
+
+// rate: one CTA per (hub, hash class) item; writes the class's best and favored candidates
+template <bool EW> __global__ void __launch_bounds__(kRateThreads, 1) sweep_hub_rate(const SweepArgs a, const HubArgs hb) {
+  constexpr int T = kRateThreads;
+  constexpr int kWarps = T / 32;
+  constexpr int B = 8; // independent label loads in flight per lane
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  uint32_t *keys = reinterpret_cast<uint32_t *>(smem_raw);
+  int32_t *vals = reinterpret_cast<int32_t *>(smem_raw + sizeof(uint32_t) * kRateSlots);
+  uint32_t *stage_k = reinterpret_cast<uint32_t *>(smem_raw + 8 * kRateSlots);
+  int32_t *stage_w = reinterpret_cast<int32_t *>(stage_k + kWarps * kRateStage); // EW only
+  uint16_t *list = reinterpret_cast<uint16_t *>(stage_k + (EW ? 2 : 1) * kWarps * kRateStage);
+  __shared__ Cand s_red[kWarps];
+  __shared__ uint32_t s_item, s_claims;
+  const int tid = threadIdx.x;
+  const int lane = tid & 31;
+  const int wib = tid >> 5;
+  const unsigned below = (1u << lane) - 1u;
+  uint32_t *stk = stage_k + wib * kRateStage;
+  int32_t *stw = stage_w + wib * kRateStage;
+  for (uint32_t s = tid; s < kRateSlots; s += T) {
+    keys[s] = kEmpty;
+    vals[s] = 0;
+  }
+  // a class with one label never splits, one with two may: the limit is >= 2 so that K stays below 2^32
+  const uint32_t limit = (hb.sel_limit != 0 && hb.sel_limit < kRateListCap) ? max(hb.sel_limit, 2u) : kRateListCap;
+  while (true) {
+    if (tid == 0) {
+      s_item = atomicAdd(hb.queue, 1u);
+    }
+    __syncthreads(); // also: the table is clean
+    const uint32_t it = s_item;
+    if (it >= hb.num_items) {
+      break;
+    }
+    const uint32_t entry = hb.item_entry[it];
+    const uint32_t c0 = hb.item_cls[it];
+    const uint32_t u = a.list[entry];
+    if (entry % hb.world == hb.rank && (a.active == nullptr || a.pull || a.active[u] != 0)) {
+      const uint32_t beg = a.xadj[u];
+      const uint32_t full_deg = a.xadj[u + 1] - beg;
+      const uint32_t deg = min(full_deg, a.max_num_neighbors);
+      const uint32_t K0 = hub_classes(full_deg);
+      const uint32_t own = a.label[u];
+      const int32_t uw = a.vwgt != nullptr ? a.vwgt[u] : 1;
+      const int32_t own_w = a.weight[own];
+      const bool store_fav = (uw == own_w) && (own_w <= a.max_cluster_weight / 2);
+      const uint32_t *lab = hb.lab + hb.lab_off[entry];
+      Cand best = cand_none(), fav = cand_none();
+      uint32_t cls = c0, K = K0;
+      while (true) {
+        if (tid == 0) {
+          s_claims = 0;
+        }
+        __syncthreads();
+        // ---- stream the staged labels: each warp takes 256-label blocks, compacts the labels of class `cls`
+        // (mod K) in its 64-entry ring and inserts them 32 at a time. No barrier inside: a warp stops once the claims
+        // have passed the limit, after at most one more batch of 32 claims, so the table stays below 3/4 full.
+        bool wover = false;
+        uint32_t head = 0, pend = 0; // ring index of the oldest staged label, labels staged (warp-uniform)
+        for (uint32_t e0 = wib * 32 * B; e0 < deg && !wover; e0 += T * B) {
+          uint32_t kb[B];
+#pragma unroll
+          for (int j = 0; j < B; ++j) {
+            const uint32_t e = e0 + j * 32 + lane;
+            kb[j] = e < deg ? __ldcg(lab + e) : kEmpty;
+          }
+#pragma unroll
+          for (int j = 0; j < B; ++j) {
+            if (!wover) {
+              const bool in = kb[j] != kEmpty && (lowbias32(kb[j]) & (K - 1)) == cls;
+              const unsigned m = __ballot_sync(kFull, in);
+              if (in) {
+                const uint32_t pos = (head + pend + __popc(m & below)) & (kRateStage - 1);
+                stk[pos] = kb[j];
+                if (EW) {
+                  stw[pos] = a.adjwgt[beg + e0 + j * 32 + lane];
+                }
+              }
+              pend += __popc(m);
+              if (pend >= 32) {
+                __syncwarp();
+                const uint32_t sl = (head + lane) & (kRateStage - 1);
+                wover = rate_insert<EW>(keys, vals, list, &s_claims, limit, stk[sl], EW ? stw[sl] : 1, true, lane);
+                __syncwarp(); // the ring slots are read before they are staged again
+                head = (head + 32) & (kRateStage - 1);
+                pend -= 32;
+              }
+            }
+          }
+        }
+        if (!wover) { // insert the rest
+          __syncwarp();
+          const bool v = lane < pend;
+          const uint32_t sl = (head + lane) & (kRateStage - 1);
+          wover = rate_insert<EW>(keys, vals, list, &s_claims, limit, v ? stk[sl] : 0u, (EW && v) ? stw[sl] : 1, v, lane);
+        }
+        const bool over = __syncthreads_or(wover);
+        if (over) {
+          // more labels than the list takes: clear the whole table (not every claim is listed), split the class
+          // by the next hash bit and stream again
+          for (uint32_t s = tid; s < kRateSlots; s += T) {
+            keys[s] = kEmpty;
+            vals[s] = 0;
+          }
+          K <<= 1;
+          __syncthreads();
+          continue;
+        }
+        const uint32_t nc = s_claims;
+        // ---- select (as the team kernels): pass A without weights, pass B only if the top entry is full
+        Cand c = cand_none(), f = cand_none();
+        for (uint32_t l = tid; l < nc; l += T) {
+          const uint32_t s = list[l];
+          const uint32_t k = keys[s];
+          const int32_t r = vals[s] + (EW ? 0 : 1);
+          if (r > 0 && r >= c.gain) {
+            const Cand x{r, 0, tie_hash(a.base_tie, u, k), k};
+            if (cand_better<0>(x, c)) {
+              c = x;
+            }
+          }
+          if (store_fav && r > 0 && r >= f.gain) {
+            const Cand y{r, 0, tie_hash(a.base_fav, u, k), k};
+            if (cand_better<0>(y, f)) {
+              f = y;
+            }
+          }
+        }
+        Cand cb = team_argmax<0, T>(1, tid, c, s_red);
+        if (store_fav) {
+          const Cand cf = team_argmax<0, T>(1, tid, f, s_red);
+          if (cand_better<0>(cf, fav)) {
+            fav = cf;
+          }
+        }
+        bool top_ok = true;
+        if (cb.gain > 0) {
+          top_ok = (a.weight[cb.key] + uw <= a.max_cluster_weight) || (cb.key == own);
+          if (a.communities != nullptr) {
+            top_ok = top_ok && (a.communities[cb.key] == a.communities[own]);
+          }
+        }
+        if (!top_ok) {
+          Cand ce = cand_none();
+          for (uint32_t l0 = 0; l0 < nc; l0 += T * 4) {
+            uint32_t kk[4];
+            int32_t rr[4], ww[4];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              const uint32_t l = l0 + j * T + tid;
+              const uint32_t s = l < nc ? list[l] : 0u;
+              kk[j] = l < nc ? keys[s] : kEmpty;
+              rr[j] = l < nc ? vals[s] + (EW ? 0 : 1) : 0;
+            }
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              ww[j] = kk[j] != kEmpty ? a.weight[kk[j]] : 0;
+            }
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              if (kk[j] != kEmpty) {
+                Cand ff;
+                const Cand cc = eval_candidate_w<0>(a, u, own, uw, own_w, kk[j], rr[j], ww[j], false, ff);
+                if (cand_better<0>(cc, ce)) {
+                  ce = cc;
+                }
+              }
+            }
+          }
+          cb = team_argmax<0, T>(1, tid, ce, s_red);
+        }
+        if (cand_better<0>(cb, best)) {
+          best = cb;
+        }
+        // every thread clears the listed slots it scanned
+        for (uint32_t l = tid; l < nc; l += T) {
+          const uint32_t s = list[l];
+          keys[s] = kEmpty;
+          vals[s] = 0;
+        }
+        __syncthreads(); // table clean, s_claims read
+        // next class: the second half of the deepest split whose first half is done, up to the item's own class
+        bool done = true;
+        while (K > K0) {
+          const uint32_t half = K >> 1;
+          if ((cls & half) == 0) {
+            cls |= half;
+            done = false;
+            break;
+          }
+          cls &= ~half;
+          K = half;
+        }
+        if (done) {
+          break;
+        }
+      }
+      if (tid == 0) {
+        hb.part_best[hb.sel_begin[entry] + c0] = best;
+        hb.part_fav[hb.sel_begin[entry] + c0] = fav;
+      }
+    }
+    __syncthreads(); // s_item consumed
+  }
+}
+
+// final: one warp per hub: reduce its buckets' (clusterer: hash classes') candidates, then propose / store the
+// favored cluster.
 template <int MODE> __global__ void __launch_bounds__(256) sweep_hub_final(const SweepArgs a, const HubArgs hb) {
   const int lane = threadIdx.x & 31;
   const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -1222,7 +1503,7 @@ template <int MODE> __global__ void __launch_bounds__(256) sweep_hub_final(const
     const uint32_t own = a.label[u];
     const int32_t uw = a.vwgt != nullptr ? a.vwgt[u] : 1;
     const int32_t own_w = a.weight[own];
-    const uint32_t pieces = hub_buckets(full_deg);
+    const uint32_t pieces = MODE == 0 ? hub_classes(full_deg) : hub_buckets(full_deg);
     const uint32_t first = hb.sel_begin[i];
     const bool store_fav = (MODE == 0) && (uw == own_w) && (own_w <= a.max_cluster_weight / 2);
     Cand c = cand_none(), f = cand_none();
