@@ -15,6 +15,8 @@
 //   OverloadBalancer   kaminpar-shm/refinement/balancer/overload_balancer.h / overload_balancer.cc:40-160
 //   UnderloadBalancer  kaminpar-shm/refinement/balancer/underload_balancer.h / underload_balancer.cc:27-104
 //   CoarseGraph / contract_clustering  kaminpar-shm/coarsening/contraction/cluster_contraction.h:22-56
+//   sparsification_target / CoarseGraph::sparsify
+//                      kaminpar-shm/coarsening/sparsification_cluster_coarsener.cc:41-228 (DESIGN.md §13)
 //
 // Error convention: the reference's path has no error codes (KASSERT aborts); here a non-zero
 // status of the C ABI becomes std::runtime_error. There is no CPU fallback.
@@ -388,6 +390,15 @@ public:
     }
     detail::check(kmp_coarse_project_down(_g, fine.data(), coarse.data()));
   }
+  // Threshold sparsification in place (kmp_coarse_sparsify) on the handle that contracted this graph: vertices,
+  // weights and mapping stay, the edges are replaced. Drops the host copy get() made and invalidates device pointers
+  // taken earlier. The caller applies the laziness rule and draws the seed (INTEGRATION.md §2e).
+  kmp_sparsify_stats sparsify(kmp_lp_handle *graph_holder, EdgeID target_m, std::uint64_t seed) {
+    kmp_sparsify_stats st{};
+    detail::check(kmp_coarse_sparsify(graph_holder, _g, target_m, seed, &st));
+    _host = HostCSR{};
+    return st;
+  }
   [[nodiscard]] const kmp_contraction_stats &stats() const { return _stats; }
   [[nodiscard]] const kmp_coarse_graph *device() const { return _g; } // kmp_coarse_device_arrays for the next level
 
@@ -396,6 +407,13 @@ private:
   kmp_contraction_stats _stats;
   HostCSR _host;
 };
+
+// SparsificationClusterCoarsener::sparsification_target (sparsification_cluster_coarsener.cc:41-48): the edge count
+// a coarse graph of c_n vertices is sparsified to, from the previous level's (or the input graph's) prev_m / prev_n.
+inline EdgeID sparsification_target(EdgeID prev_m, NodeID prev_n, NodeID c_n, double density_target_factor = 0.5,
+                                    double edge_target_factor = 0.5) {
+  return kmp_sparsification_target(prev_m, prev_n, c_n, density_target_factor, edge_target_factor);
+}
 
 // contract_clustering(graph, clustering, con_ctx) (cluster_contraction.h:47-50). `clusterer` is the LP
 // clusterer that already holds `graph` on the device (no second H2D copy); an empty `clustering` span

@@ -72,6 +72,43 @@ int kmp_coarse_project_down(const kmp_coarse_graph *g, const uint32_t *fine, uin
  * kmp_lp_destroy of that handle. */
 void kmp_coarse_destroy(kmp_coarse_graph *g);
 
+/* ---- threshold edge sparsification (SparsificationClusterCoarsener, DESIGN.md §13) --------------------------
+ *
+ *   SparsificationClusterCoarsener::sparsification_target / recontract_with_threshold_sparsification
+ *       kaminpar-shm/coarsening/sparsification_cluster_coarsener.cc:41-48, 158-228
+ *
+ * The number of edges the coarse graph of a level is cut down to:
+ *   target = min(edge_target_factor * prev_m, density_target_factor * prev_m / prev_n * c_n)   (in double)
+ * truncated to an edge count if it is below prev_m, else prev_m. prev_m / prev_n belong to the previous level's
+ * graph (the input graph on the first level). Host function: no device work. */
+uint32_t kmp_sparsification_target(uint32_t prev_m, uint32_t prev_n, uint32_t c_n, double density_target_factor,
+                                   double edge_target_factor);
+
+typedef struct kmp_sparsify_stats {
+  uint32_t c_m_before;      /* directed edges before */
+  uint32_t c_m_after;       /* directed edges kept */
+  uint32_t target_m;
+  int32_t threshold;        /* T: the (c_m_before - target_m + 1)-th smallest edge weight (0 when target_m < 2) */
+  uint32_t smaller;         /* edges with w < T */
+  uint32_t equal;           /* edges with w == T */
+  uint32_t equal_kept;      /* of those, kept by the hash (c_m_after = c_m_before - smaller - equal + equal_kept) */
+  uint32_t kernel_launches;
+  float device_ms;          /* whole call on the device, including the one wait for the selection's read-back
+                               (the host computes p between the selection and the keep pass) */
+} kmp_sparsify_stats;
+
+/* Sparsifies g in place on the device, on the stream of h (the handle that contracted g). An edge (u, v, w) is
+ * kept iff w > T, or w == T and dice(u, v) < p, with p = (target_m - #{w > T}) / #{w == T} in double and
+ *   dice(u, v) = lo32(fmix64(((max(u, v) << 32) | min(u, v)) + seed)) / (2^32 - 1)
+ * (murmur3's 64-bit finaliser). Both tests are symmetric in u and v, so the graph stays undirected; adjacency lists
+ * stay sorted by target. target_m < 2 drops every edge (seed unused). Vertices, vertex weights and the mapping are
+ * unchanged; xadj / adjncy / adjwgt are replaced, so device pointers taken earlier by kmp_coarse_device_arrays
+ * are INVALID afterwards (the old arrays are freed). The caller applies the laziness rule and draws the seed, as
+ * the reference's coarsen() does. Refused (KMP_ERR_INVALID): null arguments, target_m > kmp_coarse_m(g), and a
+ * graph that lives on another device than h. stats may be NULL. */
+int kmp_coarse_sparsify(kmp_lp_handle *h, kmp_coarse_graph *g, uint32_t target_m, uint64_t seed,
+                        kmp_sparsify_stats *stats);
+
 #ifdef __cplusplus
 }
 #endif

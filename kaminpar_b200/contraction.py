@@ -5,6 +5,8 @@ include/kaminpar_b200_contraction.h (device code: kaminpar_b200/csrc/kmp_contrac
         kaminpar-shm/coarsening/contraction/cluster_contraction.h:47-56
     CoarseGraph.get() / project_up() / project_down()
         kaminpar-shm/coarsening/contraction/cluster_contraction.h:22-32
+    sparsification_target(...), CoarseGraph.sparsify(...), sparsify_level(...)
+        kaminpar-shm/coarsening/sparsification_cluster_coarsener.cc:41-228 (DESIGN.md §13)
 
 There is no CPU fallback: without the CUDA library / a GPU every call raises.
 """
@@ -32,6 +34,30 @@ class ContractionStats(C.Structure):
     ]
 
 
+class SparsifyStats(C.Structure):
+    """kmp_sparsify_stats."""
+
+    _fields_ = [
+        ("c_m_before", C.c_uint32),
+        ("c_m_after", C.c_uint32),
+        ("target_m", C.c_uint32),
+        ("threshold", C.c_int32),
+        ("smaller", C.c_uint32),
+        ("equal", C.c_uint32),
+        ("equal_kept", C.c_uint32),
+        ("kernel_launches", C.c_uint32),
+        ("device_ms", C.c_float),
+    ]
+
+
+class SparsificationClusterCoarseningContext:  # kaminpar.h:185-189, defaults presets.cc:172-177
+    def __init__(self, density_target_factor: float = 0.5, edge_target_factor: float = 0.5,
+                 laziness_factor: float = 4.0):
+        self.density_target_factor = density_target_factor
+        self.edge_target_factor = edge_target_factor
+        self.laziness_factor = laziness_factor
+
+
 class ContractionCoarseningContext:  # kaminpar.h (ContractionCoarseningContext), defaults presets.cc:181-185
     """Accepted for interface compatibility. The reference's `algorithm` / `unbuffered_implementation`
     choose between CPU data structures with the same result; the device path has one algorithm."""
@@ -49,6 +75,12 @@ def _lib():
         lib.kmp_coarse_m.restype = C.c_uint32
         lib.kmp_coarse_fine_n.restype = C.c_uint32
         lib.kmp_coarse_destroy.restype = None
+        for sym in ("kmp_sparsification_target", "kmp_coarse_sparsify"):
+            if not hasattr(lib, sym):
+                raise RuntimeError(f"{lp.library_path()} lacks {sym}; rebuild the library")
+        lib.kmp_sparsification_target.restype = C.c_uint32
+        lib.kmp_sparsification_target.argtypes = [C.c_uint32, C.c_uint32, C.c_uint32, C.c_double, C.c_double]
+        lib.kmp_coarse_sparsify.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64, C.c_void_p]
         lib._contraction_ready = True
     return lib
 
@@ -117,6 +149,17 @@ class CoarseGraph:
         lp._check(_lib().kmp_coarse_project_down(self._g, lp._ptr(fine), lp._ptr(coarse)))
         return coarse
 
+    def sparsify(self, handle: lp.LPHandle, target_m: int, seed: int) -> SparsifyStats:
+        """kmp_coarse_sparsify: keep the edges above the threshold weight and a hashed share of those at it, until
+        about `target_m` directed edges remain (DESIGN.md §13). `handle` is the one that contracted this graph.
+        Vertices, vertex weights and the mapping stay; earlier `device_arrays()` pointers become invalid."""
+        stats = SparsifyStats()
+        lp._check(_lib().kmp_coarse_sparsify(handle._h, self._g, C.c_uint32(int(target_m)),
+                                              C.c_uint64(int(seed) & 0xFFFFFFFFFFFFFFFF), C.byref(stats)))
+        self._host = None
+        self.sparsify_stats = stats
+        return stats
+
     def close(self):
         if getattr(self, "_g", None):
             _lib().kmp_coarse_destroy(self._g)  # frees on the handle's stream: the handle must still exist
@@ -132,6 +175,38 @@ class CoarseGraph:
             self.close()
         except Exception:
             pass
+
+
+def sparsification_target(prev_m: int, prev_n: int, c_n: int, density_target_factor: float = 0.5,
+                          edge_target_factor: float = 0.5) -> int:
+    """SparsificationClusterCoarsener::sparsification_target (sparsification_cluster_coarsener.cc:41-48), computed by
+    the library so that every caller evaluates the same double expression."""
+    return int(_lib().kmp_sparsification_target(int(prev_m), int(prev_n), int(c_n), float(density_target_factor),
+                                                float(edge_target_factor)))
+
+
+def sparsify_level(handle: lp.LPHandle, cg: CoarseGraph, prev_m: int, prev_n: int,
+                   ctx: Optional[SparsificationClusterCoarseningContext] = None, seed=0) -> bool:
+    """The sparsification step of SparsificationClusterCoarsener::coarsen() (:50-156) on a contracted level:
+    sparsify iff c_m > laziness_factor * target (:89). `prev_m` / `prev_n` belong to the previous level's graph (the
+    input graph on the first level). `seed` is an int or a callable that draws one; it is called only when the
+    reference draws its seed, i.e. when sparsification runs with target >= 2. Returns whether it sparsified.
+
+    With laziness_factor < 1 the rule can ask to sparsify a level whose target exceeds its edge count; the
+    reference's selection rank c_m - target + 1 underflows there, so this is refused with ValueError (no seed is
+    drawn, the graph is left as it is)."""
+    ctx = ctx or SparsificationClusterCoarseningContext()
+    target = sparsification_target(prev_m, prev_n, cg.n, ctx.density_target_factor, ctx.edge_target_factor)
+    if not float(cg.m) > ctx.laziness_factor * target:
+        return False
+    if target > cg.m:
+        raise ValueError(f"sparsification target {target} exceeds the level's {cg.m} edges (laziness_factor "
+                         f"{ctx.laziness_factor} < 1): the reference's threshold selection is undefined there")
+    s = 0
+    if target >= 2:
+        s = seed() if callable(seed) else seed
+    cg.sparsify(handle, target, s)
+    return True
 
 
 def contract_on_handle(handle: lp.LPHandle, clustering: Optional[np.ndarray]) -> CoarseGraph:

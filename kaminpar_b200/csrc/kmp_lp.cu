@@ -207,6 +207,7 @@ struct kmp_lp_handle {
   DevBuf<int32_t> ct_vals_a, ct_vals_b;
   DevBuf<uint32_t> ct_flags, ct_rank, ct_cl;
   DevBuf<unsigned long long> ct_counter;
+  DevBuf<uint32_t> sp_ctl; // sparsification (kmp_sparsify.cuh): radix-select bins, select state, kept counter
   bool slot_state_clean = false; // incoming/slotmap/chist zeroed for current n
 
   // schedule KMP_SCHEDULE_SEQ_STRICT (lp_strict.cuh): sequential engine state
@@ -2550,6 +2551,7 @@ int kmp_lp_free_scratch(kmp_lp_handle *h) {
   h->ct_rank.release();
   h->ct_cl.release();
   h->ct_counter.release();
+  h->sp_ctl.release();
   for (DevBuf<uint32_t> *b : {&h->bal_cand, &h->bal_under, &h->bal_ctr32, &h->bal_target, &h->bal_lists, &h->bal_sv_a,
                               &h->bal_sv_b, &h->bal_blk}) {
     b->release();
@@ -2883,5 +2885,6 @@ int kmp_lp_step_finish(kmp_lp_handle *h, uint32_t *labels_out, int32_t *block_we
 } // extern "C"
 
 #include "kmp_contract.cuh"
+#include "kmp_sparsify.cuh"
 #include "kmp_balance.cuh"
 #include "kmp_underload.cuh"
