@@ -46,7 +46,8 @@ typedef struct kmp_balance_stats {
 } kmp_balance_stats;
 
 /* OverloadBalancer::refine on the graph the handle holds. partition_inout: HOST buffer of n BlockIDs, balanced in
- * place, or NULL = the labels left on the device by kmp_lp_upload_partition / kmp_lp_refine (they stay there).
+ * place, or NULL = the labels left on the device by kmp_lp_upload_partition / kmp_lp_refine (they stay there;
+ * KMP_ERR_INVALID when the device holds no labels of the current graph, or labels >= k).
  * max_block_weights[k] (PartitionContext::max_block_weight), perfectly_balanced_block_weights[k]
  * (PartitionContext::perfectly_balanced_block_weight; the floating-point part stays with the caller).
  * block_weights_out[k] nullable, stats nullable. *improved_out = the reference's return value: 0 when the input
@@ -95,7 +96,7 @@ typedef struct kmp_underload_stats {
 } kmp_underload_stats;
 
 /* UnderloadBalancer::refine on the graph the handle holds. partition_inout: HOST buffer of n BlockIDs, balanced in
- * place, or NULL = the labels on the device (they stay there). max_block_weights[k], min_block_weights[k]
+ * place, or NULL = the labels on the device (they stay there; refused as by kmp_overload_balance). max_block_weights[k], min_block_weights[k]
  * (PartitionContext::min_block_weight). min_block_weights = NULL means the context has no minimum weights: then
  * *improved_out = 0 and nothing runs on the device (block_weights_out is not written). block_weights_out[k]
  * nullable, stats nullable. *improved_out = the reference's return value: 0 when every block is at or above its

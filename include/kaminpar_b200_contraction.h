@@ -47,7 +47,8 @@ typedef struct kmp_contraction_stats {
 } kmp_contraction_stats;
 
 /* clustering: host array of n cluster (leader) ids in [0, n) -- what kmp_lp_cluster returns -- or
- * NULL to contract by the labels the last kmp_lp_cluster / kmp_lp_upload_partition left on the device.
+ * NULL to contract by the labels the last kmp_lp_cluster / kmp_lp_upload_partition left on the device
+ * for the current graph (KMP_ERR_INVALID when there are none since the last set_graph / free_scratch).
  * The caller owns *out (kmp_coarse_destroy). stats may be NULL. */
 int kmp_contract_clustering(kmp_lp_handle *h, const uint32_t *clustering, kmp_coarse_graph **out,
                             kmp_contraction_stats *stats);

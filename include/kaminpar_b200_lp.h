@@ -161,9 +161,13 @@ int kmp_lp_cluster(kmp_lp_handle *h, int32_t max_cluster_weight, uint32_t desire
                    const uint32_t *communities, uint32_t *clustering_out, kmp_lp_stats *stats);
 
 /* LabelPropagationRefiner::refine. partition_inout: HOST buffer of n BlockIDs, refined in place
- * (NULL: operate on the partition already on the device from kmp_lp_upload_partition).
+ * (NULL: operate on the labels already on the device for the current graph, e.g. from
+ * kmp_lp_upload_partition; refused with KMP_ERR_INVALID when there are none since the last
+ * set_graph / kmp_lp_free_scratch). Labels >= k on either path are refused with KMP_ERR_INVALID
+ * before any kernel indexes a [k] array by them (a clustering is not a k-way partition).
  * max_block_weights[k] (PartitionContext::max_block_weight, per block), min_block_weights[k]
- * nullable (PartitionContext::min_block_weight). block_weights_out[k] nullable. */
+ * nullable (PartitionContext::min_block_weight). block_weights_out[k] nullable. The sync hashes
+ * use the number of kmp_lp_cluster calls the handle completed before (0 if it only refines). */
 int kmp_lp_refine(kmp_lp_handle *h, uint32_t k, const int32_t *max_block_weights,
                   const int32_t *min_block_weights, const uint32_t *communities,
                   uint32_t *partition_inout, int32_t *block_weights_out, kmp_lp_stats *stats);
@@ -189,7 +193,8 @@ int kmp_lp_free_scratch(kmp_lp_handle *h);
 /* Enable per-kernel CUDA-event timing of the sweep kernels (serialises nothing, adds events). */
 int kmp_lp_set_timing(kmp_lp_handle *h, int enabled);
 
-/* Metrics on the device (metrics.cc:36-53): edge cut of the labels currently on the device. */
+/* Metrics on the device (metrics.cc:36-53): edge cut of the labels currently on the device
+ * (KMP_ERR_INVALID when they do not belong to the current graph). */
 int kmp_lp_edge_cut(kmp_lp_handle *h, int64_t *cut_out);
 
 /* ---- Stepping API: one LP sub-round at a time (sharded multi-GPU driver) ----------------------

@@ -295,18 +295,6 @@ __global__ void __launch_bounds__(kBalCtaThreads) bal_eval_cta(const BalArgs a) 
 }
 
 // ---- round set-up and selection ----------------------------------------------------------------------------
-// block weights from labels; counts labels >= k (a clustering is not a partition) into *bad
-__global__ void bal_block_weights(uint32_t n, uint32_t k, const int32_t *vwgt, const uint32_t *label, int32_t *weight,
-                                  unsigned long long *bad) {
-  for (uint32_t u = blockIdx.x * blockDim.x + threadIdx.x; u < n; u += gridDim.x * blockDim.x) {
-    const uint32_t b = label[u];
-    if (b < k) {
-      atomicAdd(&weight[b], vwgt != nullptr ? vwgt[u] : 1);
-    } else {
-      atomicAdd(bad, 1ull);
-    }
-  }
-}
 // over[b], the total overload (ctrl[0]) and the flags of the underloaded blocks (targets of internal vertices)
 __global__ void bal_block_stats(uint32_t k, const int32_t *weight, const int32_t *max_w, const int32_t *pbw, int32_t *over,
                                 uint8_t *under, unsigned long long *ctrl) {
@@ -572,8 +560,8 @@ int kmp_overload_balance(kmp_lp_handle *h, uint32_t k, const int32_t *max_block_
     return fail(KMP_ERR_INVALID, "k / max_block_weights / perfectly_balanced_block_weights missing");
   }
   const uint32_t n = h->n;
-  if (partition_inout == nullptr && h->label.cap < std::max<uint32_t>(n, 1)) {
-    return fail(KMP_ERR_INVALID, "no partition on the device: pass partition_inout or call kmp_lp_upload_partition");
+  if (partition_inout == nullptr && (rc = refuse_without_labels(h)) != KMP_OK) {
+    return rc;
   }
   KMP_CUDA(cudaSetDevice(h->device));
   if (stats != nullptr) {
@@ -598,21 +586,18 @@ int kmp_overload_balance(kmp_lp_handle *h, uint32_t k, const int32_t *max_block_
   if (partition_inout != nullptr && n > 0) {
     KMP_CUDA(cudaMemcpyAsync(h->label.p, partition_inout, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, st));
   }
+  if (partition_inout != nullptr) {
+    h->labels_valid = true;
+  }
   KMP_CUDA(cudaMemcpyAsync(h->maxw.p, max_block_weights, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, st));
   KMP_CUDA(cudaMemcpyAsync(h->bal_pbw.p, perfectly_balanced_block_weights, static_cast<size_t>(k) * 4,
                            cudaMemcpyHostToDevice, st));
   KMP_CUDA(cudaMemsetAsync(h->weight.p, 0, static_cast<size_t>(k) * 4, st));
   KMP_CUDA(cudaMemsetAsync(h->bal_ctrl.p, 0, 8 * sizeof(unsigned long long), st));
   KMP_CUDA(cudaMemsetAsync(h->bal_ctr32.p, 0, (4 + kBalMaxRounds) * sizeof(uint32_t), st));
-  bal_block_weights<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, k, h->vwgt, h->label.p, h->weight.p,
-                                                                 h->bal_ctrl.p + 3);
-  ++h->kernel_launches;
-  // labels >= k (e.g. a clustering left on the device): refused before any kernel indexes a [k] array by a label
-  unsigned long long bad = 0;
-  KMP_CUDA(cudaMemcpyAsync(&bad, h->bal_ctrl.p + 3, sizeof(bad), cudaMemcpyDeviceToHost, st));
-  KMP_CUDA(cudaStreamSynchronize(st));
-  if (bad != 0) {
-    return fail(KMP_ERR_INVALID, "labels >= k on the device: a clustering is not a k-way partition");
+  rc = checked_block_weights(h, k, h->bal_ctrl.p + 3);
+  if (rc != KMP_OK) {
+    return rc;
   }
   const uint32_t call = h->bal_calls++;
   unsigned long long ctrl[4] = {0, 0, 0, 0};

@@ -287,10 +287,7 @@ int contract_impl(kmp_lp_handle *h, const uint32_t *clustering, kmp_coarse_graph
     KMP_CUDA(cudaMemcpyAsync(d_cl.p, clustering, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, st));
     cl = d_cl.p;
   } else {
-    if (h->label.cap < n) {
-      return fail(KMP_ERR_INVALID, "no clustering on the device: run kmp_lp_cluster first or pass one");
-    }
-    cl = h->label.p;
+    cl = h->label.p; // kmp_contract_clustering refused labels of another graph
   }
   // a dedicated event pair (the handle's own pair may bracket an open stepping call -- ADVICE r1)
   if (h->ev_ct0 == nullptr) {
@@ -430,6 +427,10 @@ int kmp_contract_clustering(kmp_lp_handle *h, const uint32_t *clustering, kmp_co
   if (!h->have_graph) {
     return fail(KMP_ERR_INVALID, "no graph set");
   }
+  int rc = clustering == nullptr ? refuse_without_labels(h) : KMP_OK;
+  if (rc != KMP_OK) {
+    return rc;
+  }
   KMP_CUDA(cudaSetDevice(h->device));
   if (stats != nullptr) {
     std::memset(stats, 0, sizeof(*stats));
@@ -438,7 +439,7 @@ int kmp_contract_clustering(kmp_lp_handle *h, const uint32_t *clustering, kmp_co
   if (cg == nullptr) {
     return fail(KMP_ERR_ALLOC, "out of host memory");
   }
-  const int rc = contract_impl(h, clustering, cg, stats);
+  rc = contract_impl(h, clustering, cg, stats);
   if (rc != KMP_OK) {
     kmp_coarse_destroy(cg);
     return rc;

@@ -162,6 +162,10 @@ struct kmp_lp_handle {
 
   // state
   DevBuf<uint32_t> label, favored, communities;
+  // label[] belongs to the current graph: set by a completed clustering, kmp_lp_upload_partition and a refine or
+  // balancer call given a partition; cleared by a new graph and by kmp_lp_free_scratch. The calls that read the
+  // labels on the device (a NULL partition or clustering) refuse while it is clear.
+  bool labels_valid = false;
   DevBuf<int32_t> weight, maxw, minw;
   DevBuf<uint8_t> active;
   // scratch
@@ -259,6 +263,22 @@ struct kmp_lp_handle {
   DevBuf<int32_t> ubal_deficit;
   DevBuf<uint8_t> ubal_tmask;
 };
+
+namespace kmp {
+// block weights from labels; counts labels >= k (a clustering is not a partition) into *bad. The one range check
+// of the refiner and both balancers (checked_block_weights).
+__global__ void bal_block_weights(uint32_t n, uint32_t k, const int32_t *vwgt, const uint32_t *label, int32_t *weight,
+                                  unsigned long long *bad) {
+  for (uint32_t u = blockIdx.x * blockDim.x + threadIdx.x; u < n; u += gridDim.x * blockDim.x) {
+    const uint32_t b = label[u];
+    if (b < k) {
+      atomicAdd(&weight[b], vwgt != nullptr ? vwgt[u] : 1);
+    } else {
+      atomicAdd(bad, 1ull);
+    }
+  }
+}
+} // namespace kmp
 
 namespace {
 
@@ -363,11 +383,6 @@ template <bool P64> __global__ void k_age_stamps(uint32_t n, void *labg, uint32_
 __global__ void k_fill_u8(uint32_t n, uint8_t *p, uint8_t v) {
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     p[i] = v;
-  }
-}
-__global__ void k_block_weights(uint32_t n, const int32_t *vwgt, const uint32_t *label, int32_t *weight) {
-  for (uint32_t u = blockIdx.x * blockDim.x + threadIdx.x; u < n; u += gridDim.x * blockDim.x) {
-    atomicAdd(&weight[label[u]], vwgt != nullptr ? vwgt[u] : 1);
   }
 }
 __global__ void k_count_nonzero(uint32_t n, const int32_t *w, uint32_t *out) {
@@ -1619,6 +1634,32 @@ void launch_pack_labels(kmp_lp_handle *h) {
   }
 }
 
+// The labels on the device as a k-way partition: weight[0, k) (zeroed by the caller) += their block weights, and
+// labels >= k (e.g. a clustering left on the device, or a host partition with an id >= k) are refused before any
+// kernel indexes a [k] array by a label. bad: a zeroed device counter. One n-sized read and one host wait.
+int checked_block_weights(kmp_lp_handle *h, uint32_t k, unsigned long long *bad) {
+  const uint32_t n = h->n;
+  if (n > 0) {
+    bal_block_weights<<<capped(h, grid_for(n, 256)), 256, 0, h->stream>>>(n, k, h->vwgt, h->label.p, h->weight.p, bad);
+    ++h->kernel_launches;
+  }
+  unsigned long long b = 0;
+  KMP_CUDA(cudaMemcpyAsync(&b, bad, sizeof(b), cudaMemcpyDeviceToHost, h->stream));
+  KMP_CUDA(cudaStreamSynchronize(h->stream));
+  if (b != 0) {
+    return fail(KMP_ERR_INVALID, "labels >= k on the device: a clustering is not a k-way partition");
+  }
+  return KMP_OK;
+}
+
+int refuse_without_labels(const kmp_lp_handle *h) {
+  if (!h->labels_valid) {
+    return fail(KMP_ERR_INVALID, "no labels of the current graph on the device: cluster, pass a partition or call "
+                                 "kmp_lp_upload_partition first");
+  }
+  return KMP_OK;
+}
+
 int begin_call(kmp_lp_handle *h, kmp_lp_stats *stats) {
   if (h == nullptr || !h->have_graph) {
     return fail(KMP_ERR_INVALID, "no graph set");
@@ -1878,6 +1919,7 @@ int strict_cluster(kmp_lp_handle *h, int32_t max_cluster_weight, uint32_t desire
     KMP_CUDA(cudaMemcpyAsync(clustering_out, h->label.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, h->stream));
   }
   ++h->call_counter;
+  h->labels_valid = true;
   const kmp_lp_stats keep = stats != nullptr ? *stats : kmp_lp_stats{};
   rc = end_call(h, stats);
   if (stats != nullptr) { // end_call fills the timing / counter fields only
@@ -1901,6 +1943,14 @@ int strict_refine(kmp_lp_handle *h, uint32_t k, const int32_t *max_block_weights
   if (partition_inout != nullptr && n > 0) {
     KMP_CUDA(cudaMemcpyAsync(h->label.p, partition_inout, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, h->stream));
   }
+  if (partition_inout != nullptr) {
+    h->labels_valid = true;
+  }
+  KMP_CUDA(cudaMemsetAsync(h->weight.p, 0, static_cast<size_t>(k) * 4, h->stream));
+  int rc = checked_block_weights(h, k, h->ctr64.p + kCtrScratch); // the engine recomputes the weights itself
+  if (rc != KMP_OK) {
+    return rc;
+  }
   KMP_CUDA(cudaMemcpyAsync(h->maxw.p, max_block_weights, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, h->stream));
   if (min_block_weights != nullptr) {
     KMP_CUDA(h->minw.ensure(k));
@@ -1910,7 +1960,7 @@ int strict_refine(kmp_lp_handle *h, uint32_t k, const int32_t *max_block_weights
     KMP_CUDA(h->communities.ensure(n));
     KMP_CUDA(cudaMemcpyAsync(h->communities.p, communities, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, h->stream));
   }
-  int rc = run_strict(h, 1, k, 0, 0, k, min_block_weights != nullptr, communities != nullptr, stats);
+  rc = run_strict(h, 1, k, 0, 0, k, min_block_weights != nullptr, communities != nullptr, stats);
   if (rc != KMP_OK) {
     return rc;
   }
@@ -2144,6 +2194,7 @@ static int set_graph_common(kmp_lp_handle *h, uint32_t n, uint32_t m) {
   h->n = n;
   h->m = m;
   h->have_graph = true;
+  h->labels_valid = false;
   h->lists_valid = false;
   h->slot_state_clean = false;
   h->graph_sorted = false;
@@ -2321,6 +2372,7 @@ int kmp_lp_cluster(kmp_lp_handle *h, int32_t max_cluster_weight, uint32_t desire
     KMP_CUDA(cudaMemcpyAsync(clustering_out, h->label.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, h->stream));
   }
   ++h->call_counter;
+  h->labels_valid = true;
   return end_call(h, stats);
 }
 
@@ -2332,6 +2384,7 @@ int kmp_lp_upload_partition(kmp_lp_handle *h, const uint32_t *partition) {
   KMP_CUDA(h->label.ensure(h->n));
   KMP_CUDA(cudaMemcpyAsync(h->label.p, partition, static_cast<size_t>(h->n) * 4, cudaMemcpyHostToDevice, h->stream));
   KMP_CUDA(cudaStreamSynchronize(h->stream));
+  h->labels_valid = true;
   return KMP_OK;
 }
 
@@ -2355,6 +2408,9 @@ int kmp_lp_refine(kmp_lp_handle *h, uint32_t k, const int32_t *max_block_weights
   }
   int rc = begin_call(h, stats);
   if (rc != KMP_OK) {
+    return rc;
+  }
+  if (partition_inout == nullptr && (rc = refuse_without_labels(h)) != KMP_OK) {
     return rc;
   }
   if (h->cfg.schedule == KMP_SCHEDULE_SEQ_STRICT) {
@@ -2383,6 +2439,9 @@ int kmp_lp_refine(kmp_lp_handle *h, uint32_t k, const int32_t *max_block_weights
   if (partition_inout != nullptr && n > 0) {
     KMP_CUDA(cudaMemcpyAsync(h->label.p, partition_inout, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, h->stream));
   }
+  if (partition_inout != nullptr) {
+    h->labels_valid = true;
+  }
   KMP_CUDA(cudaMemcpyAsync(h->maxw.p, max_block_weights, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, h->stream));
   if (min_block_weights != nullptr) {
     KMP_CUDA(h->minw.ensure(k));
@@ -2395,10 +2454,13 @@ int kmp_lp_refine(kmp_lp_handle *h, uint32_t k, const int32_t *max_block_weights
   KMP_CUDA(cudaMemsetAsync(h->ctr64.p, 0, kCtrSize * sizeof(unsigned long long), h->stream));
   KMP_CUDA(cudaMemsetAsync(h->weight.p, 0, static_cast<size_t>(k) * 4, h->stream));
   if (n > 0) {
-    k_block_weights<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->vwgt, h->label.p, h->weight.p);
     k_fill_u8<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->active.p, 1); // Base::initialize: all active
-    launch_pack_labels(h);
-    h->kernel_launches += 3;
+    launch_pack_labels(h); // reads the labels without indexing by them
+    h->kernel_launches += 2;
+  }
+  rc = checked_block_weights(h, k, h->ctr64.p + kCtrScratch); // last: its wait covers the set-up above
+  if (rc != KMP_OK) {
+    return rc;
   }
   RunCtx ctx{1, k, 0, min_block_weights != nullptr, communities != nullptr};
   const uint64_t max_it = h->cfg.num_iterations == 0 ? ~0ull : h->cfg.num_iterations; // lp_refiner.cc:78-79
@@ -2510,6 +2572,7 @@ int kmp_lp_free_scratch(kmp_lp_handle *h) {
   cudaSetDevice(h->device);
   cudaStreamSynchronize(h->stream);
   h->label.release();
+  h->labels_valid = false;
   h->favored.release();
   h->communities.release();
   h->weight.release();
@@ -2579,6 +2642,10 @@ int kmp_lp_free_scratch(kmp_lp_handle *h) {
 int kmp_lp_edge_cut(kmp_lp_handle *h, int64_t *cut_out) {
   if (h == nullptr || !h->have_graph || cut_out == nullptr || h->label.p == nullptr) {
     return fail(KMP_ERR_INVALID, "bad argument");
+  }
+  const int rc = refuse_without_labels(h);
+  if (rc != KMP_OK) {
+    return rc;
   }
   KMP_CUDA(cudaSetDevice(h->device));
   KMP_CUDA(h->ctr64.ensure(kCtrSize));
@@ -2760,6 +2827,7 @@ int kmp_lp_step_begin_refine(kmp_lp_handle *h, uint32_t k, const int32_t *max_bl
     return rc;
   }
   KMP_CUDA(cudaMemcpyAsync(h->label.p, partition, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, h->stream));
+  h->labels_valid = true;
   KMP_CUDA(cudaMemcpyAsync(h->maxw.p, max_block_weights, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, h->stream));
   if (min_block_weights != nullptr) {
     KMP_CUDA(h->minw.ensure(k));
@@ -2775,8 +2843,11 @@ int kmp_lp_step_begin_refine(kmp_lp_handle *h, uint32_t k, const int32_t *max_bl
   if (rc != KMP_OK) {
     return rc;
   }
+  rc = checked_block_weights(h, k, h->ctr64.p + kCtrScratch);
+  if (rc != KMP_OK) {
+    return rc;
+  }
   if (n > 0) {
-    k_block_weights<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->vwgt, h->label.p, h->weight.p);
     k_fill_u8<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->active.p, 1);
     launch_pack_labels(h);
   }
@@ -2870,6 +2941,7 @@ int kmp_lp_step_finish(kmp_lp_handle *h, uint32_t *labels_out, int32_t *block_we
       return rc;
     }
     ++h->call_counter;
+    h->labels_valid = true;
   }
   if (labels_out != nullptr && n > 0) {
     KMP_CUDA(cudaMemcpyAsync(labels_out, h->label.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, h->stream));

@@ -220,6 +220,9 @@ int kmp_underload_balance(kmp_lp_handle *h, uint32_t k, const int32_t *max_block
   if (k == 0 || max_block_weights == nullptr) {
     return fail(KMP_ERR_INVALID, "k / max_block_weights missing");
   }
+  if (partition_inout == nullptr && (rc = refuse_without_labels(h)) != KMP_OK) {
+    return rc;
+  }
   if (stats != nullptr) {
     std::memset(stats, 0, sizeof(*stats));
   }
@@ -230,9 +233,6 @@ int kmp_underload_balance(kmp_lp_handle *h, uint32_t k, const int32_t *max_block
     return KMP_OK;
   }
   const uint32_t n = h->n;
-  if (partition_inout == nullptr && h->label.cap < std::max<uint32_t>(n, 1)) {
-    return fail(KMP_ERR_INVALID, "no partition on the device: pass partition_inout or call kmp_lp_upload_partition");
-  }
   KMP_CUDA(cudaSetDevice(h->device));
   h->kernel_launches = 0;
   cudaStream_t st = h->stream;
@@ -254,20 +254,17 @@ int kmp_underload_balance(kmp_lp_handle *h, uint32_t k, const int32_t *max_block
   if (partition_inout != nullptr && n > 0) {
     KMP_CUDA(cudaMemcpyAsync(h->label.p, partition_inout, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, st));
   }
+  if (partition_inout != nullptr) {
+    h->labels_valid = true;
+  }
   KMP_CUDA(cudaMemcpyAsync(h->maxw.p, max_block_weights, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, st));
   KMP_CUDA(cudaMemcpyAsync(h->minw.p, min_block_weights, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, st));
   KMP_CUDA(cudaMemsetAsync(h->weight.p, 0, static_cast<size_t>(k) * 4, st));
   KMP_CUDA(cudaMemsetAsync(h->bal_ctrl.p, 0, 8 * sizeof(unsigned long long), st));
   KMP_CUDA(cudaMemsetAsync(h->bal_ctr32.p, 0, (4 + kBalMaxRounds) * sizeof(uint32_t), st));
-  bal_block_weights<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, k, h->vwgt, h->label.p, h->weight.p,
-                                                                 h->bal_ctrl.p + 3);
-  ++h->kernel_launches;
-  // labels >= k (e.g. a clustering left on the device): refused before any kernel indexes a [k] array by a label
-  unsigned long long bad = 0;
-  KMP_CUDA(cudaMemcpyAsync(&bad, h->bal_ctrl.p + 3, sizeof(bad), cudaMemcpyDeviceToHost, st));
-  KMP_CUDA(cudaStreamSynchronize(st));
-  if (bad != 0) {
-    return fail(KMP_ERR_INVALID, "labels >= k on the device: a clustering is not a k-way partition");
+  rc = checked_block_weights(h, k, h->bal_ctrl.p + 3);
+  if (rc != KMP_OK) {
+    return rc;
   }
   const uint32_t call = h->ubal_calls++;
   unsigned long long ctrl[2] = {0, 0};

@@ -292,8 +292,16 @@ def oracle_rearrange(g, remove_isolated=True):
 SEQ, SYNC = 0, 1
 
 
+def _sync_only(schedule, call_index):
+    if call_index != 0 and schedule != SYNC:
+        raise ValueError("call_index is a key of the sync schedule; seq replays earlier calls (num_calls)")
+
+
 def oracle_lp_cluster(g, seed, max_cluster_weight, schedule=SEQ, desired=0, params=None, num_calls=1,
-                      communities=None, return_stats=False):
+                      communities=None, return_stats=False, call_index=0):
+    """call_index (sync): how many clusterings the device handle computed before this one, on any graph
+    (DESIGN.md, "parity across levels and calls"); with num_calls > 1 the calls take call_index, call_index + 1, ..."""
+    _sync_only(schedule, call_index)
     if not isinstance(params, OracleParams):
         params = oracle_params(params or default_cluster_params())
     b, nb = graph_buckets(g)
@@ -302,14 +310,17 @@ def oracle_lp_cluster(g, seed, max_cluster_weight, schedule=SEQ, desired=0, para
     oracle().lpo_lp_cluster(
         C.c_int(schedule), *_garrs(g), b.ctypes.data_as(C.c_void_p), C.c_uint32(nb), C.c_int(seed),
         C.c_int32(max_cluster_weight), C.c_uint32(desired), _opt(communities, np.uint32), C.byref(params),
-        C.c_int(num_calls), out.ctypes.data_as(C.c_void_p), stats,
+        C.c_int(num_calls), out.ctypes.data_as(C.c_void_p), stats, C.c_uint32(call_index),
     )
     res = out if num_calls == 1 else out.reshape(num_calls, g.n)
     return (res, stats) if return_stats else res
 
 
 def oracle_lp_refine(g, seed, k, max_block_weights, partition, schedule=SEQ, params=None, min_block_weights=None,
-                     communities=None, return_stats=False):
+                     communities=None, return_stats=False, call_index=0):
+    """call_index (sync): the number of clusterings the device handle computed before this refinement (0 for a
+    handle that only refines)."""
+    _sync_only(schedule, call_index)
     if not isinstance(params, OracleParams):
         params = oracle_params(params or default_refine_params())
     b, nb = graph_buckets(g)
@@ -321,6 +332,7 @@ def oracle_lp_refine(g, seed, k, max_block_weights, partition, schedule=SEQ, par
         C.c_int(schedule), *_garrs(g), b.ctypes.data_as(C.c_void_p), C.c_uint32(nb), C.c_int(seed), C.c_uint32(k),
         mbw.ctypes.data_as(C.c_void_p), _opt(min_block_weights, np.int32), _opt(communities, np.uint32),
         C.byref(params), part.ctypes.data_as(C.c_void_p), bw.ctypes.data_as(C.c_void_p), C.byref(stats),
+        C.c_uint32(call_index),
     )
     return (part, bw, stats) if return_stats else (part, bw)
 

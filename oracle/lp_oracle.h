@@ -78,22 +78,25 @@ int32_t lpo_max_cluster_weight(uint32_t n, int64_t total_node_weight, uint32_t k
 int32_t lpo_max_block_weight(int64_t total_node_weight, uint32_t k, double epsilon);
 
 /* ---- the path ---------------------------------------------------------------------------- */
-/* schedule: 0 = seq, 1 = sync. buckets/num_buckets as produced above. call_index: how many times
- * compute_clustering was called on this object before (sync: enters the RNG key; seq: the caller
- * must replay earlier calls itself, use num_calls). */
+/* schedule: 0 = seq, 1 = sync. buckets/num_buckets as produced above. Runs num_calls calls on the same
+ * graph. first_call (sync only; seq returns -1 unless it is 0): the call index of the first of them,
+ * i.e. how many kmp_lp_cluster calls the device handle ran before, on any graph -- it enters the
+ * hash keys of the sync schedule. seq: the caller replays earlier calls itself with num_calls. */
 int lpo_lp_cluster(int schedule, uint32_t n, uint32_t m, const uint32_t *xadj, const uint32_t *adjncy,
                    const int32_t *vwgt, const int32_t *adjwgt, const uint32_t *buckets,
                    uint32_t num_buckets, int seed, int32_t max_cluster_weight,
                    uint32_t desired_num_clusters, const uint32_t *communities /*nullable*/,
                    const lpo_params *params, int num_calls, uint32_t *out_clustering /* n*num_calls */,
-                   lpo_stats *stats /* num_calls, nullable */);
+                   lpo_stats *stats /* num_calls, nullable */, uint32_t first_call);
 
+/* call_index (sync only; seq returns -1 unless it is 0): the number of kmp_lp_cluster calls the device
+ * handle ran before this refinement (0 for a handle that only refines). */
 int lpo_lp_refine(int schedule, uint32_t n, uint32_t m, const uint32_t *xadj, const uint32_t *adjncy,
                   const int32_t *vwgt, const int32_t *adjwgt, const uint32_t *buckets,
                   uint32_t num_buckets, int seed, uint32_t k, const int32_t *max_block_weights,
                   const int32_t *min_block_weights /*nullable*/, const uint32_t *communities /*nullable*/,
                   const lpo_params *params, uint32_t *partition_inout, int32_t *block_weights_out /*k*/,
-                  lpo_stats *stats /*nullable*/);
+                  lpo_stats *stats /*nullable*/, uint32_t call_index);
 
 /* ---- T0: per-vertex decision on frozen state (sync rules), for unit parity tests ---------- */
 /* For every vertex u (regardless of active flags) compute the target the sync selection rule picks

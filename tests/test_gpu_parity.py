@@ -305,8 +305,10 @@ def test_t1_free_memory_afterwards_and_regraph():
     a = clusterer.compute_clustering(g1, free_memory_afterwards=True)
     b = clusterer.compute_clustering(g2)
     c = clusterer.compute_clustering(g1)
+    # one handle: the second and third clustering run with call indices 1 and 2
     assert np.array_equal(a, B.oracle_lp_cluster(g1, 0, mcw, schedule=B.SYNC))
-    assert len(b) == g2.n and len(c) == g1.n
+    assert np.array_equal(b, B.oracle_lp_cluster(g2, 0, mcw, schedule=B.SYNC, call_index=1))
+    assert np.array_equal(c, B.oracle_lp_cluster(g1, 0, mcw, schedule=B.SYNC, call_index=2))
 
 
 def test_empty_graph_and_isolated_only():
