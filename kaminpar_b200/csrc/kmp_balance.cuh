@@ -1,6 +1,7 @@
 // kaminpar_b200: overload balancer on the device + its C ABI (include/kaminpar_b200_balancer.h).
 // Included at the end of kmp_lp.cu (same translation unit: it balances the partition a kmp_lp_handle holds and
-// commits through the refiner's cooperative ladder kernel, lp_commit.cuh commit_refine_fused).
+// commits through the refiner's cooperative ladder kernel, lp_commit.cuh commit_refine_fused). The round driver, the
+// round tail and the select_all body here serve the underload balancer (kmp_underload.cuh) too.
 //
 // What it restates: OverloadBalancer::refine (refinement/balancer/overload_balancer.cc:51-326) as synchronous
 // rounds (DESIGN.md §11). One round:
@@ -24,7 +25,7 @@
 
 namespace kmp {
 
-enum : uint32_t { SALT_BAL_TIE = 5, SALT_BAL_DRAW = 6, SALT_BAL_COMMIT = 7 };
+enum : uint32_t { SALT_BAL_TIE = 5, SALT_BAL_DRAW = 6, SALT_BAL_COMMIT = 7, SALT_UBAL_TIE = 8, SALT_UBAL_COMMIT = 9 };
 constexpr uint32_t kBalMaxRounds = KMP_BALANCE_MAX_ROUNDS;
 constexpr uint32_t kBalThreadDeg = 8;    // deg <= 8: one thread per vertex
 constexpr uint32_t kBalWarpDeg = 256;    // deg <= 256: one warp per vertex
@@ -365,6 +366,27 @@ __global__ void bal_propose(uint32_t nc, const uint32_t *blk, const int32_t *pre
     }
   }
 }
+// underload balancer: selected iff the weight of the candidates before it in its target's segment is < deficit[target]
+__global__ void ubal_propose(uint32_t nt, const uint32_t *blk, const int32_t *prefix, const int32_t *deficit,
+                             const uint32_t *sort_val, const uint32_t *cand, uint32_t *mv_u, uint32_t *mv_t,
+                             uint32_t *mover_count) {
+  for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p < nt; p += gridDim.x * blockDim.x) {
+    const uint32_t t = blk[p];
+    if (prefix[p] < deficit[t]) {
+      const uint32_t slot = atomicAdd(mover_count, 1u);
+      mv_u[slot] = cand[sort_val[p]];
+      mv_t[slot] = t;
+    }
+  }
+}
+
+// the underload balancer's kernels of select_all (kmp_underload.cuh)
+__global__ void ubal_block_stats(uint32_t k, const int32_t *weight, const int32_t *min_w, int32_t *deficit,
+                                 uint8_t *tmask, unsigned long long *ctrl);
+__global__ void ubal_vertex_flags(uint32_t n, const uint32_t *label, const int32_t *vwgt, const int32_t *weight,
+                                  const int32_t *min_w, const uint8_t *tmask, uint8_t *flag);
+__global__ void ubal_keep_sources(uint32_t n, const uint8_t *flag, const uint32_t *label, const int32_t *vwgt,
+                                  uint32_t *target, float *key);
 
 } // namespace kmp
 
@@ -372,7 +394,12 @@ namespace {
 
 using namespace kmp;
 
-int bal_refuse(kmp_lp_handle *h, const char *what = "the overload balancer", const char *section = "§11") {
+enum class BalKind { Overload, Underload };
+
+int bal_refuse(kmp_lp_handle *h, BalKind kind) {
+  const bool under = kind == BalKind::Underload;
+  const char *what = under ? "the underload balancer" : "the overload balancer";
+  const char *section = under ? "§12" : "§11";
   if (h == nullptr || !h->have_graph) {
     return fail(KMP_ERR_INVALID, "no graph set");
   }
@@ -386,11 +413,12 @@ int bal_refuse(kmp_lp_handle *h, const char *what = "the overload balancer", con
   return KMP_OK;
 }
 
-// Scratch of the balancer, grow-only in the handle (kmp_lp_free_scratch releases it).
+// Scratch of both balancers, grow-only in the handle (kmp_lp_free_scratch releases it).
 int bal_ensure(kmp_lp_handle *h, uint32_t k, uint32_t nc) {
   const size_t n = std::max<uint32_t>(h->n, 1), kk = std::max<uint32_t>(k, 1), c = std::max<uint32_t>(nc, 1);
   KMP_CUDA(h->bal_cand.ensure(n));
   KMP_CUDA(h->bal_flag.ensure(std::max(n, kk)));
+  KMP_CUDA(h->ubal_tmask.ensure(kk));
   KMP_CUDA(h->bal_over.ensure(kk));
   KMP_CUDA(h->bal_pbw.ensure(kk));
   KMP_CUDA(h->bal_under.ensure(kk));
@@ -453,62 +481,58 @@ template <typename Fn> int bal_cub(kmp_lp_handle *h, Fn &&call) {
   return KMP_OK;
 }
 
-// One round after its read-back: evaluate, select, propose, commit (moves land in bal_ctr32[4 + r]).
-int bal_round(kmp_lp_handle *h, uint32_t k, uint32_t nc, uint32_t call, uint32_t r) {
-  int rc = bal_evaluate(h, k, nc, sync_base(h->cfg.seed, call, r, SALT_BAL_TIE), true);
-  if (rc != KMP_OK) {
-    return rc;
-  }
+// The end of a round of either balancer, after its selection left ns sort words (block << 32 | desc key bits) and
+// candidate indices in bal_sk_a / bal_sv_a: sort them by (block, key desc), scan the weights per block, propose the
+// candidates whose preceding weight in their block is below the block's quota bal_over[b], and commit the proposals
+// with the refiner's ladder, one pass (moves land in bal_ctr32[4 + r]). The overload balancer commits without
+// minimum weights: accepted moves never push a target above its maximum. The underload balancer commits with them:
+// the target side keeps every block <= max, the source side keeps every source >= min (targets are underloaded and
+// sources are not, so no block is both).
+int bal_round_tail(kmp_lp_handle *h, BalKind kind, uint32_t k, uint32_t ns, uint32_t call, uint32_t r) {
   uint32_t end_bit = 32;
   while (end_bit < 64 && (static_cast<uint64_t>(k - 1) >> (end_bit - 32)) != 0) {
     ++end_bit;
   }
   cudaStream_t st = h->stream;
-  rc = bal_cub(h, [&](void *tmp, size_t &bytes) {
+  int rc = bal_cub(h, [&](void *tmp, size_t &bytes) {
     return cub::DeviceRadixSort::SortPairs(tmp, bytes, h->bal_sk_a.p, h->bal_sk_b.p, h->bal_sv_a.p, h->bal_sv_b.p,
-                                           static_cast<int>(nc), 0, static_cast<int>(end_bit), st);
+                                           static_cast<int>(ns), 0, static_cast<int>(end_bit), st);
   });
   if (rc != KMP_OK) {
     return rc;
   }
-  bal_sorted_weights<<<capped(h, grid_for(nc, 256)), 256, 0, st>>>(nc, h->bal_sk_b.p, h->bal_sv_b.p, h->bal_cand.p, h->vwgt,
-                                                        h->bal_blk.p, h->bal_wt.p);
+  bal_sorted_weights<<<capped(h, grid_for(ns, 256)), 256, 0, st>>>(ns, h->bal_sk_b.p, h->bal_sv_b.p, h->bal_cand.p, h->vwgt,
+                                                                   h->bal_blk.p, h->bal_wt.p);
   rc = bal_cub(h, [&](void *tmp, size_t &bytes) {
     return cub::DeviceScan::ExclusiveSumByKey(tmp, bytes, h->bal_blk.p, h->bal_wt.p, h->bal_prefix.p,
-                                              static_cast<int>(nc), cub::Equality(), st);
+                                              static_cast<int>(ns), cub::Equality(), st);
   });
   if (rc != KMP_OK) {
     return rc;
   }
+  const bool under = kind == BalKind::Underload;
   uint32_t *mover_count = h->bal_ctr32.p;
-  KMP_CUDA(cudaMemsetAsync(mover_count, 0, sizeof(uint32_t), st));
-  bal_propose<<<capped(h, grid_for(nc, 256)), 256, 0, st>>>(nc, h->bal_blk.p, h->bal_prefix.p, h->bal_over.p, h->bal_sv_b.p,
-                                                 h->bal_cand.p, h->bal_target.p, h->vwgt, h->weight.p, h->maxw.p,
-                                                 h->bal_under.p, h->bal_ctrl.p,
-                                                 sync_base(h->cfg.seed, call, r, SALT_BAL_DRAW), h->mv_u.p, h->mv_t.p,
-                                                 mover_count);
-  // the refiner's commit, one pass, no minimum weights: accepted moves never push a target above its maximum
-  CommitArgs ca = make_commit_args(h, RunCtx{1, k, 0, false, false});
+  if (under) {
+    ubal_propose<<<capped(h, grid_for(ns, 256)), 256, 0, st>>>(ns, h->bal_blk.p, h->bal_prefix.p, h->bal_over.p,
+                                                               h->bal_sv_b.p, h->bal_cand.p, h->mv_u.p, h->mv_t.p,
+                                                               mover_count);
+  } else {
+    bal_propose<<<capped(h, grid_for(ns, 256)), 256, 0, st>>>(ns, h->bal_blk.p, h->bal_prefix.p, h->bal_over.p,
+                                                              h->bal_sv_b.p, h->bal_cand.p, h->bal_target.p, h->vwgt,
+                                                              h->weight.p, h->maxw.p, h->bal_under.p, h->bal_ctrl.p,
+                                                              sync_base(h->cfg.seed, call, r, SALT_BAL_DRAW), h->mv_u.p,
+                                                              h->mv_t.p, mover_count);
+  }
+  CommitArgs ca = make_commit_args(h, RunCtx{1, k, 0, under, false});
   ca.mover_count = mover_count;
   ca.next_mover_count = h->bal_ctr32.p + 1; // scratch: nothing reads it
   ca.also_zero = nullptr;
   ca.moved_count = h->bal_ctr32.p + 4 + r;
-  ca.base_commit = sync_base(h->cfg.seed, call, r, SALT_BAL_COMMIT);
+  ca.base_commit = sync_base(h->cfg.seed, call, r, under ? SALT_UBAL_COMMIT : SALT_BAL_COMMIT);
   ca.stamp = 0;
-  GatheredArgs ga{nullptr, 1, 0, nullptr};
-  GridBarrier bar{h->grid_bar.p, h->grid_bar.p + 1};
-  uint32_t passes = 1;
-  const size_t smem = 4 * std::max<size_t>(k * kLadderLevels <= kSmemPrivLimit ? static_cast<size_t>(k) * kLadderLevels : 0,
-                                           k <= kSmemPrivLimit ? k : 0);
-  const uint32_t blocks = capped(h, std::min<uint32_t>(grid_for(std::max<uint32_t>(nc, k), 256),
-                                                       static_cast<uint32_t>(h->fused_blocks_refine)));
-  void *args[] = {&ca, &ga, &bar, &passes};
-  if (h->p64) {
-    KMP_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void *>(commit_refine_fused<true>), dim3(blocks), dim3(256), args,
-                                         smem, st));
-  } else {
-    KMP_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void *>(commit_refine_fused<false>), dim3(blocks), dim3(256), args,
-                                         smem, st));
+  rc = launch_commit_refine(h, ca, GatheredArgs{nullptr, 1, 0, nullptr}, 1, ns);
+  if (rc != KMP_OK) {
+    return rc;
   }
   h->kernel_launches += 5;
   KMP_CUDA(cudaGetLastError());
@@ -545,133 +569,118 @@ int bal_round_begin(kmp_lp_handle *h, uint32_t k, unsigned long long *host_ctrl,
   return KMP_OK;
 }
 
-} // namespace
+// the underload balancer's round steps (kmp_underload.cuh)
+int ubal_round_begin(kmp_lp_handle *h, uint32_t k, unsigned long long *host_ctrl, uint32_t *host_proposals);
+int ubal_select(kmp_lp_handle *h, uint32_t k, uint32_t nc, uint32_t call, uint32_t r, uint32_t *nt);
 
-extern "C" {
+struct BalResult {
+  uint32_t rounds = 0;
+  uint32_t moved[kBalMaxRounds] = {};
+  unsigned long long before = 0, after = 0; // total overload / underload
+  unsigned long long candidates = 0, edges = 0;
+  float device_ms = 0.f;
+};
 
-int kmp_overload_balance(kmp_lp_handle *h, uint32_t k, const int32_t *max_block_weights,
-                         const int32_t *perfectly_balanced_block_weights, uint32_t *partition_inout,
-                         int32_t *block_weights_out, int *improved_out, kmp_balance_stats *stats) {
-  int rc = bal_refuse(h);
-  if (rc != KMP_OK) {
-    return rc;
-  }
-  if (k == 0 || max_block_weights == nullptr || perfectly_balanced_block_weights == nullptr) {
-    return fail(KMP_ERR_INVALID, "k / max_block_weights / perfectly_balanced_block_weights missing");
-  }
+// One balancer call after its entry point's checks: load the partition (pbw: the overload balancer's perfectly
+// balanced weights, min_w: the underload balancer's minimum weights), run rounds until the stop rule, download.
+int bal_run(kmp_lp_handle *h, BalKind kind, uint32_t k, const int32_t *max_w, const int32_t *min_w, const int32_t *pbw,
+            uint32_t *partition_inout, int32_t *block_weights_out, BalResult &res) {
   const uint32_t n = h->n;
-  if (partition_inout == nullptr && (rc = refuse_without_labels(h)) != KMP_OK) {
-    return rc;
-  }
   KMP_CUDA(cudaSetDevice(h->device));
-  if (stats != nullptr) {
-    std::memset(stats, 0, sizeof(*stats));
-  }
   h->kernel_launches = 0;
   cudaStream_t st = h->stream;
   KMP_CUDA(cudaEventRecord(h->ev_begin, st));
-  rc = ensure_scratch(h, 1, k); // the commit's ladder histograms (zeroed), counters, active flags
+  int rc = ensure_scratch(h, 1, k); // the commit's ladder histograms (zeroed), counters, active flags
   if (rc == KMP_OK) {
     rc = prepare_labg(h, k); // the commit writes the packed labels (kmp_lp_refine repacks them on entry)
   }
   if (rc == KMP_OK) {
     rc = bal_ensure(h, k, 0);
   }
+  if (rc == KMP_OK) {
+    rc = load_partition(h, k, partition_inout, max_w, min_w);
+  }
   if (rc != KMP_OK) {
     return rc;
   }
-  KMP_CUDA(h->label.ensure(n));
-  KMP_CUDA(h->weight.ensure(k));
-  KMP_CUDA(h->maxw.ensure(k));
-  if (partition_inout != nullptr && n > 0) {
-    KMP_CUDA(cudaMemcpyAsync(h->label.p, partition_inout, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, st));
+  if (pbw != nullptr) {
+    KMP_CUDA(cudaMemcpyAsync(h->bal_pbw.p, pbw, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, st));
   }
-  if (partition_inout != nullptr) {
-    h->labels_valid = true;
-  }
-  KMP_CUDA(cudaMemcpyAsync(h->maxw.p, max_block_weights, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, st));
-  KMP_CUDA(cudaMemcpyAsync(h->bal_pbw.p, perfectly_balanced_block_weights, static_cast<size_t>(k) * 4,
-                           cudaMemcpyHostToDevice, st));
-  KMP_CUDA(cudaMemsetAsync(h->weight.p, 0, static_cast<size_t>(k) * 4, st));
   KMP_CUDA(cudaMemsetAsync(h->bal_ctrl.p, 0, 8 * sizeof(unsigned long long), st));
   KMP_CUDA(cudaMemsetAsync(h->bal_ctr32.p, 0, (4 + kBalMaxRounds) * sizeof(uint32_t), st));
   rc = checked_block_weights(h, k, h->bal_ctrl.p + 3);
   if (rc != KMP_OK) {
     return rc;
   }
-  const uint32_t call = h->bal_calls++;
+  const bool under = kind == BalKind::Underload;
+  const uint32_t call = under ? h->ubal_calls++ : h->bal_calls++;
   unsigned long long ctrl[4] = {0, 0, 0, 0};
-  unsigned long long before = 0, candidates = 0;
   uint32_t proposals = 0;
-  uint32_t rounds = 0;
-  for (;; ++rounds) {
-    rc = bal_round_begin(h, k, ctrl, &proposals);
+  for (;; ++res.rounds) {
+    const uint32_t r = res.rounds;
+    rc = under ? ubal_round_begin(h, k, ctrl, &proposals) : bal_round_begin(h, k, ctrl, &proposals);
     if (rc != KMP_OK) {
       return rc;
     }
-    if (rounds == 0) {
-      before = ctrl[0];
+    if (r == 0) {
+      res.before = ctrl[0];
     }
-    // stop: feasible, or the last round proposed no move (then no round would: without moves the next round
-    // selects the same candidates with the same feasible targets), or the cap. A round whose proposals the
-    // ladder rejected is retried: its commit priorities and draws are hashed with the round.
-    if (ctrl[0] == 0 || (rounds > 0 && proposals == 0) || rounds == kBalMaxRounds) {
+    // stop: balanced, or the last round proposed no move (then no round would: without moves the next round selects
+    // the same candidates with the same targets and quotas), or the cap. A round whose proposals the ladder
+    // rejected is retried: its commit priorities, ties and draws are hashed with the round.
+    if (ctrl[0] == 0 || (r > 0 && proposals == 0) || r == kBalMaxRounds) {
       break;
     }
     const uint32_t nc = static_cast<uint32_t>(ctrl[1]);
-    candidates += nc;
+    res.candidates += nc;
     rc = bal_ensure(h, k, nc);
     if (rc == KMP_OK && h->mv_u.cap < nc) {
       KMP_CUDA(h->mv_u.ensure(nc));
       KMP_CUDA(h->mv_t.ensure(nc));
       KMP_CUDA(h->acc.ensure(nc));
     }
-    if (rc == KMP_OK) {
-      rc = bal_round(h, k, nc, call, rounds);
+    if (rc != KMP_OK) {
+      return rc;
+    }
+    KMP_CUDA(cudaMemsetAsync(h->bal_ctr32.p, 0, sizeof(uint32_t), st)); // this round's proposals
+    uint32_t ns = nc; // sort words the selection left
+    rc = under ? ubal_select(h, k, nc, call, r, &ns)
+               : bal_evaluate(h, k, nc, sync_base(h->cfg.seed, call, r, SALT_BAL_TIE), true);
+    // an underload round without a candidate that has a target ends here; an overload round always commits
+    if (rc == KMP_OK && (ns > 0 || !under)) {
+      rc = bal_round_tail(h, kind, k, ns, call, r);
     }
     if (rc != KMP_OK) {
       return rc;
     }
   }
-  if (partition_inout != nullptr && before != 0 && n > 0) {
+  res.after = ctrl[0];
+  if (partition_inout != nullptr && res.before != 0 && n > 0) {
     KMP_CUDA(cudaMemcpyAsync(partition_inout, h->label.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, st));
   }
   if (block_weights_out != nullptr) {
     KMP_CUDA(cudaMemcpyAsync(block_weights_out, h->weight.p, static_cast<size_t>(k) * 4, cudaMemcpyDeviceToHost, st));
   }
-  uint32_t moved[kBalMaxRounds] = {};
-  unsigned long long edges = 0;
-  KMP_CUDA(cudaMemcpyAsync(moved, h->bal_ctr32.p + 4, sizeof(moved), cudaMemcpyDeviceToHost, st));
-  KMP_CUDA(cudaMemcpyAsync(&edges, h->bal_ctrl.p + 4, sizeof(edges), cudaMemcpyDeviceToHost, st));
+  KMP_CUDA(cudaMemcpyAsync(res.moved, h->bal_ctr32.p + 4, sizeof(res.moved), cudaMemcpyDeviceToHost, st));
+  KMP_CUDA(cudaMemcpyAsync(&res.edges, h->bal_ctrl.p + 4, sizeof(res.edges), cudaMemcpyDeviceToHost, st));
   KMP_CUDA(cudaEventRecord(h->ev_end, st));
   KMP_CUDA(cudaStreamSynchronize(st));
-  if (improved_out != nullptr) {
-    *improved_out = before != 0 ? 1 : 0;
-  }
-  if (stats != nullptr) {
-    stats->rounds = rounds;
-    std::memcpy(stats->moved, moved, sizeof(moved));
-    stats->overload_before = static_cast<int64_t>(before);
-    stats->overload_after = static_cast<int64_t>(ctrl[0]);
-    stats->candidates = candidates;
-    stats->edges_scanned = edges;
-    stats->kernel_launches = h->kernel_launches;
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, h->ev_begin, h->ev_end);
-    stats->device_ms = ms;
-  }
+  cudaEventElapsedTime(&res.device_ms, h->ev_begin, h->ev_end);
   return KMP_OK;
 }
 
-int kmp_balance_select_all(kmp_lp_handle *h, uint32_t k, const uint32_t *labels, const int32_t *block_weights,
-                           const int32_t *max_block_weights, uint32_t call_index, uint32_t round, uint32_t *target_out,
-                           float *key_out) {
-  int rc = bal_refuse(h);
+// Target and key of every vertex against host labels and block weights, for one (call, round) of either balancer's
+// hash schedule (min_w: the underload balancer's minimum weights, required for it).
+int bal_select_all(kmp_lp_handle *h, BalKind kind, uint32_t k, const uint32_t *labels, const int32_t *block_weights,
+                   const int32_t *max_w, const int32_t *min_w, uint32_t call_index, uint32_t round, uint32_t *target_out,
+                   float *key_out) {
+  int rc = bal_refuse(h, kind);
   if (rc != KMP_OK) {
     return rc;
   }
-  if (k == 0 || labels == nullptr || block_weights == nullptr || max_block_weights == nullptr || target_out == nullptr ||
-      key_out == nullptr) {
+  const bool under = kind == BalKind::Underload;
+  if (k == 0 || labels == nullptr || block_weights == nullptr || max_w == nullptr || (under && min_w == nullptr) ||
+      target_out == nullptr || key_out == nullptr) {
     return fail(KMP_ERR_INVALID, "null argument");
   }
   const uint32_t n = h->n;
@@ -693,19 +702,82 @@ int kmp_balance_select_all(kmp_lp_handle *h, uint32_t k, const uint32_t *labels,
     KMP_CUDA(cudaMemcpyAsync(h->label.p, labels, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, st));
   }
   KMP_CUDA(cudaMemcpyAsync(h->weight.p, block_weights, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, st));
-  KMP_CUDA(cudaMemcpyAsync(h->maxw.p, max_block_weights, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, st));
+  KMP_CUDA(cudaMemcpyAsync(h->maxw.p, max_w, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, st));
   KMP_CUDA(cudaMemsetAsync(h->bal_ctrl.p, 0, 8 * sizeof(unsigned long long), st));
+  if (under) { // the target mask
+    KMP_CUDA(h->minw.ensure(k));
+    KMP_CUDA(cudaMemcpyAsync(h->minw.p, min_w, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, st));
+    ubal_block_stats<<<capped(h, grid_for(k, 256)), 256, 0, st>>>(k, h->weight.p, h->minw.p, h->bal_over.p,
+                                                                  h->ubal_tmask.p, h->bal_ctrl.p);
+  }
   if (n > 0) {
     bal_iota<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, h->bal_cand.p);
-    rc = bal_evaluate(h, k, n, sync_base(h->cfg.seed, call_index, round, SALT_BAL_TIE), false);
+    rc = bal_evaluate(h, k, n, sync_base(h->cfg.seed, call_index, round, under ? SALT_UBAL_TIE : SALT_BAL_TIE), false,
+                      under ? h->ubal_tmask.p : nullptr);
     if (rc != KMP_OK) {
       return rc;
+    }
+    if (under) { // a vertex that may not leave its block keeps it
+      ubal_vertex_flags<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, h->label.p, h->vwgt, h->weight.p, h->minw.p,
+                                                                     h->ubal_tmask.p, h->bal_flag.p);
+      ubal_keep_sources<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, h->bal_flag.p, h->label.p, h->vwgt,
+                                                                     h->bal_target.p, h->bal_key.p);
+      KMP_CUDA(cudaGetLastError());
     }
     KMP_CUDA(cudaMemcpyAsync(target_out, h->bal_target.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, st));
     KMP_CUDA(cudaMemcpyAsync(key_out, h->bal_key.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, st));
   }
   KMP_CUDA(cudaStreamSynchronize(st));
   return KMP_OK;
+}
+
+} // namespace
+
+extern "C" {
+
+int kmp_overload_balance(kmp_lp_handle *h, uint32_t k, const int32_t *max_block_weights,
+                         const int32_t *perfectly_balanced_block_weights, uint32_t *partition_inout,
+                         int32_t *block_weights_out, int *improved_out, kmp_balance_stats *stats) {
+  int rc = bal_refuse(h, BalKind::Overload);
+  if (rc != KMP_OK) {
+    return rc;
+  }
+  if (k == 0 || max_block_weights == nullptr || perfectly_balanced_block_weights == nullptr) {
+    return fail(KMP_ERR_INVALID, "k / max_block_weights / perfectly_balanced_block_weights missing");
+  }
+  if (partition_inout == nullptr && (rc = refuse_without_labels(h)) != KMP_OK) {
+    return rc;
+  }
+  if (stats != nullptr) {
+    std::memset(stats, 0, sizeof(*stats));
+  }
+  BalResult res;
+  rc = bal_run(h, BalKind::Overload, k, max_block_weights, nullptr, perfectly_balanced_block_weights, partition_inout,
+               block_weights_out, res);
+  if (rc != KMP_OK) {
+    return rc;
+  }
+  if (improved_out != nullptr) {
+    *improved_out = res.before != 0 ? 1 : 0;
+  }
+  if (stats != nullptr) {
+    stats->rounds = res.rounds;
+    std::memcpy(stats->moved, res.moved, sizeof(res.moved));
+    stats->overload_before = static_cast<int64_t>(res.before);
+    stats->overload_after = static_cast<int64_t>(res.after);
+    stats->candidates = res.candidates;
+    stats->edges_scanned = res.edges;
+    stats->kernel_launches = h->kernel_launches;
+    stats->device_ms = res.device_ms;
+  }
+  return KMP_OK;
+}
+
+int kmp_balance_select_all(kmp_lp_handle *h, uint32_t k, const uint32_t *labels, const int32_t *block_weights,
+                           const int32_t *max_block_weights, uint32_t call_index, uint32_t round, uint32_t *target_out,
+                           float *key_out) {
+  return bal_select_all(h, BalKind::Overload, k, labels, block_weights, max_block_weights, nullptr, call_index, round,
+                        target_out, key_out);
 }
 
 } // extern "C"

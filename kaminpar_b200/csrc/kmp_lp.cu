@@ -251,17 +251,19 @@ struct kmp_lp_handle {
   bool step_has_min = false, step_has_comm = false;
   uint32_t mover_parity = 0; // proposal counter in use: ctr32[0] (parity 0) or ctr32[3] (parity 1)
   bool stepping = false; // proposals are accumulated by kmp_lp_step_commit, not by the sweep kernels
-  // overload balancer (kmp_balance.cuh): its own call counter, so that LP calls hash the same with or without it
-  uint32_t bal_calls = 0;
+  // overload and underload balancers (kmp_balance.cuh, kmp_underload.cuh): one call counter each, so that LP calls
+  // and either balancer hash the same with or without the other; one set of scratch
+  uint32_t bal_calls = 0, ubal_calls = 0;
   DevBuf<uint32_t> bal_cand, bal_under, bal_ctr32, bal_target, bal_lists, bal_sv_a, bal_sv_b, bal_blk;
+  // bal_over[b]: the quota a block's segment of sorted candidates is selected against (overload of b, or the
+  // underload balancer's deficit of target b)
   DevBuf<int32_t> bal_over, bal_pbw, bal_wt, bal_prefix;
-  DevBuf<uint8_t> bal_flag;
+  DevBuf<uint8_t> bal_flag, ubal_tmask;
   DevBuf<float> bal_key;
+  // bal_ctrl: [0] total over- / underload [1] candidates [2] |U| (underloaded blocks) [3] bad labels [4] edges
+  //           [5] candidates with a target
+  // bal_ctr32: [0] movers [1] scratch [2..3] tier counts [4 + r] moved in round r
   DevBuf<unsigned long long> bal_ctrl, bal_sk_a, bal_sk_b;
-  // underload balancer (kmp_underload.cuh): its own call counter; shares the overload balancer's scratch
-  uint32_t ubal_calls = 0;
-  DevBuf<int32_t> ubal_deficit;
-  DevBuf<uint8_t> ubal_tmask;
 };
 
 namespace kmp {
@@ -1286,6 +1288,26 @@ void launch_push_activation(kmp_lp_handle *h, const CommitArgs &ca, const SubRou
   timed_end(h, ev);
   ++h->kernel_launches;
 }
+// The refiner's ladder commit (lp_commit.cuh commit_refine_fused) in one cooperative launch, for the LP refiner and
+// both balancers. Its dynamic shared memory follows the kernel's choice of CTA-private level histograms (priv_h) and
+// block-weight deltas (priv_k) for k = ca.k; work: the proposals the launch handles (grid before the clamp).
+int launch_commit_refine(kmp_lp_handle *h, CommitArgs ca, GatheredArgs ga, uint32_t passes, uint32_t work) {
+  const uint32_t k = ca.k;
+  const size_t smem = 4 * std::max<size_t>(k * kLadderLevels <= kSmemPrivLimit ? static_cast<size_t>(k) * kLadderLevels : 0,
+                                           k <= kSmemPrivLimit ? k : 0);
+  const uint32_t blocks = capped(h, std::min<uint32_t>(grid_for(std::max<uint32_t>(work, k), 256),
+                                                       static_cast<uint32_t>(h->fused_blocks_refine)));
+  GridBarrier bar{h->grid_bar.p, h->grid_bar.p + 1};
+  void *args[] = {&ca, &ga, &bar, &passes};
+  if (h->p64) {
+    KMP_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void *>(commit_refine_fused<true>), dim3(blocks), dim3(256), args,
+                                         smem, h->stream));
+  } else {
+    KMP_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void *>(commit_refine_fused<false>), dim3(blocks), dim3(256), args,
+                                         smem, h->stream));
+  }
+  return KMP_OK;
+}
 // The whole commit of sub-round sg in one cooperative launch, over the proposals in mv_u / mv_t -- or, with
 // gathered != nullptr, over the all-gathered proposal buffers (world * (4 + 2 * cap) words) of a sharded run or of
 // the stepping API, which the same launch unpacks and accumulates first. Every rank runs the same
@@ -1297,24 +1319,14 @@ int commit_subround(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t 
   ca.stamp = h->stamps_ok ? make_stamp(iter, sg) : 0;
   GatheredArgs ga{gathered, h->world, gathered != nullptr ? subround_cap(h, q) : 0u,
                   h->ctr32.p + (h->mover_parity ? 3 : 0)};
-  GridBarrier bar{h->grid_bar.p, h->grid_bar.p + 1};
   const int ev = timed_begin(h, kTagCommit);
   if (rc.mode == 1) {
-    uint32_t passes = std::max<uint32_t>(1, h->cfg.sync_commit_passes);
-    const uint32_t k = rc.num_labels;
-    const size_t smem = 4 * std::max<size_t>(k * kLadderLevels <= kSmemPrivLimit ? static_cast<size_t>(k) * kLadderLevels : 0,
-                                             k <= kSmemPrivLimit ? k : 0);
-    const uint32_t blocks = capped(h, std::min<uint32_t>(grid_for(std::max<uint32_t>(q.total, k), 256),
-                                                         static_cast<uint32_t>(h->fused_blocks_refine)));
-    void *rargs[] = {&ca, &ga, &bar, &passes};
-    if (h->p64) {
-      KMP_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void *>(commit_refine_fused<true>), dim3(blocks), dim3(256), rargs,
-                                           smem, h->stream));
-    } else {
-      KMP_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void *>(commit_refine_fused<false>), dim3(blocks), dim3(256), rargs,
-                                           smem, h->stream));
+    const int r = launch_commit_refine(h, ca, ga, std::max<uint32_t>(1, h->cfg.sync_commit_passes), q.total);
+    if (r != KMP_OK) {
+      return r;
     }
   } else {
+    GridBarrier bar{h->grid_bar.p, h->grid_bar.p + 1};
     const uint32_t blocks = capped(h, std::min<uint32_t>(grid_for(q.total, 256), static_cast<uint32_t>(h->fused_blocks)));
     void *args[] = {&ca, &ga, &bar};
     if (h->p64) {
@@ -1649,6 +1661,28 @@ int checked_block_weights(kmp_lp_handle *h, uint32_t k, unsigned long long *bad)
   if (b != 0) {
     return fail(KMP_ERR_INVALID, "labels >= k on the device: a clustering is not a k-way partition");
   }
+  return KMP_OK;
+}
+
+// A k-way partition onto the handle: the labels (uploaded from partition when non-null, else the device labels
+// stay), the max (and, when given, min) block weights, weight[0, k) zeroed for checked_block_weights, which the
+// caller runs last so that its host wait covers this set-up.
+int load_partition(kmp_lp_handle *h, uint32_t k, const uint32_t *partition, const int32_t *max_block_weights,
+                   const int32_t *min_block_weights) {
+  const uint32_t n = h->n;
+  KMP_CUDA(h->label.ensure(n));
+  KMP_CUDA(h->weight.ensure(k));
+  KMP_CUDA(h->maxw.ensure(k));
+  if (partition != nullptr) {
+    KMP_CUDA(cudaMemcpyAsync(h->label.p, partition, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, h->stream));
+    h->labels_valid = true;
+  }
+  KMP_CUDA(cudaMemcpyAsync(h->maxw.p, max_block_weights, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, h->stream));
+  if (min_block_weights != nullptr) {
+    KMP_CUDA(h->minw.ensure(k));
+    KMP_CUDA(cudaMemcpyAsync(h->minw.p, min_block_weights, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, h->stream));
+  }
+  KMP_CUDA(cudaMemsetAsync(h->weight.p, 0, static_cast<size_t>(k) * 4, h->stream));
   return KMP_OK;
 }
 
@@ -2425,34 +2459,20 @@ int kmp_lp_refine(kmp_lp_handle *h, uint32_t k, const int32_t *max_block_weights
   if (rc != KMP_OK) {
     return rc;
   }
-  KMP_CUDA(h->label.ensure(n));
-  KMP_CUDA(h->weight.ensure(k));
-  KMP_CUDA(h->maxw.ensure(k));
   rc = ensure_scratch(h, 1, k);
-  if (rc != KMP_OK) {
-    return rc;
+  if (rc == KMP_OK) {
+    rc = prepare_labg(h, k);
   }
-  rc = prepare_labg(h, k);
-  if (rc != KMP_OK) {
-    return rc;
+  if (rc == KMP_OK) {
+    rc = load_partition(h, k, partition_inout, max_block_weights, min_block_weights);
   }
-  if (partition_inout != nullptr && n > 0) {
-    KMP_CUDA(cudaMemcpyAsync(h->label.p, partition_inout, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, h->stream));
+  if (rc == KMP_OK) {
+    rc = upload_optional_u32(h, h->communities, communities, n);
   }
-  if (partition_inout != nullptr) {
-    h->labels_valid = true;
-  }
-  KMP_CUDA(cudaMemcpyAsync(h->maxw.p, max_block_weights, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, h->stream));
-  if (min_block_weights != nullptr) {
-    KMP_CUDA(h->minw.ensure(k));
-    KMP_CUDA(cudaMemcpyAsync(h->minw.p, min_block_weights, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, h->stream));
-  }
-  rc = upload_optional_u32(h, h->communities, communities, n);
   if (rc != KMP_OK) {
     return rc;
   }
   KMP_CUDA(cudaMemsetAsync(h->ctr64.p, 0, kCtrSize * sizeof(unsigned long long), h->stream));
-  KMP_CUDA(cudaMemsetAsync(h->weight.p, 0, static_cast<size_t>(k) * 4, h->stream));
   if (n > 0) {
     k_fill_u8<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->active.p, 1); // Base::initialize: all active
     launch_pack_labels(h); // reads the labels without indexing by them
@@ -2623,12 +2643,11 @@ int kmp_lp_free_scratch(kmp_lp_handle *h) {
     b->release();
   }
   h->bal_flag.release();
+  h->ubal_tmask.release();
   h->bal_key.release();
   h->bal_ctrl.release();
   h->bal_sk_a.release();
   h->bal_sk_b.release();
-  h->ubal_deficit.release();
-  h->ubal_tmask.release();
   {
     cudaMemPool_t pool = kmp_private_pool(h->device); // blocks cached for coarse graphs (kmp_contract.cuh)
     if (pool != nullptr) {
@@ -2819,26 +2838,17 @@ int kmp_lp_step_begin_refine(kmp_lp_handle *h, uint32_t k, const int32_t *max_bl
   if (rc != KMP_OK) {
     return rc;
   }
-  KMP_CUDA(h->label.ensure(n));
-  KMP_CUDA(h->weight.ensure(k));
-  KMP_CUDA(h->maxw.ensure(k));
   rc = ensure_scratch(h, 1, k);
-  if (rc != KMP_OK) {
-    return rc;
+  if (rc == KMP_OK) {
+    rc = load_partition(h, k, partition, max_block_weights, min_block_weights);
   }
-  KMP_CUDA(cudaMemcpyAsync(h->label.p, partition, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, h->stream));
-  h->labels_valid = true;
-  KMP_CUDA(cudaMemcpyAsync(h->maxw.p, max_block_weights, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, h->stream));
-  if (min_block_weights != nullptr) {
-    KMP_CUDA(h->minw.ensure(k));
-    KMP_CUDA(cudaMemcpyAsync(h->minw.p, min_block_weights, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, h->stream));
+  if (rc == KMP_OK) {
+    rc = upload_optional_u32(h, h->communities, communities, n);
   }
-  rc = upload_optional_u32(h, h->communities, communities, n);
   if (rc != KMP_OK) {
     return rc;
   }
   KMP_CUDA(cudaMemsetAsync(h->ctr64.p, 0, kCtrSize * sizeof(unsigned long long), h->stream));
-  KMP_CUDA(cudaMemsetAsync(h->weight.p, 0, static_cast<size_t>(k) * 4, h->stream));
   rc = prepare_labg(h, k);
   if (rc != KMP_OK) {
     return rc;
