@@ -17,6 +17,8 @@
 //   CoarseGraph / contract_clustering  kaminpar-shm/coarsening/contraction/cluster_contraction.h:22-56
 //   sparsification_target / CoarseGraph::sparsify
 //                      kaminpar-shm/coarsening/sparsification_cluster_coarsener.cc:41-228 (DESIGN.md §13)
+//   LPClustering::compute_overlay_clustering
+//                      kaminpar-shm/coarsening/overlay_cluster_coarsener.cc:34-151 (DESIGN.md §14)
 //
 // Error convention: the reference's path has no error codes (KASSERT aborts); here a non-zero
 // status of the C ABI becomes std::runtime_error. There is no CPU fallback.
@@ -164,7 +166,22 @@ public:
       detail::check(kmp_lp_free_scratch(_handle.get()));
     }
   }
+  // The clustering step of OverlayClusterCoarsener::coarsen(): 2^num_levels compute_clustering calls on this
+  // clusterer, intersected in the reference's tree order on the device (kmp_lp_cluster_overlay). The overlay is
+  // written to `clustering` (ids in [0, n), not dense) and stays on the device for contract_clustering(handle(), {}).
+  // num_levels = 0 is one compute_clustering. Its stats: last_overlay_stats().
+  void compute_overlay_clustering(std::span<NodeID> clustering, const CSRGraphView &graph, const int num_levels,
+                                  const bool free_memory_afterwards) {
+    _handle.set_graph(graph);
+    detail::check(kmp_lp_cluster_overlay(_handle.get(), num_levels, _max_cluster_weight, _desired,
+                                         _communities.empty() ? nullptr : _communities.data(),
+                                         clustering.empty() ? nullptr : clustering.data(), &_overlay_stats));
+    if (free_memory_afterwards) {
+      detail::check(kmp_lp_free_scratch(_handle.get()));
+    }
+  }
   [[nodiscard]] const kmp_lp_stats &last_stats() const { return _stats; }
+  [[nodiscard]] const kmp_overlay_stats &last_overlay_stats() const { return _overlay_stats; }
   [[nodiscard]] kmp_lp_handle *handle() const { return _handle.get(); } // graph holder for contract_clustering
   void invalidate_graph() { _handle.invalidate_graph(); }                // the borrowed graph changed in place
 
@@ -193,6 +210,7 @@ private:
   NodeID _desired = 0;
   std::span<const NodeID> _communities;
   kmp_lp_stats _stats{};
+  kmp_overlay_stats _overlay_stats{};
 };
 
 // Same surface as kaminpar::shm::Refiner (refiner.h:34-56).

@@ -110,6 +110,50 @@ typedef struct kmp_sparsify_stats {
 int kmp_coarse_sparsify(kmp_lp_handle *h, kmp_coarse_graph *g, uint32_t target_m, uint64_t seed,
                         kmp_sparsify_stats *stats);
 
+/* ---- overlay of clusterings (OverlayClusterCoarsener, DESIGN.md §14) -----------------------------------------------
+ *
+ *   OverlayClusterCoarsener::coarsen / overlay   kaminpar-shm/coarsening/overlay_cluster_coarsener.cc:34-151
+ *
+ * The overlay of two clusterings a, b of the same n vertices is their intersection, with the reference's ids:
+ *   out[u] = index(ra(a[u])) + |{distinct b[v] : a[v] == a[u], b[v] < b[u]}|
+ * where ra(x) is the rank of x among the distinct values of a and index(c) the number of vertices u with
+ * ra(a[u]) < c. out[u] == out[v] iff a[u] == a[v] and b[u] == b[v]; ids lie in [0, n) and are not dense. 2^L
+ * clusterings C[0 .. 2^L) are reduced in the reference's tree order: for level = L .. 1, h = 2^(level-1),
+ * C[p] = overlay(C[p], C[h + p]) for p < h; the result is C[0].
+ *
+ * The result becomes the handle's device labels, so kmp_contract_clustering(h, NULL, ...) contracts it without a
+ * copy. The handle's per-cluster weights (of its last LP call) do NOT describe overlaid labels: the calls that read
+ * the device labels (contraction, refinement, the balancers, kmp_lp_edge_cut) recompute whatever weights they use.
+ * The 2^L clusterings are stashed in device memory the handle owns (2^L * n * 4 bytes, kept for the next call);
+ * kmp_lp_set_graph* and kmp_lp_free_scratch release it.
+ *
+ * Refused: no graph (KMP_ERR_INVALID); sharded, NCCL or stepping handles (KMP_ERR_UNSUPPORTED); a label >= n
+ * (KMP_ERR_INVALID, the device labels stay as they were). n = 0 does no device work. stats may be NULL. */
+#define KMP_OVERLAY_MAX_LEVELS 16
+
+typedef struct kmp_overlay_stats {
+  uint32_t num_clusterings;  /* 2^L */
+  uint32_t num_clusters;     /* distinct ids of the result */
+  uint32_t sort_bits;        /* largest key width of a pairwise overlay's radix sort: ceil(log2 n) + ceil(log2 c_a) */
+  uint32_t kernel_launches;  /* hand-written overlay kernels (not the LP calls', not CUB's sort and scans) */
+  float lp_device_ms;        /* the LP calls (kmp_lp_cluster_overlay; 0 for kmp_overlay_clusterings) */
+  float overlay_device_ms;   /* the tree on the device, including one host wait per pairwise overlay */
+} kmp_overlay_stats;
+
+/* OverlayClusterCoarsener's clustering step: 2^num_levels kmp_lp_cluster calls on the handle's graph with the same
+ * arguments (equal to as many separate calls: the call counter advances by 2^num_levels, and under
+ * KMP_SCHEDULE_SEQ_STRICT the random stream continues across them), reduced by the tree above. num_levels = 0 is
+ * exactly one kmp_lp_cluster. num_levels in [0, KMP_OVERLAY_MAX_LEVELS]. clustering_out: HOST buffer of n ids or
+ * NULL (the result stays on the device). */
+int kmp_lp_cluster_overlay(kmp_lp_handle *h, int num_levels, int32_t max_cluster_weight, uint32_t desired_num_clusters,
+                           const uint32_t *communities, uint32_t *clustering_out, kmp_overlay_stats *stats);
+
+/* The same tree over `count` (a power of two, at most 2^KMP_OVERLAY_MAX_LEVELS) given clusterings of the handle's
+ * graph: clusterings is a HOST array of count x n ids in [0, n), C[i] = clusterings + i * n. out: HOST buffer of n
+ * ids or NULL. */
+int kmp_overlay_clusterings(kmp_lp_handle *h, uint32_t count, const uint32_t *clusterings, uint32_t *out,
+                            kmp_overlay_stats *stats);
+
 #ifdef __cplusplus
 }
 #endif

@@ -7,6 +7,8 @@ include/kaminpar_b200_contraction.h (device code: kaminpar_b200/csrc/kmp_contrac
         kaminpar-shm/coarsening/contraction/cluster_contraction.h:22-32
     sparsification_target(...), CoarseGraph.sparsify(...), sparsify_level(...)
         kaminpar-shm/coarsening/sparsification_cluster_coarsener.cc:41-228 (DESIGN.md §13)
+    overlay_level(...)
+        kaminpar-shm/coarsening/overlay_cluster_coarsener.cc:34-80 (DESIGN.md §14)
 
 There is no CPU fallback: without the CUDA library / a GPU every call raises.
 """
@@ -19,6 +21,8 @@ import numpy as np
 
 from . import lp
 from .graph import CSRGraph
+
+INT_MAX = 2**31 - 1
 
 
 class ContractionStats(C.Structure):
@@ -56,6 +60,12 @@ class SparsificationClusterCoarseningContext:  # kaminpar.h:185-189, defaults pr
         self.density_target_factor = density_target_factor
         self.edge_target_factor = edge_target_factor
         self.laziness_factor = laziness_factor
+
+
+class OverlayClusterCoarseningContext:  # kaminpar.h (OverlayClusterCoarseningContext), defaults presets.cc:167-171
+    def __init__(self, num_levels: int = 1, max_level: int = INT_MAX):
+        self.num_levels = num_levels
+        self.max_level = max_level
 
 
 class ContractionCoarseningContext:  # kaminpar.h (ContractionCoarseningContext), defaults presets.cc:181-185
@@ -217,6 +227,22 @@ def contract_on_handle(handle: lp.LPHandle, clustering: Optional[np.ndarray]) ->
     stats = ContractionStats()
     lp._check(_lib().kmp_contract_clustering(handle._h, lp._ptr(cl), C.byref(out), C.byref(stats)))
     return CoarseGraph(out, stats, keepalive=handle)
+
+
+def overlay_level(handle: lp.LPHandle, level: int, ctx: Optional[OverlayClusterCoarseningContext],
+                  max_cluster_weight: int, desired: int = 0, communities=None) -> CoarseGraph:
+    """One level of OverlayClusterCoarsener::coarsen() (:34-80) on the graph `handle` holds: 2^num_levels clusterings
+    intersected on the device if `level` (the number of coarse graphs built so far, AbstractClusterCoarsener::level())
+    is at most max_level, else one clustering; then the contraction, with the clustering left on the device.
+
+    The comparison is the reference's, `level <= static_cast<std::size_t>(max_level)`: a negative max_level converts
+    to a huge unsigned value, so it never turns the overlay off."""
+    ctx = ctx or OverlayClusterCoarseningContext()
+    if level <= int(ctx.max_level) % 2**64:
+        handle.cluster_overlay(ctx.num_levels, max_cluster_weight, desired, communities, fetch=False)
+    else:
+        handle.cluster(max_cluster_weight, desired, communities, fetch=False)
+    return contract_on_handle(handle, None)
 
 
 def contract_clustering(graph: CSRGraph, clustering, con_ctx: Optional[ContractionCoarseningContext] = None,

@@ -107,6 +107,9 @@ template <typename T> struct DevBuf {
 } // namespace
 
 cudaMemPool_t kmp_private_pool(int device); // kmp_contract.cuh
+namespace {
+struct OverlayState; // kmp_overlay.cuh
+} // namespace
 
 struct kmp_lp_handle {
   kmp_lp_config cfg{};
@@ -212,6 +215,9 @@ struct kmp_lp_handle {
   DevBuf<uint32_t> ct_flags, ct_rank, ct_cl;
   DevBuf<unsigned long long> ct_counter;
   DevBuf<uint32_t> sp_ctl; // sparsification (kmp_sparsify.cuh): radix-select bins, select state, kept counter
+  // overlay (kmp_overlay.cuh): the stashed clusterings of the last overlay call and the sort's values. The stash is
+  // released by set_graph and kmp_lp_free_scratch, the rest by kmp_lp_free_scratch.
+  OverlayState *ov = nullptr;
   bool slot_state_clean = false; // incoming/slotmap/chist zeroed for current n
 
   // schedule KMP_SCHEDULE_SEQ_STRICT (lp_strict.cuh): sequential engine state
@@ -265,6 +271,10 @@ struct kmp_lp_handle {
   // bal_ctr32: [0] movers [1] scratch [2..3] tier counts [4 + r] moved in round r
   DevBuf<unsigned long long> bal_ctrl, bal_sk_a, bal_sk_b;
 };
+
+namespace {
+void overlay_release(kmp_lp_handle *h, bool scratch); // kmp_overlay.cuh
+} // namespace
 
 namespace kmp {
 // block weights from labels; counts labels >= k (a clustering is not a partition) into *bad. The one range check
@@ -2229,6 +2239,7 @@ static int set_graph_common(kmp_lp_handle *h, uint32_t n, uint32_t m) {
   h->m = m;
   h->have_graph = true;
   h->labels_valid = false;
+  overlay_release(h, false); // stream-ordered: the stash belongs to the previous graph
   h->lists_valid = false;
   h->slot_state_clean = false;
   h->graph_sorted = false;
@@ -2635,6 +2646,7 @@ int kmp_lp_free_scratch(kmp_lp_handle *h) {
   h->ct_cl.release();
   h->ct_counter.release();
   h->sp_ctl.release();
+  overlay_release(h, true);
   for (DevBuf<uint32_t> *b : {&h->bal_cand, &h->bal_under, &h->bal_ctr32, &h->bal_target, &h->bal_lists, &h->bal_sv_a,
                               &h->bal_sv_b, &h->bal_blk}) {
     b->release();
@@ -2968,5 +2980,6 @@ int kmp_lp_step_finish(kmp_lp_handle *h, uint32_t *labels_out, int32_t *block_we
 
 #include "kmp_contract.cuh"
 #include "kmp_sparsify.cuh"
+#include "kmp_overlay.cuh"
 #include "kmp_balance.cuh"
 #include "kmp_underload.cuh"

@@ -115,6 +115,17 @@ class KmpUnderloadStats(C.Structure):  # include/kaminpar_b200_balancer.h
         return list(self.moved[: self.rounds])
 
 
+class KmpOverlayStats(C.Structure):  # include/kaminpar_b200_contraction.h
+    _fields_ = [
+        ("num_clusterings", C.c_uint32),
+        ("num_clusters", C.c_uint32),
+        ("sort_bits", C.c_uint32),
+        ("kernel_launches", C.c_uint32),
+        ("lp_device_ms", C.c_float),
+        ("overlay_device_ms", C.c_float),
+    ]
+
+
 def library_path() -> str:
     return _LIB_PATH
 
@@ -132,7 +143,8 @@ def load_library():
         lib.kmp_last_error.restype = C.c_char_p
         lib.kmp_lp_labels_device.restype = C.c_void_p
         for sym in ("kmp_overload_balance", "kmp_balance_select_all",  # include/kaminpar_b200_balancer.h
-                    "kmp_underload_balance", "kmp_underload_select_all"):
+                    "kmp_underload_balance", "kmp_underload_select_all",
+                    "kmp_lp_cluster_overlay", "kmp_overlay_clusterings"):  # include/kaminpar_b200_contraction.h
             if not hasattr(lib, sym):
                 raise RuntimeError(f"{_LIB_PATH} lacks {sym}; rebuild the library")
         if lib.kmp_lp_abi_version() != ABI_VERSION:  # the ctypes structs below mirror exactly this header version
@@ -415,6 +427,33 @@ class LPHandle:
         comm = None if communities is None else np.ascontiguousarray(communities, np.uint32)
         _check(self._lib.kmp_lp_cluster(self._h, C.c_int32(int(max_cluster_weight)), C.c_uint32(int(desired)),
                                         _ptr(comm), _ptr(out) if fetch else None, C.byref(stats)))
+        return out, stats
+
+    def cluster_overlay(self, num_levels, max_cluster_weight, desired=0, communities=None,
+                        out: Optional[np.ndarray] = None, fetch=True):
+        """kmp_lp_cluster_overlay: 2^num_levels clusterings of the graph (the same arguments, consecutive calls),
+        intersected in OverlayClusterCoarsener's tree order (DESIGN.md §14). The result stays on the device as the
+        handle's labels (contract_on_handle(handle, None) contracts it). Returns (clustering or None, stats)."""
+        stats = KmpOverlayStats()
+        if fetch and out is None:
+            out = np.empty(self._n, np.uint32)
+        comm = None if communities is None else np.ascontiguousarray(communities, np.uint32)
+        _check(self._lib.kmp_lp_cluster_overlay(self._h, C.c_int(int(num_levels)), C.c_int32(int(max_cluster_weight)),
+                                                C.c_uint32(int(desired)), _ptr(comm), _ptr(out) if fetch else None,
+                                                C.byref(stats)))
+        return out, stats
+
+    def overlay(self, clusterings, out: Optional[np.ndarray] = None, fetch=True):
+        """kmp_overlay_clusterings: the overlay tree over given clusterings of the handle's graph (a power of two of
+        them, each n ids in [0, n)). The result becomes the handle's device labels. Returns (overlay or None, stats)."""
+        cl = np.ascontiguousarray(np.asarray(clusterings, np.uint32))
+        if cl.ndim != 2 or cl.shape[1] != self._n:
+            raise ValueError("clusterings must be a sequence of clusterings of the graph's n vertices")
+        stats = KmpOverlayStats()
+        if fetch and out is None:
+            out = np.empty(self._n, np.uint32)
+        _check(self._lib.kmp_overlay_clusterings(self._h, C.c_uint32(cl.shape[0]), _ptr(cl),
+                                                 _ptr(out) if fetch else None, C.byref(stats)))
         return out, stats
 
     def refine(self, k, max_block_weights, partition: Optional[np.ndarray], min_block_weights=None,
