@@ -77,7 +77,8 @@ typedef struct {
   uint32_t sync_subrounds;     /* S: hashed sub-rounds per degree group and iteration (8; 0 = 8, at most 31) */
   uint32_t sync_granule_log2;  /* vertices u >> g share a sub-round (4) */
   uint32_t sync_commit_passes; /* commit passes crediting departures: 1 clusterer, 4 refiner. The clusterer's
-                                  commit is single-pass: kmp_lp_cluster refuses > 1 with KMP_ERR_UNSUPPORTED */
+                                  commit is single-pass: kmp_lp_cluster and kmp_lp_step_begin_cluster refuse
+                                  > 1 with KMP_ERR_UNSUPPORTED */
   int32_t device;              /* CUDA device ordinal, -1 = current */
   int32_t schedule;            /* KMP_SCHEDULE_SYNC (default) or KMP_SCHEDULE_SEQ_STRICT */
 } kmp_lp_config;

@@ -2800,6 +2800,9 @@ int kmp_lp_step_begin_cluster(kmp_lp_handle *h, int32_t max_cluster_weight, cons
   if (h->cfg.schedule != KMP_SCHEDULE_SYNC) {
     return fail(KMP_ERR_UNSUPPORTED, "the stepping API drives the sync schedule");
   }
+  if (h->cfg.sync_commit_passes > 1) { // as kmp_lp_cluster: the cluster commit kernels decide in one pass
+    return fail(KMP_ERR_UNSUPPORTED, "the clusterer's sync commit is single-pass (sync_commit_passes must be 1)");
+  }
   const uint32_t n = h->n;
   rc = ensure_lists(h);
   if (rc != KMP_OK) {
@@ -2895,6 +2898,9 @@ int kmp_lp_step_sweep(kmp_lp_handle *h, uint32_t iter, uint32_t sg, void *d_send
   if (h == nullptr || h->step_mode < 0 || d_send == nullptr) {
     return fail(KMP_ERR_INVALID, "bad argument");
   }
+  if (sg >= kNumGroups * h->lists_S) { // subround_of_sg indexes list_off by sg
+    return fail(KMP_ERR_INVALID, "bad sub-round");
+  }
   const RunCtx rc{h->step_mode, h->step_labels, h->step_mcw, h->step_has_min, h->step_has_comm};
   return dist_sweep_pack(h, rc, iter, sg, subround_of_sg(h, sg), static_cast<uint32_t *>(d_send));
 }
@@ -2904,12 +2910,15 @@ int kmp_lp_step_commit(kmp_lp_handle *h, uint32_t iter, uint32_t sg, const void 
   if (h == nullptr || h->step_mode < 0 || d_gathered == nullptr) {
     return fail(KMP_ERR_INVALID, "bad argument");
   }
+  if (sg >= kNumGroups * h->lists_S) {
+    return fail(KMP_ERR_INVALID, "bad sub-round");
+  }
   const RunCtx rc{h->step_mode, h->step_labels, h->step_mcw, h->step_has_min, h->step_has_comm};
   return commit_subround(h, rc, iter, sg, subround_of_sg(h, sg), static_cast<const uint32_t *>(d_gathered));
 }
 
 int kmp_lp_step_end_iteration(kmp_lp_handle *h, uint32_t *moved) {
-  if (h == nullptr || moved == nullptr) {
+  if (h == nullptr || h->step_mode < 0 || moved == nullptr) {
     return fail(KMP_ERR_INVALID, "bad argument");
   }
   uint32_t host[2] = {0, 0};

@@ -1,6 +1,7 @@
 """Stepping / sharded path on real GPUs: world = 1 always (pack -> unpack -> accumulate -> commit
 through the stepping C ABI), world = 2 over NCCL when the box has two GPUs. Result must equal the
-oracle's `sync` schedule bit for bit, i.e. be independent of the number of GPUs."""
+oracle's `sync` schedule bit for bit, i.e. be independent of the number of GPUs. Worlds of 2, 3 and 5
+ranks emulated on one GPU: tests/test_gpu_shards.py."""
 import os
 import sys
 
@@ -155,67 +156,3 @@ def test_library_nccl_two_gpus(tmp_path):
     out = str(tmp_path / "r")
     mp.spawn(_run_rank_library, args=(2, 29741, out), nprocs=2, join=True)
     _check(2, out)
-
-
-def test_two_shards_emulated_on_one_gpu():
-    """Both ranks of a world-2 run as two handles on ONE GPU with a hand-made all-gather: exercises
-    the rank slicing, hub ownership, pack / unpack / accumulate kernels without NCCL."""
-    import torch
-
-    from kaminpar_b200 import lp
-    from kaminpar_b200.dist import CudaBackend
-    from kaminpar_b200.graph import rmat
-    from oracle import bindings as B
-
-    dev = torch.device("cuda", 0)
-    g = B.oracle_rearrange(rmat(16, 16, 3))[0]  # has vertices of every kernel tier
-    ctx = lp.create_default_context()
-    ctx.engine.seed = 2
-    ctx.partition.setup(g, 8, 0.03)
-    mcw = lp.compute_max_cluster_weight(ctx.coarsening, ctx.partition, g.n, g.total_node_weight())
-    world = 2
-    backs = []
-    for r in range(world):
-        h = lp.LPHandle(lp._cluster_config(ctx.coarsening.clustering.lp, ctx.engine))
-        h.set_graph(g)
-        b = CudaBackend(h, dev)
-        b.set_shard(r, world)
-        b.begin_cluster(mcw, None)
-        backs.append(b)
-    moved_rounds = []
-    for it in range(5):
-        for b in backs:
-            b.begin_iteration()
-        for sg in range(backs[0].num_subrounds()):
-            cap, size = backs[0].subround_cap(sg)
-            if size == 0:
-                continue
-            words = 4 + 2 * cap
-            recv = torch.zeros(words * world, dtype=torch.int32, device=dev)
-            total = 0
-            for r, b in enumerate(backs):
-                send = torch.zeros(words, dtype=torch.int32, device=dev)
-                b.sweep(it, sg, send)
-                recv[r * words:(r + 1) * words] = send
-                total += int(send[0].item())
-            assert total <= size, (sg, total, size)
-            for b in backs:
-                b.commit(it, sg, recv)
-        moved = [b.end_iteration() for b in backs]
-        assert moved[0] == moved[1]
-        moved_rounds.append(moved[0])
-        if moved[0] == 0:
-            break
-    bufs = []
-    for b in backs:
-        buf = torch.zeros(g.n, dtype=torch.int32, device=dev)
-        b.favored_export(buf)
-        bufs.append(buf)
-    fav = torch.maximum(bufs[0], bufs[1])  # MAX all-reduce (values are small non-negative xor diffs)
-    outs = []
-    for b in backs:
-        b.favored_import(fav.clone())
-        outs.append(b.finish(g.n)[0])
-    expect, st = B.oracle_lp_cluster(g, 2, mcw, schedule=B.SYNC, return_stats=True)
-    assert moved_rounds == list(st[0].moved[: st[0].iterations])
-    assert np.array_equal(outs[0], expect) and np.array_equal(outs[1], expect)
