@@ -200,6 +200,10 @@ struct kmp_lp_handle {
   // clusterer hub path (gather + rate): per list entry the start of its row in hub_lab (sub-round-relative) and its
   // first rate item result; the (entry, hash class) rate items of each sub-round, largest degree first
   DevBuf<uint32_t> t4_lab_off, t4_rate_begin, t4_rate_entry, t4_rate_cls;
+  // unit edge weights: per list entry the start of its chunks' class offsets in hub_cls (sub-round-relative)
+  DevBuf<uint32_t> t4_cls_off;
+  uint64_t t4_max_subround_cls = 0;
+  DevBuf<uint16_t> hub_cls; // class offsets of the running sub-round's staged chunks (hub_sort_classes + 1 each)
   std::vector<uint32_t> t4_rate_off; // S + 1
   uint64_t t4_max_subround_edges = 0;
   DevBuf<uint32_t> hub_lab; // staged neighbour labels of the running sub-round's hubs (4 B per edge)
@@ -709,6 +713,10 @@ template <int MODE, bool EW, bool P64> cudaError_t launch_sweep_t(kmp_lp_handle 
       hb.num_items = ihi - ilo;
       hb.lab = h->hub_lab.p;
       hb.lab_off = h->t4_lab_off.p + first;
+      if constexpr (!EW) {
+        hb.cls = h->hub_cls.p;
+        hb.cls_off = h->t4_cls_off.p + first;
+      }
       sweep_hub_gather<P64><<<capped(h, std::min<uint32_t>(hb.num_items, kSMs * 8)), 256, 0, h->sweep_stream>>>(a, hb);
       const uint32_t rlo = h->t4_rate_off[s_idx], rhi = h->t4_rate_off[s_idx + 1];
       hb.item_entry = h->t4_rate_entry.p + rlo;
@@ -913,6 +921,7 @@ int ensure_lists(kmp_lp_handle *h) {
     h->t4_max_slots = 0;
     h->t4_max_wave_edges = 0;
     h->t4_max_subround_edges = 0;
+    h->t4_max_subround_cls = 0;
     if (t4_cnt > 0) {
       DevBuf<uint32_t> &d_deg = h->t4_tmp_deg, &d_beg = h->t4_tmp_beg, &d_ids = h->t4_tmp_ids; // grow-only
       KMP_CUDA(d_deg.ensure(t4_cnt));
@@ -992,17 +1001,22 @@ int ensure_lists(kmp_lp_handle *h) {
       }
       // clusterer: per entry its row in the staged labels and its first result slot, and the (entry, hash class)
       // rate items of every sub-round, largest degree first (the longest items start first)
-      std::vector<uint32_t> loff(t4_cnt), rbeg(t4_cnt), rent, rcls, ord;
+      std::vector<uint32_t> loff(t4_cnt), coff(t4_cnt), rbeg(t4_cnt), rent, rcls, ord;
       h->t4_rate_off.assign(S + 1, 0);
       size_t max_rate = 0;
       for (uint32_t sr = 0; sr < S; ++sr) {
         const uint32_t lo = h->list_off[kHubTier * S + sr] - t4_begin, hi = h->list_off[kHubTier * S + sr + 1] - t4_begin;
-        uint64_t edges = 0; // <= m < 2^32
+        // edges <= m < 2^32; cls <= (m / 2048 + hubs) * 257 < 2^31 (hubs <= m / 8192)
+        uint64_t edges = 0, cls = 0;
         uint32_t res = 0;
         ord.clear();
         for (uint32_t i = lo; i < hi; ++i) {
           loff[i] = static_cast<uint32_t>(edges);
           edges += deg[i];
+          coff[i] = static_cast<uint32_t>(cls);
+          if (h->adjwgt == nullptr) {
+            cls += static_cast<uint64_t>((deg[i] + kChunkEdges - 1) / kChunkEdges) * (hub_sort_classes(deg[i]) + 1);
+          }
           rbeg[i] = res;
           res += hub_classes(deg[i]);
           ord.push_back(i);
@@ -1017,6 +1031,7 @@ int ensure_lists(kmp_lp_handle *h) {
         h->t4_rate_off[sr + 1] = static_cast<uint32_t>(rent.size());
         max_rate = std::max<size_t>(max_rate, res);
         h->t4_max_subround_edges = std::max(h->t4_max_subround_edges, edges);
+        h->t4_max_subround_cls = std::max(h->t4_max_subround_cls, cls);
       }
       max_sel = std::max(max_sel, max_rate);
       KMP_CUDA(h->t4_lab_off.ensure(t4_cnt));
@@ -1024,6 +1039,8 @@ int ensure_lists(kmp_lp_handle *h) {
       KMP_CUDA(h->t4_rate_entry.ensure(rent.size()));
       KMP_CUDA(h->t4_rate_cls.ensure(rcls.size()));
       KMP_CUDA(cudaMemcpyAsync(h->t4_lab_off.p, loff.data(), t4_cnt * 4, cudaMemcpyHostToDevice, h->stream));
+      KMP_CUDA(h->t4_cls_off.ensure(t4_cnt));
+      KMP_CUDA(cudaMemcpyAsync(h->t4_cls_off.p, coff.data(), t4_cnt * 4, cudaMemcpyHostToDevice, h->stream));
       KMP_CUDA(cudaMemcpyAsync(h->t4_rate_begin.p, rbeg.data(), t4_cnt * 4, cudaMemcpyHostToDevice, h->stream));
       KMP_CUDA(cudaMemcpyAsync(h->t4_rate_entry.p, rent.data(), rent.size() * 4, cudaMemcpyHostToDevice, h->stream));
       KMP_CUDA(cudaMemcpyAsync(h->t4_rate_cls.p, rcls.data(), rcls.size() * 4, cudaMemcpyHostToDevice, h->stream));
@@ -1101,6 +1118,7 @@ int ensure_scratch(kmp_lp_handle *h, int mode, uint32_t num_labels) {
   // regions, cursors and an overflow list
   if (mode == 0 && h->t4_max_subround_edges > 0) {
     KMP_CUDA(h->hub_lab.ensure(h->t4_max_subround_edges));
+    KMP_CUDA(h->hub_cls.ensure(h->t4_max_subround_cls));
   }
   if (mode == 1 && h->t4_max_slots > 0) {
     KMP_CUDA(h->hub_tab.ensure(h->t4_max_slots)); // no initialisation: the cursors say how much of a region is valid
@@ -2629,6 +2647,7 @@ int kmp_lp_free_scratch(kmp_lp_handle *h) {
   h->hub_cursor.release();
   h->hub_ovf.release();
   h->hub_lab.release();
+  h->hub_cls.release();
   h->labg.release();
   h->sort_keys_in.release();
   h->sort_keys_out.release();
@@ -2992,3 +3011,20 @@ int kmp_lp_step_finish(kmp_lp_handle *h, uint32_t *labels_out, int32_t *block_we
 #include "kmp_overlay.cuh"
 #include "kmp_balance.cuh"
 #include "kmp_underload.cuh"
+
+#ifdef KMP_HUB_PHASE_STAMPS
+// scripts/hub_rate_phases.py: reads (and with reset != 0 zeroes) the rate kernel's 7 phase accumulators
+// (lp_sweep.cuh, g_hub_phase). Only in a library built with -DKMP_HUB_PHASE_STAMPS.
+extern "C" int kmp_hub_phase_read(unsigned long long *out, int reset) {
+  if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpyFromSymbol(out, kmp::g_hub_phase, sizeof(kmp::g_hub_phase)) != cudaSuccess) {
+    return 1;
+  }
+  if (reset != 0) {
+    const unsigned long long zero[7] = {};
+    if (cudaMemcpyToSymbol(kmp::g_hub_phase, zero, sizeof(zero)) != cudaSuccess) {
+      return 1;
+    }
+  }
+  return 0;
+}
+#endif

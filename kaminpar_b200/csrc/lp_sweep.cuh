@@ -667,13 +667,19 @@ __global__ void __launch_bounds__(T *TEAMS, team_ctas_per_sm<T>()) sweep_team(co
 // tier 7 (deg >= 8192 / 16384), clusterer (MODE 0): label-partitioned rating with final results per CTA.
 //   gather : edge-parallel over the 2048-edge chunks of the sub-round's hubs: every neighbour label is gathered
 //            once and written, coalesced, to a scratch row per hub (4 B per edge); the stamps mark pull activation.
+//            With unit edge weights each chunk is counting-sorted by class (lowbias32(label) & (Ks - 1), Ks =
+//            hub_sort_classes(deg)) in shared memory before it is written back, and its Ks + 1 class offsets are
+//            stored beside the row.
 //   rate   : one 1024-thread CTA per work item (hub u, hash class c of K_u = hub_classes(deg) classes, taken from a
-//            queue in order of decreasing degree). It streams all staged labels of u from L2 and inserts only those
-//            with lowbias32(label) & (K_u - 1) == c -- compacted per warp first, so a class costs inserts only for
-//            its own labels -- into a 16384-slot shared-memory table with a claim list, then selects as the team
-//            kernels do. Classes of a hub hold disjoint labels, so each result is final for its class: no merge.
-//            A class that claims more than the list holds is split by the next hash bit and streamed again, until
-//            every sub-class fits (lowbias32 is a bijection, so this terminates).
+//            queue in order of decreasing degree). Its warps claim (chunk, part) pieces from a shared counter and
+//            read only class c's range of each sorted chunk, inserting every label into a 16384-slot shared-memory
+//            table with a claim list; then it selects as the team kernels do. Classes of a hub hold disjoint labels,
+//            so each result is final for its class: no merge. Where a chunk's range holds more than class c
+//            (edge weights: unsorted chunks; K_u > Ks; a split class) the labels are filtered by their hash and
+//            compacted per warp first. A class that claims more than the list holds is split by the next hash bit
+//            and read again, until every sub-class fits (lowbias32 is a bijection, so this terminates). While an
+//            item streams, one warp claims the next item and loads its header, so the CTA does not wait on that
+//            chain of dependent loads between items.
 //   final  : as below: the arg-max over the K_u class results of each hub.
 // tier 7, refiner (MODE 1): edge-parallel, label-partitioned two-pass aggregation (a refiner hub sees at most k
 // labels, so the slice maps compress 256 edges to <= k appends). No random access ever touches a table outside
@@ -740,6 +746,10 @@ struct HubArgs {
   uint32_t *__restrict__ lab;
   const uint32_t *__restrict__ lab_off;
   const uint32_t *__restrict__ item_cls;
+  // unit edge weights: each staged chunk is sorted by class; its hub_sort_classes + 1 class offsets start at
+  // cls[cls_off[entry] + chunk * (Ks + 1)]. nullptr with edge weights (chunks stay in edge order)
+  uint16_t *__restrict__ cls;
+  const uint32_t *__restrict__ cls_off;
 };
 
 // buckets of a hub: a power of two with <= kBucketTargetFill expected distinct labels per bucket
@@ -1181,10 +1191,28 @@ __host__ __device__ __forceinline__ uint32_t hub_classes(uint32_t full_degree) {
   return p;
 }
 
-// gather: one 256-thread CTA per (hub, 2048-edge chunk) item, 8 independent label gathers per thread
-template <bool P64> __global__ void __launch_bounds__(256) sweep_hub_gather(const SweepArgs a, const HubArgs hb) {
+// classes a staged chunk is sorted by: the hub's hash classes, at most kHubSortClasses of them (a hub with more
+// classes reads the range of its class's low bits and filters by the rest); 1 (unsorted) with edge weights, whose
+// rate items read each label's weight by its edge index
+constexpr uint32_t kHubSortClasses = 256;
+static_assert(kHubSortClasses <= 256, "sweep_hub_gather scans the class counts with one class per thread");
+__host__ __device__ __forceinline__ uint32_t hub_sort_classes(uint32_t full_degree) {
+  const uint32_t k = hub_classes(full_degree);
+  return k < kHubSortClasses ? k : kHubSortClasses;
+}
+
+// gather: one 256-thread CTA per (hub, 2048-edge chunk) item, 8 independent label gathers per thread. With
+// hb.cls_off set (unit edge weights), the chunk is counting-sorted by sort class in shared memory, written back to
+// its own range of the row, and its Ks + 1 class offsets go to hb.cls. Order inside a class is free: ratings are
+// sums and the selection is a total order.
+template <bool P64> __global__ void __launch_bounds__(256, 8) sweep_hub_gather(const SweepArgs a, const HubArgs hb) {
   constexpr int B = kChunkEdges / 256;
+  __shared__ uint32_t s_lab[kChunkEdges], s_sorted[kChunkEdges];
+  __shared__ uint16_t s_rank[kChunkEdges]; // a label's rank within its class in the chunk
+  __shared__ uint32_t s_cnt[kHubSortClasses + 1];
+  __shared__ uint32_t s_wsum[256 / 32];
   const int lane = threadIdx.x & 31;
+  const int wib = threadIdx.x >> 5;
   for (uint32_t it = blockIdx.x; it < hb.num_items; it += gridDim.x) {
     const uint32_t entry = hb.item_entry[it];
     const uint32_t u = hb.item_u[it];
@@ -1205,18 +1233,90 @@ template <bool P64> __global__ void __launch_bounds__(256) sweep_hub_gather(cons
       const uint32_t e = cbeg + j * 256 + threadIdx.x;
       v[j] = e < cend ? adj[e] : kEmpty;
     }
+    const uint32_t Ks = hb.cls_off != nullptr ? hub_sort_classes(hb.item_deg[it]) : 1u;
     bool hit = false;
 #pragma unroll
     for (int j = 0; j < B; ++j) {
       if (v[j] != kEmpty) {
         const typename LabG<P64>::word g = load_labg<P64>(a, v[j]);
         hit = hit || stamp_hit(LabG<P64>::stamp(g), a.window);
-        out[cbeg + j * 256 + threadIdx.x] = LabG<P64>::label(g);
+        if (Ks == 1) {
+          out[cbeg + j * 256 + threadIdx.x] = LabG<P64>::label(g);
+        } else {
+          s_lab[j * 256 + threadIdx.x] = LabG<P64>::label(g);
+        }
       }
     }
     if (a.pull && __any_sync(kFull, hit) && lane == 0) {
       atomicOr(&hb.hit[entry], 1u);
     }
+    if (Ks == 1) {
+      continue;
+    }
+    // ---- counting sort by class: per-class counts (warp-aggregated: one atomic per class and warp), an
+    // exclusive scan of the counts, the scatter into s_sorted and a coalesced copy back to the row
+    for (uint32_t t = threadIdx.x; t <= Ks; t += 256) {
+      s_cnt[t] = 0;
+    }
+    __syncthreads();
+#pragma unroll 1
+    for (int j = 0; j < B; ++j) {
+      const uint32_t e = j * 256 + threadIdx.x;
+      const uint32_t cls = cbeg + e < cend ? lowbias32(s_lab[e]) & (Ks - 1) : kEmpty;
+      const unsigned peers = __match_any_sync(kFull, cls);
+      const int leader = __ffs(peers) - 1;
+      uint32_t base = 0;
+      if (cls != kEmpty && lane == leader) {
+        base = atomicAdd(&s_cnt[cls], static_cast<uint32_t>(__popc(peers)));
+      }
+      s_rank[e] =
+          static_cast<uint16_t>(__shfl_sync(kFull, base, leader) + __popc(peers & ((1u << lane) - 1u)));
+    }
+    __syncthreads();
+    {
+      const uint32_t c = threadIdx.x < Ks ? s_cnt[threadIdx.x] : 0u;
+      uint32_t x = c;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t y = __shfl_up_sync(kFull, x, o);
+        x += lane >= o ? y : 0u;
+      }
+      if (lane == 31) {
+        s_wsum[wib] = x;
+      }
+      __syncthreads();
+      for (int w = 0; w < wib; ++w) {
+        x += s_wsum[w];
+      }
+      if (threadIdx.x < Ks) {
+        s_cnt[threadIdx.x] = x - c; // only this thread reads or writes entry threadIdx.x
+      }
+      if (threadIdx.x == 0) {
+        s_cnt[Ks] = cend - cbeg;
+      }
+    }
+    __syncthreads();
+#pragma unroll 1
+    for (int j = 0; j < B; ++j) {
+      const uint32_t e = j * 256 + threadIdx.x;
+      if (cbeg + e < cend) {
+        const uint32_t l = s_lab[e];
+        s_sorted[s_cnt[lowbias32(l) & (Ks - 1)] + s_rank[e]] = l;
+      }
+    }
+    uint16_t *off = hb.cls + hb.cls_off[entry] + hb.item_chunk[it] * (Ks + 1);
+    for (uint32_t t = threadIdx.x; t <= Ks; t += 256) {
+      off[t] = static_cast<uint16_t>(s_cnt[t]);
+    }
+    __syncthreads();
+#pragma unroll 1
+    for (int j = 0; j < B; ++j) {
+      const uint32_t e = j * 256 + threadIdx.x;
+      if (cbeg + e < cend) {
+        out[cbeg + e] = s_sorted[e];
+      }
+    }
+    __syncthreads(); // s_sorted and s_cnt are free for the next item
   }
 }
 
@@ -1260,6 +1360,73 @@ __device__ __forceinline__ bool rate_insert(uint32_t *keys, int32_t *vals, uint1
   return base + n > limit;
 }
 
+// header of a rate item in shared memory, loaded by one thread
+struct RateHead {
+  uint32_t it;  // item index; >= num_items once the queue is drained
+  uint32_t go;  // the item's hub is this rank's and active
+  uint32_t c0, u, beg, full_deg, own, row, coff, res;
+  int32_t uw, own_w;
+};
+
+__device__ __forceinline__ void rate_load_head(const SweepArgs &a, const HubArgs &hb, RateHead *h) {
+  const uint32_t it = atomicAdd(hb.queue, 1u);
+  h->it = it;
+  h->go = 0;
+  if (it >= hb.num_items) {
+    return;
+  }
+  const uint32_t entry = hb.item_entry[it];
+  const uint32_t u = a.list[entry];
+  if (entry % hb.world != hb.rank || !(a.active == nullptr || a.pull || a.active[u] != 0)) {
+    return;
+  }
+  const uint32_t beg = a.xadj[u];
+  const uint32_t own = a.label[u];
+  h->go = 1;
+  h->c0 = hb.item_cls[it];
+  h->u = u;
+  h->beg = beg;
+  h->full_deg = a.xadj[u + 1] - beg;
+  h->own = own;
+  h->row = hb.lab_off[entry];
+  h->coff = hb.cls_off != nullptr ? hb.cls_off[entry] : 0u;
+  h->res = hb.sel_begin[entry];
+  h->uw = a.vwgt != nullptr ? a.vwgt[u] : 1;
+  h->own_w = a.weight[own];
+}
+
+// Per-phase device time of the rate kernel's items, for scripts/hub_rate_phases.py: only a library built with
+// -DKMP_HUB_PHASE_STAMPS takes %globaltimer stamps; otherwise the stamps compile to nothing. Thread 0 adds, in ns:
+// [0] waiting for the item's header (from the end of the previous item to the barrier after which it is read),
+// [1] stream + insert, [2] select, [3] clear (also the full clear of a split), [4] items rated, [5] items claimed,
+// [6] time the loading thread spends in rate_load_head (for the next item).
+#ifdef KMP_HUB_PHASE_STAMPS
+constexpr bool kHubPhaseStamps = true;
+#else
+constexpr bool kHubPhaseStamps = false;
+#endif
+__device__ unsigned long long g_hub_phase[7];
+__device__ __forceinline__ unsigned long long phase_clock() {
+  unsigned long long t = 0;
+  if constexpr (kHubPhaseStamps) {
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  }
+  return t;
+}
+// adds now - t0 (or 1 when count) to slot i and returns now
+__device__ __forceinline__ unsigned long long phase_add(int i, unsigned long long t0, bool count = false) {
+  const unsigned long long t = phase_clock();
+  if constexpr (kHubPhaseStamps) {
+    atomicAdd(&g_hub_phase[i], count ? 1ull : t - t0);
+  }
+  return t;
+}
+__device__ __forceinline__ void rate_load_head_timed(const SweepArgs &a, const HubArgs &hb, RateHead *h) {
+  const unsigned long long t0 = phase_clock();
+  rate_load_head(a, hb, h);
+  phase_add(6, t0);
+}
+
 // rate: one CTA per (hub, hash class) item; writes the class's best and favored candidates
 template <bool EW> __global__ void __launch_bounds__(kRateThreads, 1) sweep_hub_rate(const SweepArgs a, const HubArgs hb) {
   constexpr int T = kRateThreads;
@@ -1272,7 +1439,8 @@ template <bool EW> __global__ void __launch_bounds__(kRateThreads, 1) sweep_hub_
   int32_t *stage_w = reinterpret_cast<int32_t *>(stage_k + kWarps * kRateStage); // EW only
   uint16_t *list = reinterpret_cast<uint16_t *>(stage_k + (EW ? 2 : 1) * kWarps * kRateStage);
   __shared__ Cand s_red[kWarps];
-  __shared__ uint32_t s_item, s_claims;
+  __shared__ RateHead s_head[2];
+  __shared__ uint32_t s_claims, s_piece;
   const int tid = threadIdx.x;
   const int lane = tid & 31;
   const int wib = tid >> 5;
@@ -1285,67 +1453,113 @@ template <bool EW> __global__ void __launch_bounds__(kRateThreads, 1) sweep_hub_
   }
   // a class with one label never splits, one with two may: the limit is >= 2 so that K stays below 2^32
   const uint32_t limit = (hb.sel_limit != 0 && hb.sel_limit < kRateListCap) ? max(hb.sel_limit, 2u) : kRateListCap;
-  while (true) {
+  if (tid == 0) {
+    rate_load_head_timed(a, hb, &s_head[0]);
+  }
+  unsigned long long t_ph = phase_clock(); // thread 0: the last phase stamp
+  for (uint32_t b = 0;; b ^= 1) {
+    __syncthreads(); // s_head[b] is loaded, the table is clean, s_head[b ^ 1] is no longer read
     if (tid == 0) {
-      s_item = atomicAdd(hb.queue, 1u);
+      t_ph = phase_add(0, t_ph);
     }
-    __syncthreads(); // also: the table is clean
-    const uint32_t it = s_item;
-    if (it >= hb.num_items) {
+    if (s_head[b].it >= hb.num_items) {
       break;
     }
-    const uint32_t entry = hb.item_entry[it];
-    const uint32_t c0 = hb.item_cls[it];
-    const uint32_t u = a.list[entry];
-    if (entry % hb.world == hb.rank && (a.active == nullptr || a.pull || a.active[u] != 0)) {
-      const uint32_t beg = a.xadj[u];
-      const uint32_t full_deg = a.xadj[u + 1] - beg;
+    if (tid == 0) {
+      phase_add(5, 0, true);
+    }
+    // lane 0 of the last warp loads the next item's header while this item streams
+    bool next = tid == (kWarps - 1) * 32;
+    if (s_head[b].go != 0) {
+      const uint32_t c0 = s_head[b].c0, u = s_head[b].u, beg = s_head[b].beg, full_deg = s_head[b].full_deg;
+      const uint32_t own = s_head[b].own;
+      const int32_t uw = s_head[b].uw, own_w = s_head[b].own_w;
       const uint32_t deg = min(full_deg, a.max_num_neighbors);
       const uint32_t K0 = hub_classes(full_deg);
-      const uint32_t own = a.label[u];
-      const int32_t uw = a.vwgt != nullptr ? a.vwgt[u] : 1;
-      const int32_t own_w = a.weight[own];
+      const uint32_t Ks = EW ? 1u : hub_sort_classes(full_deg);
+      // a chunk is read in P parts of about 256 labels of the class each: (chunk, part) pieces go to the warps
+      const uint32_t pshift = Ks >= 8 ? 0u : 3u - (31 - __clz(Ks));
+      const uint32_t pieces = ((deg + kChunkEdges - 1) / kChunkEdges) << pshift;
       const bool store_fav = (uw == own_w) && (own_w <= a.max_cluster_weight / 2);
-      const uint32_t *lab = hb.lab + hb.lab_off[entry];
+      const uint32_t *lab = hb.lab + s_head[b].row;
+      const uint16_t *coff = hb.cls + s_head[b].coff;
       Cand best = cand_none(), fav = cand_none();
       uint32_t cls = c0, K = K0;
       while (true) {
         if (tid == 0) {
           s_claims = 0;
+          s_piece = 0;
         }
         __syncthreads();
-        // ---- stream the staged labels: each warp takes 256-label blocks, compacts the labels of class `cls`
-        // (mod K) in its 64-entry ring and inserts them 32 at a time. No barrier inside: a warp stops once the claims
-        // have passed the limit, after at most one more batch of 32 claims, so the table stays below 3/4 full.
+        if (tid == 0) {
+          t_ph = phase_clock();
+        }
+        if (next) {
+          rate_load_head_timed(a, hb, &s_head[b ^ 1]);
+          next = false;
+        }
+        // ---- read class `cls` (mod K): the range of its sort class in each chunk. Only where that range may
+        // hold other classes (K > Ks) are the labels filtered and compacted in the warp's 64-entry ring, then
+        // inserted 32 at a time. No barrier inside: a warp stops once the claims have passed the limit, after at
+        // most one more batch of 32 claims, so the table stays below 3/4 full.
+        const bool filter = K > Ks;
+        const uint32_t scls = cls & (Ks - 1);
         bool wover = false;
         uint32_t head = 0, pend = 0; // ring index of the oldest staged label, labels staged (warp-uniform)
-        for (uint32_t e0 = wib * 32 * B; e0 < deg && !wover; e0 += T * B) {
-          uint32_t kb[B];
-#pragma unroll
-          for (int j = 0; j < B; ++j) {
-            const uint32_t e = e0 + j * 32 + lane;
-            kb[j] = e < deg ? __ldcg(lab + e) : kEmpty;
+        while (!wover) {
+          uint32_t p = 0;
+          if (lane == 0) {
+            p = atomicAdd(&s_piece, 1u);
           }
+          p = __shfl_sync(kFull, p, 0);
+          if (p >= pieces) {
+            break;
+          }
+          const uint32_t ch = p >> pshift;
+          const uint32_t step = 32u << pshift; // lane stride within the range
+          uint32_t lo = 0, hi = min(deg - ch * kChunkEdges, static_cast<uint32_t>(kChunkEdges));
+          if (Ks > 1) {
+            const uint16_t *o = coff + ch * (Ks + 1) + scls;
+            lo = o[0];
+            hi = o[1];
+          }
+          const uint32_t *cl = lab + ch * kChunkEdges;
+          const uint32_t wbase = beg + ch * kChunkEdges; // edge index of the chunk's first label (EW: unsorted)
+          for (uint32_t i0 = lo + (p & ((1u << pshift) - 1)) * 32; i0 < hi && !wover; i0 += step * B) {
+            uint32_t kb[B];
 #pragma unroll
-          for (int j = 0; j < B; ++j) {
-            if (!wover) {
-              const bool in = kb[j] != kEmpty && (lowbias32(kb[j]) & (K - 1)) == cls;
-              const unsigned m = __ballot_sync(kFull, in);
-              if (in) {
-                const uint32_t pos = (head + pend + __popc(m & below)) & (kRateStage - 1);
-                stk[pos] = kb[j];
-                if (EW) {
-                  stw[pos] = a.adjwgt[beg + e0 + j * 32 + lane];
+            for (int j = 0; j < B; ++j) {
+              const uint32_t i = i0 + j * step + lane;
+              kb[j] = i < hi ? __ldcg(cl + i) : kEmpty;
+            }
+#pragma unroll
+            for (int j = 0; j < B; ++j) {
+              if (!wover) {
+                const uint32_t i = i0 + j * step + lane;
+                if (!filter) {
+                  const bool v = kb[j] != kEmpty;
+                  wover = rate_insert<EW>(keys, vals, list, &s_claims, limit, kb[j], (EW && v) ? a.adjwgt[wbase + i] : 1,
+                                          v, lane);
+                  continue;
                 }
-              }
-              pend += __popc(m);
-              if (pend >= 32) {
-                __syncwarp();
-                const uint32_t sl = (head + lane) & (kRateStage - 1);
-                wover = rate_insert<EW>(keys, vals, list, &s_claims, limit, stk[sl], EW ? stw[sl] : 1, true, lane);
-                __syncwarp(); // the ring slots are read before they are staged again
-                head = (head + 32) & (kRateStage - 1);
-                pend -= 32;
+                const bool in = kb[j] != kEmpty && (lowbias32(kb[j]) & (K - 1)) == cls;
+                const unsigned m = __ballot_sync(kFull, in);
+                if (in) {
+                  const uint32_t pos = (head + pend + __popc(m & below)) & (kRateStage - 1);
+                  stk[pos] = kb[j];
+                  if (EW) {
+                    stw[pos] = a.adjwgt[wbase + i];
+                  }
+                }
+                pend += __popc(m);
+                if (pend >= 32) {
+                  __syncwarp();
+                  const uint32_t sl = (head + lane) & (kRateStage - 1);
+                  wover = rate_insert<EW>(keys, vals, list, &s_claims, limit, stk[sl], EW ? stw[sl] : 1, true, lane);
+                  __syncwarp(); // the ring slots are read before they are staged again
+                  head = (head + 32) & (kRateStage - 1);
+                  pend -= 32;
+                }
               }
             }
           }
@@ -1357,6 +1571,9 @@ template <bool EW> __global__ void __launch_bounds__(kRateThreads, 1) sweep_hub_
           wover = rate_insert<EW>(keys, vals, list, &s_claims, limit, v ? stk[sl] : 0u, (EW && v) ? stw[sl] : 1, v, lane);
         }
         const bool over = __syncthreads_or(wover);
+        if (tid == 0) {
+          t_ph = phase_add(1, t_ph);
+        }
         if (over) {
           // more labels than the list takes: clear the whole table (not every claim is listed), split the class
           // by the next hash bit and stream again
@@ -1366,6 +1583,9 @@ template <bool EW> __global__ void __launch_bounds__(kRateThreads, 1) sweep_hub_
           }
           K <<= 1;
           __syncthreads();
+          if (tid == 0) {
+            t_ph = phase_add(3, t_ph);
+          }
           continue;
         }
         const uint32_t nc = s_claims;
@@ -1434,6 +1654,9 @@ template <bool EW> __global__ void __launch_bounds__(kRateThreads, 1) sweep_hub_
         if (cand_better<0>(cb, best)) {
           best = cb;
         }
+        if (tid == 0) {
+          t_ph = phase_add(2, t_ph);
+        }
         // every thread clears the listed slots it scanned
         for (uint32_t l = tid; l < nc; l += T) {
           const uint32_t s = list[l];
@@ -1441,6 +1664,9 @@ template <bool EW> __global__ void __launch_bounds__(kRateThreads, 1) sweep_hub_
           vals[s] = 0;
         }
         __syncthreads(); // table clean, s_claims read
+        if (tid == 0) {
+          t_ph = phase_add(3, t_ph);
+        }
         // next class: the second half of the deepest split whose first half is done, up to the item's own class
         bool done = true;
         while (K > K0) {
@@ -1458,11 +1684,17 @@ template <bool EW> __global__ void __launch_bounds__(kRateThreads, 1) sweep_hub_
         }
       }
       if (tid == 0) {
-        hb.part_best[hb.sel_begin[entry] + c0] = best;
-        hb.part_fav[hb.sel_begin[entry] + c0] = fav;
+        hb.part_best[s_head[b].res + c0] = best;
+        hb.part_fav[s_head[b].res + c0] = fav;
+        phase_add(4, 0, true);
       }
     }
-    __syncthreads(); // s_item consumed
+    if (next) { // an item with nothing to do
+      rate_load_head_timed(a, hb, &s_head[b ^ 1]);
+    }
+    if (tid == 0) {
+      t_ph = phase_clock();
+    }
   }
 }
 
