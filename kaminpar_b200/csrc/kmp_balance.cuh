@@ -406,11 +406,7 @@ int bal_refuse(kmp_lp_handle *h, BalKind kind) {
   if (h->cfg.schedule == KMP_SCHEDULE_SEQ_STRICT) {
     return fail(KMP_ERR_UNSUPPORTED, std::string(what) + " has no seq_strict schedule (DESIGN.md " + section + ")");
   }
-  if (h->world > 1 || h->comm != nullptr || h->stepping || h->step_mode >= 0) {
-    return fail(KMP_ERR_UNSUPPORTED,
-                std::string(what) + " runs on one GPU: sharded, NCCL and stepping handles are refused");
-  }
-  return KMP_OK;
+  return refuse_multi_gpu(h, what);
 }
 
 // Scratch of both balancers, grow-only in the handle (kmp_lp_free_scratch releases it).

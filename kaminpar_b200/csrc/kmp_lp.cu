@@ -109,6 +109,15 @@ template <typename T> struct DevBuf {
 cudaMemPool_t kmp_private_pool(int device); // kmp_contract.cuh
 namespace {
 struct OverlayState; // kmp_overlay.cuh
+
+// What one LP run (a clustering or a refinement) passes to its sweeps and commits.
+struct RunCtx {
+  int mode;
+  uint32_t num_labels;
+  int32_t max_cluster_weight;
+  bool has_min;
+  bool has_comm;
+};
 } // namespace
 
 struct kmp_lp_handle {
@@ -253,12 +262,10 @@ struct kmp_lp_handle {
   // resident CTAs of each sweep_team instantiation on the device, [MODE][EW][P64][team size 32 / 128 / 512 / 1024]:
   // a larger grid only adds CTAs that start after the work queue is drained
   uint32_t team_grid[2][2][2][4] = {};
-  // stepping API state
-  int step_mode = -1;
-  uint32_t step_iter = 0; // LP round of the stepping API
-  uint32_t step_labels = 0;
-  int32_t step_mcw = 0;
-  bool step_has_min = false, step_has_comm = false;
+  // stepping API state: the open run (between kmp_lp_step_begin_* and kmp_lp_step_finish) and its LP round
+  RunCtx step{};
+  bool step_open = false;
+  uint32_t step_iter = 0;
   uint32_t mover_parity = 0; // proposal counter in use: ctr32[0] (parity 0) or ctr32[3] (parity 1)
   bool stepping = false; // proposals are accumulated by kmp_lp_step_commit, not by the sweep kernels
   // overload and underload balancers (kmp_balance.cuh, kmp_underload.cuh): one call counter each, so that LP calls
@@ -1130,14 +1137,6 @@ int ensure_scratch(kmp_lp_handle *h, int mode, uint32_t num_labels) {
   return KMP_OK;
 }
 
-struct RunCtx {
-  int mode;
-  uint32_t num_labels;
-  int32_t max_cluster_weight;
-  bool has_min;
-  bool has_comm;
-};
-
 SweepArgs make_sweep_args(kmp_lp_handle *h, const RunCtx &rc) {
   SweepArgs a{};
   a.xadj = h->xadj;
@@ -1427,9 +1426,15 @@ int begin_iteration(kmp_lp_handle *h, uint32_t iter) {
   return KMP_OK;
 }
 
-void end_iteration(kmp_lp_handle *h, uint32_t moved) {
+// The accepted moves of the round into *moved (one host wait), and into the history choose_activation reads.
+int end_iteration(kmp_lp_handle *h, uint32_t *moved) {
+  uint32_t host[2] = {0, 0};
+  KMP_CUDA(cudaMemcpyAsync(host, h->ctr32.p, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+  KMP_CUDA(cudaStreamSynchronize(h->stream));
+  *moved = host[1];
   h->moved_hist[1] = h->moved_hist[0];
-  h->moved_hist[0] = moved;
+  h->moved_hist[0] = host[1];
+  return KMP_OK;
 }
 
 // ---- NCCL, loaded on demand ----------------------------------------------------------------------------
@@ -1592,7 +1597,7 @@ int run_low_group(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, int group) 
 }
 
 // One LP round over all (group, sub-round) lists. Returns via *moved the accepted moves.
-int run_iteration(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t *moved, uint32_t *proposals) {
+int run_iteration(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t *moved) {
   const uint32_t S = h->lists_S;
   int rc0 = begin_iteration(h, iter);
   if (rc0 != KMP_OK) {
@@ -1642,13 +1647,7 @@ int run_iteration(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t *m
       return rc2;
     }
   }
-  uint32_t host[2] = {0, 0};
-  KMP_CUDA(cudaMemcpyAsync(host, h->ctr32.p, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
-  KMP_CUDA(cudaStreamSynchronize(h->stream));
-  *moved = host[1];
-  end_iteration(h, host[1]);
-  (void)proposals;
-  return KMP_OK;
+  return end_iteration(h, moved);
 }
 
 // packed gather array: word width by the label range; (re)allocated grow-only
@@ -1718,6 +1717,15 @@ int refuse_without_labels(const kmp_lp_handle *h) {
   if (!h->labels_valid) {
     return fail(KMP_ERR_INVALID, "no labels of the current graph on the device: cluster, pass a partition or call "
                                  "kmp_lp_upload_partition first");
+  }
+  return KMP_OK;
+}
+
+// The calls that run on one GPU only (the balancers, the overlay) refuse sharded, NCCL and open stepping handles.
+int refuse_multi_gpu(const kmp_lp_handle *h, const char *what) {
+  if (h->world > 1 || h->comm != nullptr || h->step_open) {
+    return fail(KMP_ERR_UNSUPPORTED,
+                std::string(what) + " runs on one GPU: sharded, NCCL and stepping handles are refused");
   }
   return KMP_OK;
 }
@@ -1864,6 +1872,117 @@ int cluster_post_passes(kmp_lp_handle *h, int32_t max_w, uint32_t num_clusters, 
   return KMP_OK;
 }
 
+// ---- one LP run of the sync schedule: set-up and finish of kmp_lp_cluster / kmp_lp_refine and the stepping API ----
+// Clustering set-up: every vertex its own cluster. *ctx is written only when the set-up succeeds.
+int begin_cluster_run(kmp_lp_handle *h, int32_t max_cluster_weight, const uint32_t *communities, RunCtx *ctx) {
+  if (h->cfg.sync_commit_passes > 1) { // the cluster commit kernels decide in one pass: no departure credit
+    return fail(KMP_ERR_UNSUPPORTED, "the clusterer's sync commit is single-pass (sync_commit_passes must be 1)");
+  }
+  const uint32_t n = h->n;
+  int rc = ensure_lists(h);
+  if (rc != KMP_OK) {
+    return rc;
+  }
+  KMP_CUDA(h->label.ensure(n));
+  KMP_CUDA(h->favored.ensure(n));
+  KMP_CUDA(h->weight.ensure(n));
+  rc = ensure_scratch(h, 0, n);
+  if (rc == KMP_OK) {
+    rc = prepare_labg(h, n);
+  }
+  if (rc == KMP_OK) {
+    rc = upload_optional_u32(h, h->communities, communities, n);
+  }
+  if (rc != KMP_OK) {
+    return rc;
+  }
+  KMP_CUDA(cudaMemsetAsync(h->ctr64.p, 0, kCtrSize * sizeof(unsigned long long), h->stream));
+  if (n > 0) {
+    launch_init_cluster(h);
+    ++h->kernel_launches;
+  }
+  *ctx = RunCtx{0, n, max_cluster_weight, false, communities != nullptr};
+  return KMP_OK;
+}
+
+// Refinement set-up: the partition (uploaded when non-null, else the device labels), all vertices active. *ctx is
+// written only when the set-up succeeds.
+int begin_refine_run(kmp_lp_handle *h, uint32_t k, const int32_t *max_block_weights, const int32_t *min_block_weights,
+                     const uint32_t *communities, const uint32_t *partition, RunCtx *ctx) {
+  const uint32_t n = h->n;
+  int rc = ensure_lists(h);
+  if (rc == KMP_OK) {
+    rc = ensure_scratch(h, 1, k);
+  }
+  if (rc == KMP_OK) {
+    rc = prepare_labg(h, k);
+  }
+  if (rc == KMP_OK) {
+    rc = load_partition(h, k, partition, max_block_weights, min_block_weights);
+  }
+  if (rc == KMP_OK) {
+    rc = upload_optional_u32(h, h->communities, communities, n);
+  }
+  if (rc != KMP_OK) {
+    return rc;
+  }
+  KMP_CUDA(cudaMemsetAsync(h->ctr64.p, 0, kCtrSize * sizeof(unsigned long long), h->stream));
+  if (n > 0) {
+    k_fill_u8<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->active.p, 1); // Base::initialize: all active
+    launch_pack_labels(h); // reads the labels without indexing by them
+    h->kernel_launches += 2;
+  }
+  rc = checked_block_weights(h, k, h->ctr64.p + kCtrScratch); // last: its wait covers the set-up above
+  if (rc != KMP_OK) {
+    return rc;
+  }
+  *ctx = RunCtx{1, k, 0, min_block_weights != nullptr, communities != nullptr};
+  return KMP_OK;
+}
+
+// The clusters (labels of nonzero weight) of a non-empty graph: two launches, which the caller counts, and a host wait.
+int count_clusters(kmp_lp_handle *h, uint32_t *num_clusters) {
+  reset_u32<<<1, 1, 0, h->stream>>>(h->ctr32.p + 2);
+  k_count_nonzero<<<grid_for(h->n, 256), 256, 0, h->stream>>>(h->n, h->weight.p, h->ctr32.p + 2);
+  KMP_CUDA(cudaMemcpyAsync(num_clusters, h->ctr32.p + 2, 4, cudaMemcpyDeviceToHost, h->stream));
+  KMP_CUDA(cudaStreamSynchronize(h->stream));
+  return KMP_OK;
+}
+
+// Clustering finish: the cluster count and the post passes. Every completed clustering, of an empty graph too,
+// advances the call index of the sync hashes.
+int finish_cluster_run(kmp_lp_handle *h, int32_t max_cluster_weight, kmp_lp_stats *stats) {
+  if (h->n > 0) {
+    uint32_t num_clusters = 0;
+    int rc = count_clusters(h, &num_clusters);
+    if (rc != KMP_OK) {
+      return rc;
+    }
+    h->kernel_launches += 2;
+    if (stats != nullptr) {
+      stats->num_clusters = num_clusters;
+    }
+    rc = cluster_post_passes(h, max_cluster_weight, num_clusters, stats); // lp_clusterer.cc:107-108
+    if (rc != KMP_OK) {
+      return rc;
+    }
+  }
+  ++h->call_counter;
+  h->labels_valid = true;
+  return KMP_OK;
+}
+
+// n labels into labels_out and k block weights into block_weights_out, each when non-null.
+int download_results(kmp_lp_handle *h, uint32_t *labels_out, int32_t *block_weights_out, uint32_t k) {
+  if (labels_out != nullptr && h->n > 0) {
+    KMP_CUDA(cudaMemcpyAsync(labels_out, h->label.p, static_cast<size_t>(h->n) * 4, cudaMemcpyDeviceToHost, h->stream));
+  }
+  if (block_weights_out != nullptr) {
+    KMP_CUDA(cudaMemcpyAsync(block_weights_out, h->weight.p, static_cast<size_t>(k) * 4, cudaMemcpyDeviceToHost, h->stream));
+  }
+  return KMP_OK;
+}
+
 // ---- schedule KMP_SCHEDULE_SEQ_STRICT ----------------------------------------------------------------
 // mode 0: labels are (re)initialised by the engine; mode 1: h->label holds the partition. Results stay in
 // h->label / h->weight; iteration statistics go to *stats, the scan counters to the last tier slot of ctr64.
@@ -1960,8 +2079,6 @@ int run_strict(kmp_lp_handle *h, int mode, uint32_t num_keys, int32_t max_cluste
   return KMP_OK;
 }
 
-int end_call(kmp_lp_handle *h, kmp_lp_stats *stats);
-
 int strict_cluster(kmp_lp_handle *h, int32_t max_cluster_weight, uint32_t desired_num_clusters,
                    const uint32_t *communities, uint32_t *clustering_out, kmp_lp_stats *stats) {
   const uint32_t n = h->n;
@@ -1969,76 +2086,47 @@ int strict_cluster(kmp_lp_handle *h, int32_t max_cluster_weight, uint32_t desire
   KMP_CUDA(h->weight.ensure(std::max<uint32_t>(n, 1)));
   KMP_CUDA(h->ctr64.ensure(kCtrSize));
   KMP_CUDA(cudaMemsetAsync(h->ctr64.p, 0, kCtrSize * sizeof(unsigned long long), h->stream));
-  if (communities != nullptr) {
-    KMP_CUDA(h->communities.ensure(n));
-    KMP_CUDA(cudaMemcpyAsync(h->communities.p, communities, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, h->stream));
+  int rc = upload_optional_u32(h, h->communities, communities, n);
+  if (rc == KMP_OK) {
+    rc = run_strict(h, 0, n, max_cluster_weight, desired_num_clusters, 0, false, communities != nullptr, stats);
   }
-  int rc = run_strict(h, 0, n, max_cluster_weight, desired_num_clusters, 0, false, communities != nullptr, stats);
+  if (rc == KMP_OK) {
+    rc = download_results(h, clustering_out, nullptr, 0);
+  }
   if (rc != KMP_OK) {
     return rc;
   }
-  if (clustering_out != nullptr && n > 0) {
-    KMP_CUDA(cudaMemcpyAsync(clustering_out, h->label.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, h->stream));
-  }
   ++h->call_counter;
   h->labels_valid = true;
-  const kmp_lp_stats keep = stats != nullptr ? *stats : kmp_lp_stats{};
-  rc = end_call(h, stats);
-  if (stats != nullptr) { // end_call fills the timing / counter fields only
-    stats->iterations = keep.iterations;
-    std::memcpy(stats->moved, keep.moved, sizeof(keep.moved));
-    stats->num_clusters = keep.num_clusters;
-    stats->two_hop_ran = keep.two_hop_ran;
-  }
-  return rc;
+  return end_call(h, stats);
 }
 
 int strict_refine(kmp_lp_handle *h, uint32_t k, const int32_t *max_block_weights, const int32_t *min_block_weights,
                   const uint32_t *communities, uint32_t *partition_inout, int32_t *block_weights_out,
                   kmp_lp_stats *stats) {
   const uint32_t n = h->n;
+  // the engine's sizes, above the n labels and k weights load_partition ensures
   KMP_CUDA(h->label.ensure(std::max<uint32_t>(n, 1)));
   KMP_CUDA(h->weight.ensure(std::max<uint32_t>(std::max(n, k), 1)));
-  KMP_CUDA(h->maxw.ensure(k));
   KMP_CUDA(h->ctr64.ensure(kCtrSize));
   KMP_CUDA(cudaMemsetAsync(h->ctr64.p, 0, kCtrSize * sizeof(unsigned long long), h->stream));
-  if (partition_inout != nullptr && n > 0) {
-    KMP_CUDA(cudaMemcpyAsync(h->label.p, partition_inout, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, h->stream));
+  int rc = load_partition(h, k, partition_inout, max_block_weights, min_block_weights);
+  if (rc == KMP_OK) {
+    rc = upload_optional_u32(h, h->communities, communities, n);
   }
-  if (partition_inout != nullptr) {
-    h->labels_valid = true;
+  if (rc == KMP_OK) {
+    rc = checked_block_weights(h, k, h->ctr64.p + kCtrScratch); // the engine recomputes the weights itself
   }
-  KMP_CUDA(cudaMemsetAsync(h->weight.p, 0, static_cast<size_t>(k) * 4, h->stream));
-  int rc = checked_block_weights(h, k, h->ctr64.p + kCtrScratch); // the engine recomputes the weights itself
+  if (rc == KMP_OK) {
+    rc = run_strict(h, 1, k, 0, 0, k, min_block_weights != nullptr, communities != nullptr, stats);
+  }
+  if (rc == KMP_OK) {
+    rc = download_results(h, partition_inout, block_weights_out, k);
+  }
   if (rc != KMP_OK) {
     return rc;
   }
-  KMP_CUDA(cudaMemcpyAsync(h->maxw.p, max_block_weights, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, h->stream));
-  if (min_block_weights != nullptr) {
-    KMP_CUDA(h->minw.ensure(k));
-    KMP_CUDA(cudaMemcpyAsync(h->minw.p, min_block_weights, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, h->stream));
-  }
-  if (communities != nullptr) {
-    KMP_CUDA(h->communities.ensure(n));
-    KMP_CUDA(cudaMemcpyAsync(h->communities.p, communities, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, h->stream));
-  }
-  rc = run_strict(h, 1, k, 0, 0, k, min_block_weights != nullptr, communities != nullptr, stats);
-  if (rc != KMP_OK) {
-    return rc;
-  }
-  if (partition_inout != nullptr && n > 0) {
-    KMP_CUDA(cudaMemcpyAsync(partition_inout, h->label.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, h->stream));
-  }
-  if (block_weights_out != nullptr) {
-    KMP_CUDA(cudaMemcpyAsync(block_weights_out, h->weight.p, static_cast<size_t>(k) * 4, cudaMemcpyDeviceToHost, h->stream));
-  }
-  const kmp_lp_stats keep = stats != nullptr ? *stats : kmp_lp_stats{};
-  rc = end_call(h, stats);
-  if (stats != nullptr) {
-    stats->iterations = keep.iterations;
-    std::memcpy(stats->moved, keep.moved, sizeof(keep.moved));
-  }
-  return rc;
+  return end_call(h, stats);
 }
 
 } // namespace
@@ -2354,43 +2442,19 @@ int kmp_lp_cluster(kmp_lp_handle *h, int32_t max_cluster_weight, uint32_t desire
   if (h->cfg.schedule == KMP_SCHEDULE_SEQ_STRICT) {
     return strict_cluster(h, max_cluster_weight, desired_num_clusters, communities, clustering_out, stats);
   }
-  if (h->cfg.sync_commit_passes > 1) { // the cluster commit kernels decide in one pass: no departure credit
-    return fail(KMP_ERR_UNSUPPORTED, "the clusterer's sync commit is single-pass (sync_commit_passes must be 1)");
-  }
   if (h->world > 1 && h->comm == nullptr) {
     return fail(KMP_ERR_INVALID, "sharded handle without a communicator: call kmp_lp_dist_init (or drive the "
                                  "stepping API yourself)");
   }
   const uint32_t n = h->n;
-  rc = ensure_lists(h);
+  RunCtx ctx;
+  rc = begin_cluster_run(h, max_cluster_weight, communities, &ctx);
   if (rc != KMP_OK) {
     return rc;
   }
-  KMP_CUDA(h->label.ensure(n));
-  KMP_CUDA(h->favored.ensure(n));
-  KMP_CUDA(h->weight.ensure(n));
-  rc = ensure_scratch(h, 0, n);
-  if (rc != KMP_OK) {
-    return rc;
-  }
-  rc = prepare_labg(h, n);
-  if (rc != KMP_OK) {
-    return rc;
-  }
-  rc = upload_optional_u32(h, h->communities, communities, n);
-  if (rc != KMP_OK) {
-    return rc;
-  }
-  KMP_CUDA(cudaMemsetAsync(h->ctr64.p, 0, kCtrSize * sizeof(unsigned long long), h->stream));
-  if (n > 0) {
-    launch_init_cluster(h);
-    ++h->kernel_launches;
-  }
-  RunCtx ctx{0, n, max_cluster_weight, false, communities != nullptr};
-  uint32_t num_clusters = n;
   for (uint32_t it = 0; it < h->cfg.num_iterations && n > 0; ++it) { // lp_clusterer.cc:94-105
     uint32_t moved = 0;
-    rc = run_iteration(h, ctx, it, &moved, nullptr);
+    rc = run_iteration(h, ctx, it, &moved);
     if (rc != KMP_OK) {
       return rc;
     }
@@ -2402,40 +2466,29 @@ int kmp_lp_cluster(kmp_lp_handle *h, int32_t max_cluster_weight, uint32_t desire
       break;
     }
     if (desired_num_clusters > 0) { // should_stop(), label_propagation.h:260-265
-      reset_u32<<<1, 1, 0, h->stream>>>(h->ctr32.p + 2);
-      k_count_nonzero<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->weight.p, h->ctr32.p + 2);
-      KMP_CUDA(cudaMemcpyAsync(&num_clusters, h->ctr32.p + 2, 4, cudaMemcpyDeviceToHost, h->stream));
-      KMP_CUDA(cudaStreamSynchronize(h->stream));
+      uint32_t num_clusters = 0;
+      rc = count_clusters(h, &num_clusters);
+      if (rc != KMP_OK) {
+        return rc;
+      }
       if (num_clusters <= desired_num_clusters) {
         break;
       }
     }
   }
-  if (n > 0) {
-    reset_u32<<<1, 1, 0, h->stream>>>(h->ctr32.p + 2);
-    k_count_nonzero<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->weight.p, h->ctr32.p + 2);
-    KMP_CUDA(cudaMemcpyAsync(&num_clusters, h->ctr32.p + 2, 4, cudaMemcpyDeviceToHost, h->stream));
-    KMP_CUDA(cudaStreamSynchronize(h->stream));
-    h->kernel_launches += 2;
-    if (stats != nullptr) {
-      stats->num_clusters = num_clusters;
-    }
-    if (h->world > 1) { // favored[u] is only written by the rank that swept u: MAX over (favored ^ u), 0 elsewhere
-      KMP_CUDA(h->dist_recv.ensure(n));
-      k_xor_iota<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->favored.p, h->dist_recv.p);
-      KMP_NCCL(g_nccl.AllReduce(h->dist_recv.p, h->dist_recv.p, n, ncclUint32, ncclMax, h->comm, h->stream));
-      k_xor_iota<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->dist_recv.p, h->favored.p);
-    }
-    rc = cluster_post_passes(h, max_cluster_weight, num_clusters, stats); // lp_clusterer.cc:107-108
-    if (rc != KMP_OK) {
-      return rc;
-    }
+  if (h->world > 1 && n > 0) { // favored[u] is only written by the rank that swept u: MAX over (favored ^ u), 0 elsewhere
+    KMP_CUDA(h->dist_recv.ensure(n));
+    k_xor_iota<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->favored.p, h->dist_recv.p);
+    KMP_NCCL(g_nccl.AllReduce(h->dist_recv.p, h->dist_recv.p, n, ncclUint32, ncclMax, h->comm, h->stream));
+    k_xor_iota<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->dist_recv.p, h->favored.p);
   }
-  if (clustering_out != nullptr && n > 0) {
-    KMP_CUDA(cudaMemcpyAsync(clustering_out, h->label.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, h->stream));
+  rc = finish_cluster_run(h, max_cluster_weight, stats);
+  if (rc == KMP_OK) {
+    rc = download_results(h, clustering_out, nullptr, 0);
   }
-  ++h->call_counter;
-  h->labels_valid = true;
+  if (rc != KMP_OK) {
+    return rc;
+  }
   return end_call(h, stats);
 }
 
@@ -2484,38 +2537,15 @@ int kmp_lp_refine(kmp_lp_handle *h, uint32_t k, const int32_t *max_block_weights
                                  "stepping API yourself)");
   }
   const uint32_t n = h->n;
-  rc = ensure_lists(h);
+  RunCtx ctx;
+  rc = begin_refine_run(h, k, max_block_weights, min_block_weights, communities, partition_inout, &ctx);
   if (rc != KMP_OK) {
     return rc;
   }
-  rc = ensure_scratch(h, 1, k);
-  if (rc == KMP_OK) {
-    rc = prepare_labg(h, k);
-  }
-  if (rc == KMP_OK) {
-    rc = load_partition(h, k, partition_inout, max_block_weights, min_block_weights);
-  }
-  if (rc == KMP_OK) {
-    rc = upload_optional_u32(h, h->communities, communities, n);
-  }
-  if (rc != KMP_OK) {
-    return rc;
-  }
-  KMP_CUDA(cudaMemsetAsync(h->ctr64.p, 0, kCtrSize * sizeof(unsigned long long), h->stream));
-  if (n > 0) {
-    k_fill_u8<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->active.p, 1); // Base::initialize: all active
-    launch_pack_labels(h); // reads the labels without indexing by them
-    h->kernel_launches += 2;
-  }
-  rc = checked_block_weights(h, k, h->ctr64.p + kCtrScratch); // last: its wait covers the set-up above
-  if (rc != KMP_OK) {
-    return rc;
-  }
-  RunCtx ctx{1, k, 0, min_block_weights != nullptr, communities != nullptr};
   const uint64_t max_it = h->cfg.num_iterations == 0 ? ~0ull : h->cfg.num_iterations; // lp_refiner.cc:78-79
   for (uint64_t it = 0; it < max_it && n > 0; ++it) {
     uint32_t moved = 0;
-    rc = run_iteration(h, ctx, static_cast<uint32_t>(it), &moved, nullptr);
+    rc = run_iteration(h, ctx, static_cast<uint32_t>(it), &moved);
     if (rc != KMP_OK) {
       return rc;
     }
@@ -2527,11 +2557,9 @@ int kmp_lp_refine(kmp_lp_handle *h, uint32_t k, const int32_t *max_block_weights
       break;
     }
   }
-  if (partition_inout != nullptr && n > 0) {
-    KMP_CUDA(cudaMemcpyAsync(partition_inout, h->label.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, h->stream));
-  }
-  if (block_weights_out != nullptr) {
-    KMP_CUDA(cudaMemcpyAsync(block_weights_out, h->weight.p, static_cast<size_t>(k) * 4, cudaMemcpyDeviceToHost, h->stream));
+  rc = download_results(h, partition_inout, block_weights_out, k);
+  if (rc != KMP_OK) {
+    return rc;
   }
   return end_call(h, stats);
 }
@@ -2819,39 +2847,12 @@ int kmp_lp_step_begin_cluster(kmp_lp_handle *h, int32_t max_cluster_weight, cons
   if (h->cfg.schedule != KMP_SCHEDULE_SYNC) {
     return fail(KMP_ERR_UNSUPPORTED, "the stepping API drives the sync schedule");
   }
-  if (h->cfg.sync_commit_passes > 1) { // as kmp_lp_cluster: the cluster commit kernels decide in one pass
-    return fail(KMP_ERR_UNSUPPORTED, "the clusterer's sync commit is single-pass (sync_commit_passes must be 1)");
-  }
-  const uint32_t n = h->n;
-  rc = ensure_lists(h);
+  rc = begin_cluster_run(h, max_cluster_weight, communities, &h->step);
   if (rc != KMP_OK) {
     return rc;
   }
-  KMP_CUDA(h->label.ensure(n));
-  KMP_CUDA(h->favored.ensure(n));
-  KMP_CUDA(h->weight.ensure(n));
-  rc = ensure_scratch(h, 0, n);
-  if (rc != KMP_OK) {
-    return rc;
-  }
-  rc = upload_optional_u32(h, h->communities, communities, n);
-  if (rc != KMP_OK) {
-    return rc;
-  }
-  rc = prepare_labg(h, n);
-  if (rc != KMP_OK) {
-    return rc;
-  }
-  KMP_CUDA(cudaMemsetAsync(h->ctr64.p, 0, kCtrSize * sizeof(unsigned long long), h->stream));
-  if (n > 0) {
-    launch_init_cluster(h);
-  }
+  h->step_open = true;
   h->step_iter = 0;
-  h->step_mode = 0;
-  h->step_labels = n;
-  h->step_mcw = max_cluster_weight;
-  h->step_has_min = false;
-  h->step_has_comm = communities != nullptr;
   return KMP_OK;
 }
 
@@ -2867,45 +2868,17 @@ int kmp_lp_step_begin_refine(kmp_lp_handle *h, uint32_t k, const int32_t *max_bl
   if (h->cfg.schedule != KMP_SCHEDULE_SYNC) {
     return fail(KMP_ERR_UNSUPPORTED, "the stepping API drives the sync schedule");
   }
-  const uint32_t n = h->n;
-  rc = ensure_lists(h);
+  rc = begin_refine_run(h, k, max_block_weights, min_block_weights, communities, partition, &h->step);
   if (rc != KMP_OK) {
     return rc;
   }
-  rc = ensure_scratch(h, 1, k);
-  if (rc == KMP_OK) {
-    rc = load_partition(h, k, partition, max_block_weights, min_block_weights);
-  }
-  if (rc == KMP_OK) {
-    rc = upload_optional_u32(h, h->communities, communities, n);
-  }
-  if (rc != KMP_OK) {
-    return rc;
-  }
-  KMP_CUDA(cudaMemsetAsync(h->ctr64.p, 0, kCtrSize * sizeof(unsigned long long), h->stream));
-  rc = prepare_labg(h, k);
-  if (rc != KMP_OK) {
-    return rc;
-  }
-  rc = checked_block_weights(h, k, h->ctr64.p + kCtrScratch);
-  if (rc != KMP_OK) {
-    return rc;
-  }
-  if (n > 0) {
-    k_fill_u8<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->active.p, 1);
-    launch_pack_labels(h);
-  }
+  h->step_open = true;
   h->step_iter = 0;
-  h->step_mode = 1;
-  h->step_labels = k;
-  h->step_mcw = 0;
-  h->step_has_min = min_block_weights != nullptr;
-  h->step_has_comm = communities != nullptr;
   return KMP_OK;
 }
 
 int kmp_lp_step_begin_iteration(kmp_lp_handle *h) {
-  if (h == nullptr || h->step_mode < 0) {
+  if (h == nullptr || !h->step_open) {
     return fail(KMP_ERR_INVALID, "step_begin_* not called");
   }
   return begin_iteration(h, h->step_iter);
@@ -2914,37 +2887,34 @@ int kmp_lp_step_begin_iteration(kmp_lp_handle *h) {
 // Sweep this rank's share of sub-round sg and pack its proposals into d_send (device memory,
 // 4 + 2 * cap words: [count, -, -, -, u[cap], t[cap]]).
 int kmp_lp_step_sweep(kmp_lp_handle *h, uint32_t iter, uint32_t sg, void *d_send) {
-  if (h == nullptr || h->step_mode < 0 || d_send == nullptr) {
+  if (h == nullptr || !h->step_open || d_send == nullptr) {
     return fail(KMP_ERR_INVALID, "bad argument");
   }
   if (sg >= kNumGroups * h->lists_S) { // subround_of_sg indexes list_off by sg
     return fail(KMP_ERR_INVALID, "bad sub-round");
   }
-  const RunCtx rc{h->step_mode, h->step_labels, h->step_mcw, h->step_has_min, h->step_has_comm};
-  return dist_sweep_pack(h, rc, iter, sg, subround_of_sg(h, sg), static_cast<uint32_t *>(d_send));
+  return dist_sweep_pack(h, h->step, iter, sg, subround_of_sg(h, sg), static_cast<uint32_t *>(d_send));
 }
 
 // Commit sub-round sg from the all-gathered proposal buffers (world * (4 + 2 * cap) words).
 int kmp_lp_step_commit(kmp_lp_handle *h, uint32_t iter, uint32_t sg, const void *d_gathered) {
-  if (h == nullptr || h->step_mode < 0 || d_gathered == nullptr) {
+  if (h == nullptr || !h->step_open || d_gathered == nullptr) {
     return fail(KMP_ERR_INVALID, "bad argument");
   }
   if (sg >= kNumGroups * h->lists_S) {
     return fail(KMP_ERR_INVALID, "bad sub-round");
   }
-  const RunCtx rc{h->step_mode, h->step_labels, h->step_mcw, h->step_has_min, h->step_has_comm};
-  return commit_subround(h, rc, iter, sg, subround_of_sg(h, sg), static_cast<const uint32_t *>(d_gathered));
+  return commit_subround(h, h->step, iter, sg, subround_of_sg(h, sg), static_cast<const uint32_t *>(d_gathered));
 }
 
 int kmp_lp_step_end_iteration(kmp_lp_handle *h, uint32_t *moved) {
-  if (h == nullptr || h->step_mode < 0 || moved == nullptr) {
+  if (h == nullptr || !h->step_open || moved == nullptr) {
     return fail(KMP_ERR_INVALID, "bad argument");
   }
-  uint32_t host[2] = {0, 0};
-  KMP_CUDA(cudaMemcpyAsync(host, h->ctr32.p, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
-  KMP_CUDA(cudaStreamSynchronize(h->stream));
-  *moved = host[1];
-  end_iteration(h, host[1]);
+  const int rc = end_iteration(h, moved);
+  if (rc != KMP_OK) {
+    return rc;
+  }
   ++h->step_iter;
   return KMP_OK;
 }
@@ -2952,7 +2922,7 @@ int kmp_lp_step_end_iteration(kmp_lp_handle *h, uint32_t *moved) {
 // favored[u] ^ u into / out of a caller-provided device buffer of n words (for a MAX all-reduce:
 // only the rank that owns u ever writes favored[u]; everybody else still holds u, i.e. 0 here).
 int kmp_lp_step_favored_export(kmp_lp_handle *h, void *d_buf) {
-  if (h == nullptr || d_buf == nullptr || h->step_mode != 0) {
+  if (h == nullptr || d_buf == nullptr || !h->step_open || h->step.mode != 0) {
     return fail(KMP_ERR_INVALID, "bad argument");
   }
   k_xor_iota<<<grid_for(h->n, 256), 256, 0, h->stream>>>(h->n, h->favored.p, static_cast<uint32_t *>(d_buf));
@@ -2960,7 +2930,7 @@ int kmp_lp_step_favored_export(kmp_lp_handle *h, void *d_buf) {
   return KMP_OK;
 }
 int kmp_lp_step_favored_import(kmp_lp_handle *h, const void *d_buf) {
-  if (h == nullptr || d_buf == nullptr || h->step_mode != 0) {
+  if (h == nullptr || d_buf == nullptr || !h->step_open || h->step.mode != 0) {
     return fail(KMP_ERR_INVALID, "bad argument");
   }
   k_xor_iota<<<grid_for(h->n, 256), 256, 0, h->stream>>>(h->n, static_cast<const uint32_t *>(d_buf), h->favored.p);
@@ -2970,37 +2940,21 @@ int kmp_lp_step_favored_import(kmp_lp_handle *h, const void *d_buf) {
 
 // Post passes (clusterer) and result download; stats hold THIS rank's share of the scan counters.
 int kmp_lp_step_finish(kmp_lp_handle *h, uint32_t *labels_out, int32_t *block_weights_out, kmp_lp_stats *stats) {
-  if (h == nullptr || h->step_mode < 0) {
+  if (h == nullptr || !h->step_open) {
     return fail(KMP_ERR_INVALID, "step_begin_* not called");
   }
-  const uint32_t n = h->n;
   if (stats != nullptr) {
     std::memset(stats, 0, sizeof(*stats));
   }
-  if (h->step_mode == 0 && n > 0) {
-    uint32_t num_clusters = 0;
-    reset_u32<<<1, 1, 0, h->stream>>>(h->ctr32.p + 2);
-    k_count_nonzero<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->weight.p, h->ctr32.p + 2);
-    KMP_CUDA(cudaMemcpyAsync(&num_clusters, h->ctr32.p + 2, 4, cudaMemcpyDeviceToHost, h->stream));
-    KMP_CUDA(cudaStreamSynchronize(h->stream));
-    if (stats != nullptr) {
-      stats->num_clusters = num_clusters;
-    }
-    int rc = cluster_post_passes(h, h->step_mcw, num_clusters, stats);
-    if (rc != KMP_OK) {
-      return rc;
-    }
-    ++h->call_counter;
-    h->labels_valid = true;
+  const bool cluster = h->step.mode == 0;
+  int rc = cluster ? finish_cluster_run(h, h->step.max_cluster_weight, stats) : KMP_OK;
+  if (rc == KMP_OK) {
+    rc = download_results(h, labels_out, cluster ? nullptr : block_weights_out, h->step.num_labels);
   }
-  if (labels_out != nullptr && n > 0) {
-    KMP_CUDA(cudaMemcpyAsync(labels_out, h->label.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, h->stream));
+  if (rc != KMP_OK) {
+    return rc;
   }
-  if (block_weights_out != nullptr && h->step_mode == 1) {
-    KMP_CUDA(cudaMemcpyAsync(block_weights_out, h->weight.p, static_cast<size_t>(h->step_labels) * 4,
-                             cudaMemcpyDeviceToHost, h->stream));
-  }
-  h->step_mode = -1;
+  h->step_open = false;
   return end_call(h, stats);
 }
 

@@ -217,10 +217,7 @@ int overlay_checks(kmp_lp_handle *h) {
   if (!h->have_graph) {
     return fail(KMP_ERR_INVALID, "no graph set");
   }
-  if (h->world > 1 || h->comm != nullptr || h->stepping || h->step_mode >= 0) {
-    return fail(KMP_ERR_UNSUPPORTED, "the overlay runs on one GPU: sharded, NCCL and stepping handles are refused");
-  }
-  return KMP_OK;
+  return refuse_multi_gpu(h, "the overlay");
 }
 
 // reduce the stash's first `count` clusterings into the handle's labels; timing and stats

@@ -382,6 +382,29 @@ def test_sharded_handles_cluster_twice_then_refine(world):
         sh.close()
 
 
+def test_sharded_clustering_of_an_empty_graph_counts_as_a_call():
+    """A stepping clustering of an empty graph is a completed clustering, as in kmp_lp_cluster: the next one, on
+    the same handles and another graph, hashes with call index 1 (DESIGN.md, "parity across levels and calls")."""
+    name, seed, world = "rmat16_hubs", 6, 3
+    g = graph(name)
+    case = Case(name, 0, seed)
+    mcw, _ = inputs(case)
+    want, st = B.oracle_lp_cluster(g, seed, mcw, schedule=B.SYNC, params=oracle_params(case), return_stats=True,
+                                   call_index=1)
+    sh = Shards(H.empty_graph(0), config(case), world, "rotated")
+    try:
+        for b in sh.ranks:  # no vertices: no sub-round to sweep and no favored entry to exchange
+            b.begin_cluster(mcw, None)
+        res = sh.finish(sh.rounds())
+        assert all(len(labels) == 0 for labels in res.labels)
+        for h in sh.handles:
+            h.set_graph(g)
+        sh.n = g.n
+        check(sh.cluster(mcw), (want, None, st[0]), world, 1)
+    finally:
+        sh.close()
+
+
 # ------------------------------------------------------------------------------------------------
 # Knobs at world 3 (each read once, when a handle is created)
 # ------------------------------------------------------------------------------------------------
