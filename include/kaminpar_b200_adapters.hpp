@@ -19,6 +19,8 @@
 //                      kaminpar-shm/coarsening/sparsification_cluster_coarsener.cc:41-228 (DESIGN.md §13)
 //   LPClustering::compute_overlay_clustering
 //                      kaminpar-shm/coarsening/overlay_cluster_coarsener.cc:34-151 (DESIGN.md §14)
+//   PreparedGraph / rearrange_by_degree_buckets / assign_isolated_nodes
+//                      kaminpar-shm/graphutils/permutator.cc:66-91, 236-264, kaminpar.cc:368-445 (DESIGN.md §15)
 //
 // Error convention: the reference's path has no error codes (KASSERT aborts); here a non-zero
 // status of the C ABI becomes std::runtime_error. There is no CPU fallback.
@@ -34,6 +36,7 @@
 #include "kaminpar_b200_balancer.h"
 #include "kaminpar_b200_contraction.h"
 #include "kaminpar_b200_lp.h"
+#include "kaminpar_b200_prepare.h"
 
 namespace kaminpar_b200 {
 
@@ -441,6 +444,66 @@ inline std::unique_ptr<CoarseGraph> contract_clustering(kmp_lp_handle *graph_hol
   kmp_contraction_stats stats{};
   detail::check(kmp_contract_clustering(graph_holder, clustering.empty() ? nullptr : clustering.data(), &g, &stats));
   return std::make_unique<CoarseGraph>(g, stats);
+}
+
+// The caller's graph rearranged by degree bucket on the device, its isolated vertices cut off the end
+// (graph::rearrange_by_degree_buckets + CSRGraph::remove_isolated_nodes, kaminpar.cc:368-402). set_on() hands the
+// n() non-isolated vertices to a handle (sorted); assign_isolated_nodes() below brings the isolated ones back.
+// Owns device memory of the preparing handle's pool: destroy it before that handle.
+class PreparedGraph {
+public:
+  explicit PreparedGraph(kmp_prepared_graph *g, const kmp_prepare_stats &stats) : _g(g), _stats(stats) {}
+  PreparedGraph(const PreparedGraph &) = delete;
+  PreparedGraph &operator=(const PreparedGraph &) = delete;
+  ~PreparedGraph() { kmp_prepared_destroy(_g); }
+
+  [[nodiscard]] NodeID n() const { return kmp_prepared_n(_g); } // n': the vertices the LP sees
+  [[nodiscard]] NodeID num_isolated() const { return kmp_prepared_num_isolated(_g); }
+  [[nodiscard]] EdgeID m() const { return kmp_prepared_m(_g); }
+  // kmp_lp_set_graph_prepared: the handle's graph becomes the n() prepared vertices, marked sorted
+  void set_on(kmp_lp_handle *h) const { detail::check(kmp_lp_set_graph_prepared(h, _g)); }
+  // original id -> prepared id (CSRGraph::map_original_node), all n() + num_isolated() vertices
+  [[nodiscard]] std::vector<NodeID> old_to_new() const {
+    std::vector<NodeID> o2n(static_cast<std::size_t>(n()) + num_isolated());
+    detail::check(kmp_prepared_download(_g, nullptr, nullptr, nullptr, nullptr, o2n.data()));
+    return o2n;
+  }
+  [[nodiscard]] const kmp_prepare_stats &stats() const { return _stats; }
+  [[nodiscard]] const kmp_prepared_graph *device() const { return _g; } // kmp_prepared_device_arrays
+
+private:
+  kmp_prepared_graph *_g;
+  kmp_prepare_stats _stats;
+};
+
+// graph::rearrange_by_degree_buckets(graph) (permutator.cc:66-91) + the isolated-vertex cut, on the device, stream
+// and pool of `h`. Set the PartitionContext up on `graph` before this, as compute_partition does (kaminpar.cc:316):
+// its max block weights count the isolated vertices.
+inline std::unique_ptr<PreparedGraph> rearrange_by_degree_buckets(kmp_lp_handle *h, const CSRGraphView &graph) {
+  kmp_prepared_graph *g = nullptr;
+  kmp_prepare_stats stats{};
+  detail::check(kmp_prepare_graph(h, graph.n(), graph.m(), graph.nodes.data(), graph.edges.data(),
+                                  graph.node_weights.empty() ? nullptr : graph.node_weights.data(),
+                                  graph.edge_weights.empty() ? nullptr : graph.edge_weights.data(), &g, &stats));
+  return std::make_unique<PreparedGraph>(g, stats);
+}
+
+// graph::assign_isolated_nodes(p_graph, num_isolated_nodes, p_ctx) (permutator.cc:236-264) and the map back to the
+// caller's ids (kaminpar.cc:434-440): p_graph partitions the prepared graph's n() vertices (an empty partition span
+// takes the labels `h` holds on the device for `graph`); its block_weights (k entries, or empty) receive the weights
+// including the isolated vertices; partition_out gets one block per original vertex, in the caller's ids.
+inline void assign_isolated_nodes(kmp_lp_handle *h, const PreparedGraph &graph, const PartitionedGraphView &p_graph,
+                                  NodeID num_isolated_nodes, const PartitionContextView &p_ctx,
+                                  std::span<BlockID> partition_out) {
+  if (num_isolated_nodes != graph.num_isolated() || partition_out.size() != graph.n() + graph.num_isolated() ||
+      (!p_graph.partition.empty() && p_graph.partition.size() != graph.n()) ||
+      p_ctx.max_block_weights.size() < p_graph.k ||
+      (!p_graph.block_weights.empty() && p_graph.block_weights.size() != p_graph.k)) {
+    throw std::invalid_argument("assign_isolated_nodes: wrong span size or isolated vertex count");
+  }
+  detail::check(kmp_prepared_finish(h, graph.device(), p_graph.k, p_ctx.max_block_weights.data(),
+                                    p_graph.partition.empty() ? nullptr : p_graph.partition.data(), partition_out.data(),
+                                    p_graph.block_weights.empty() ? nullptr : p_graph.block_weights.data()));
 }
 
 } // namespace kaminpar_b200

@@ -26,6 +26,7 @@
 
 #include "../../include/kaminpar_b200_contraction.h"
 #include "../../include/kaminpar_b200_lp.h"
+#include "../../include/kaminpar_b200_prepare.h"
 #include "lp_commit.cuh"
 #include "lp_device.cuh"
 #include "lp_lowgroup.cuh"
@@ -2965,6 +2966,7 @@ int kmp_lp_step_finish(kmp_lp_handle *h, uint32_t *labels_out, int32_t *block_we
 #include "kmp_overlay.cuh"
 #include "kmp_balance.cuh"
 #include "kmp_underload.cuh"
+#include "kmp_prepare.cuh"
 
 #ifdef KMP_HUB_PHASE_STAMPS
 // scripts/hub_rate_phases.py: reads (and with reset != 0 zeroes) the rate kernel's 7 phase accumulators
