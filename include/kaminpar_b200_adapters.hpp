@@ -21,6 +21,8 @@
 //                      kaminpar-shm/coarsening/overlay_cluster_coarsener.cc:34-151 (DESIGN.md §14)
 //   PreparedGraph / rearrange_by_degree_buckets / assign_isolated_nodes
 //                      kaminpar-shm/graphutils/permutator.cc:66-91, 236-264, kaminpar.cc:368-445 (DESIGN.md §15)
+//   Subgraphs / extract_subgraphs / copy_subgraph_partitions
+//                      kaminpar-shm/graphutils/subgraph_extractor.cc:181-324, 492-533 (DESIGN.md §16)
 //
 // Error convention: the reference's path has no error codes (KASSERT aborts); here a non-zero
 // status of the C ABI becomes std::runtime_error. There is no CPU fallback.
@@ -37,6 +39,7 @@
 #include "kaminpar_b200_contraction.h"
 #include "kaminpar_b200_lp.h"
 #include "kaminpar_b200_prepare.h"
+#include "kaminpar_b200_subgraph.h"
 
 namespace kaminpar_b200 {
 
@@ -504,6 +507,100 @@ inline void assign_isolated_nodes(kmp_lp_handle *h, const PreparedGraph &graph, 
   detail::check(kmp_prepared_finish(h, graph.device(), p_graph.k, p_ctx.max_block_weights.data(),
                                     p_graph.partition.empty() ? nullptr : p_graph.partition.data(), partition_out.data(),
                                     p_graph.block_weights.empty() ? nullptr : p_graph.block_weights.data()));
+}
+
+// The k block-induced subgraphs of the graph `h` holds (graph::lazy_extract_subgraphs_preprocessing +
+// graph::extract_subgraph for every block, subgraph_extractor.cc:181-324), on the device in the reference's
+// SubgraphMemory shape: one xadj of n + k entries, block b's local xadj at node_offsets()[b] + b. get() copies them to
+// host vectors once; block_nodes() / mapping() are the preprocessing's arrays. Owns device memory of the extracting
+// handle's pool: destroy it before that handle.
+class Subgraphs {
+public:
+  struct HostBlocks {
+    std::vector<NodeID> node_offsets, edge_offsets; // k + 1 each
+    std::vector<EdgeID> nodes;                      // n + k
+    std::vector<NodeID> edges;
+    std::vector<NodeWeight> node_weights; // empty for unit weights
+    std::vector<EdgeWeight> edge_weights; // empty for unit weights
+    std::vector<NodeID> mapping, block_nodes;
+  };
+  explicit Subgraphs(kmp_subgraphs *g, const kmp_subgraph_stats &stats) : _g(g), _stats(stats) {}
+  Subgraphs(const Subgraphs &) = delete;
+  Subgraphs &operator=(const Subgraphs &) = delete;
+  ~Subgraphs() { kmp_subgraphs_destroy(_g); }
+
+  [[nodiscard]] BlockID k() const { return kmp_subgraphs_k(_g); }
+  [[nodiscard]] NodeID n() const { return kmp_subgraphs_n(_g); }
+  [[nodiscard]] EdgeID m() const { return kmp_subgraphs_m(_g); } // internal directed edges of all blocks
+  const HostBlocks &get() {
+    if (_host.nodes.empty()) {
+      const DeviceArrays d = device_arrays();
+      _host.node_offsets.resize(static_cast<std::size_t>(k()) + 1);
+      _host.edge_offsets.resize(static_cast<std::size_t>(k()) + 1);
+      detail::check(kmp_subgraphs_offsets(_g, _host.node_offsets.data(), _host.edge_offsets.data()));
+      _host.nodes.resize(static_cast<std::size_t>(n()) + k());
+      _host.edges.resize(m());
+      _host.node_weights.resize(d.node_weights != nullptr ? n() : 0);
+      _host.edge_weights.resize(d.edge_weights != nullptr ? m() : 0);
+      _host.mapping.resize(n());
+      _host.block_nodes.resize(n());
+      detail::check(kmp_subgraphs_download(_g, _host.nodes.data(), _host.edges.data(), _host.node_weights.data(),
+                                           _host.edge_weights.data(), _host.mapping.data(), _host.block_nodes.data()));
+    }
+    return _host;
+  }
+  // Block b of get() as a borrowed CSR view (valid while this object and its host copy live).
+  CSRGraphView block(BlockID b) {
+    const HostBlocks &h = get();
+    const NodeID n0 = h.node_offsets[b], n1 = h.node_offsets[b + 1];
+    const EdgeID e0 = h.edge_offsets[b], e1 = h.edge_offsets[b + 1];
+    return CSRGraphView{std::span<const EdgeID>(h.nodes.data() + n0 + b, n1 - n0 + 1),
+                        std::span<const NodeID>(h.edges.data() + e0, e1 - e0),
+                        h.node_weights.empty() ? std::span<const NodeWeight>()
+                                               : std::span<const NodeWeight>(h.node_weights.data() + n0, n1 - n0),
+                        h.edge_weights.empty() ? std::span<const EdgeWeight>()
+                                               : std::span<const EdgeWeight>(h.edge_weights.data() + e0, e1 - e0)};
+  }
+  struct DeviceArrays {
+    const std::uint32_t *nodes = nullptr, *edges = nullptr;
+    const std::int32_t *node_weights = nullptr, *edge_weights = nullptr;
+  };
+  [[nodiscard]] DeviceArrays device_arrays() const {
+    DeviceArrays d;
+    detail::check(kmp_subgraphs_device_arrays(_g, &d.nodes, &d.edges, &d.node_weights, &d.edge_weights, nullptr,
+                                              nullptr, nullptr, nullptr));
+    return d;
+  }
+  [[nodiscard]] const kmp_subgraph_stats &stats() const { return _stats; }
+  [[nodiscard]] const kmp_subgraphs *device() const { return _g; }
+
+private:
+  kmp_subgraphs *_g;
+  kmp_subgraph_stats _stats;
+  HostBlocks _host;
+};
+
+// The block-induced subgraphs of the k-way partition of the graph `h` holds: `partition` (n block ids, loaded as h's
+// labels), or, when empty, the labels h holds on the device (e.g. left by the last LP refinement).
+inline std::unique_ptr<Subgraphs> extract_subgraphs(kmp_lp_handle *h, BlockID k, std::span<const BlockID> partition = {}) {
+  kmp_subgraphs *g = nullptr;
+  kmp_subgraph_stats stats{};
+  detail::check(kmp_extract_subgraphs(h, k, partition.empty() ? nullptr : partition.data(), &g, &stats));
+  return std::make_unique<Subgraphs>(g, stats);
+}
+
+// graph::copy_subgraph_partitions(p_graph, subgraph_partitions, k_prime, input_k, mapping) (subgraph_extractor.cc:
+// 492-533) on the handle that extracted `subgraphs`: sub_partitions holds every block's sub-partition block-major
+// (block b's at node_offsets()[b]; a block that was not split holds zeros). The k'-way result becomes h's labels and
+// block weights; `out` (n entries, or empty) receives a host copy.
+inline void copy_subgraph_partitions(kmp_lp_handle *h, const Subgraphs &subgraphs,
+                                     std::span<const BlockID> sub_partitions, BlockID k_prime, BlockID input_k,
+                                     std::span<BlockID> out = {}) {
+  if (sub_partitions.size() != subgraphs.n() || (!out.empty() && out.size() != subgraphs.n())) {
+    throw std::invalid_argument("copy_subgraph_partitions: wrong span size");
+  }
+  detail::check(kmp_subgraphs_copy_partitions(h, subgraphs.device(), k_prime, input_k, sub_partitions.data(),
+                                              out.empty() ? nullptr : out.data(), nullptr));
 }
 
 } // namespace kaminpar_b200

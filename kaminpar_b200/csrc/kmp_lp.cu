@@ -27,6 +27,7 @@
 #include "../../include/kaminpar_b200_contraction.h"
 #include "../../include/kaminpar_b200_lp.h"
 #include "../../include/kaminpar_b200_prepare.h"
+#include "../../include/kaminpar_b200_subgraph.h"
 #include "lp_commit.cuh"
 #include "lp_device.cuh"
 #include "lp_lowgroup.cuh"
@@ -162,6 +163,7 @@ struct kmp_lp_handle {
   DevBuf<uint32_t> own_xadj, own_adjncy;
   DevBuf<int32_t> own_vwgt, own_adjwgt;
   bool have_graph = false;
+  uint64_t graph_epoch = 0; // counts set_graph calls: a kmp_subgraphs knows which graph it was extracted from
   uint32_t max_degree = 0;
   uint32_t num_isolated = 0;
 
@@ -290,15 +292,31 @@ void overlay_release(kmp_lp_handle *h, bool scratch); // kmp_overlay.cuh
 
 namespace kmp {
 // block weights from labels; counts labels >= k (a clustering is not a partition) into *bad. The one range check
-// of the refiner and both balancers (checked_block_weights).
+// of the refiner and both balancers (checked_block_weights). Warp-aggregated: the lanes of a warp that share a block
+// add their weights first and one lane issues the atomic, so that with few blocks (k = 2 on 10^7 vertices) the
+// atomics do not serialise on a handful of addresses. Integer sums: the result is the per-vertex atomics' result.
+// blockDim.x must be a multiple of 32 (the loop bound is warp-uniform).
 __global__ void bal_block_weights(uint32_t n, uint32_t k, const int32_t *vwgt, const uint32_t *label, int32_t *weight,
                                   unsigned long long *bad) {
-  for (uint32_t u = blockIdx.x * blockDim.x + threadIdx.x; u < n; u += gridDim.x * blockDim.x) {
-    const uint32_t b = label[u];
-    if (b < k) {
-      atomicAdd(&weight[b], vwgt != nullptr ? vwgt[u] : 1);
-    } else {
-      atomicAdd(bad, 1ull);
+  const uint32_t lane = threadIdx.x & 31;
+  for (uint32_t base = blockIdx.x * blockDim.x + (threadIdx.x & ~31u); base < n; base += gridDim.x * blockDim.x) {
+    const uint32_t u = base + lane;
+    const bool live = u < n;
+    const uint32_t b = live ? label[u] : 0xFFFFFFFFu;
+    const bool ok = live && b < k;
+    const int32_t w = ok ? (vwgt != nullptr ? vwgt[u] : 1) : 0;
+    const unsigned out_of_range = __ballot_sync(kFull, live && !ok);
+    if (lane == 0 && out_of_range != 0) {
+      atomicAdd(bad, static_cast<unsigned long long>(__popc(out_of_range)));
+    }
+    const unsigned peers = __match_any_sync(kFull, ok ? b : 0xFFFFFFFFu);
+    int32_t sum = 0;
+    for (int j = 0; j < 32; ++j) {
+      const int32_t x = __shfl_sync(kFull, w, j);
+      sum += ((peers >> j) & 1u) ? x : 0;
+    }
+    if (ok && lane == static_cast<uint32_t>(__ffs(peers) - 1)) {
+      atomicAdd(&weight[b], sum);
     }
   }
 }
@@ -2345,6 +2363,7 @@ static int set_graph_common(kmp_lp_handle *h, uint32_t n, uint32_t m) {
   h->n = n;
   h->m = m;
   h->have_graph = true;
+  ++h->graph_epoch;
   h->labels_valid = false;
   overlay_release(h, false); // stream-ordered: the stash belongs to the previous graph
   h->lists_valid = false;
@@ -2967,6 +2986,7 @@ int kmp_lp_step_finish(kmp_lp_handle *h, uint32_t *labels_out, int32_t *block_we
 #include "kmp_balance.cuh"
 #include "kmp_underload.cuh"
 #include "kmp_prepare.cuh"
+#include "kmp_subgraph.cuh"
 
 #ifdef KMP_HUB_PHASE_STAMPS
 // scripts/hub_rate_phases.py: reads (and with reset != 0 zeroes) the rate kernel's 7 phase accumulators
