@@ -95,16 +95,14 @@ def _lib():
     return lib
 
 
-class CoarseGraph:
+class CoarseGraph(lp.DeviceResult):
     """``kaminpar::shm::CoarseGraph`` (cluster_contraction.h:22-32). The coarse graph lives on the
     device; `get()` downloads it once, `device_arrays()` hands it to the next level's LP handle."""
 
-    def __init__(self, handle_ptr, stats: ContractionStats, keepalive=None):
-        self._g = handle_ptr
-        self.stats = stats
-        self._keepalive = keepalive  # the LPHandle whose graph was contracted (owns the stream)
-        if keepalive is not None:
-            keepalive._children += 1  # the handle is destroyed after this graph (see close)
+    _destroy = "kmp_coarse_destroy"
+
+    def __init__(self, ptr, stats: ContractionStats, handle: lp.LPHandle):
+        super().__init__(ptr, stats, handle)
         self._host: Optional[CSRGraph] = None
         self._mapping: Optional[np.ndarray] = None
 
@@ -137,9 +135,7 @@ class CoarseGraph:
 
     def device_arrays(self):
         """(d_xadj, d_adjncy, d_vwgt, d_adjwgt, d_mapping) as integers; valid while this object lives."""
-        ptrs = [C.c_void_p() for _ in range(5)]
-        lp._check(_lib().kmp_coarse_device_arrays(self._g, *[C.byref(p) for p in ptrs]))
-        return tuple(int(p.value or 0) for p in ptrs)
+        return self._device_ptrs("kmp_coarse_device_arrays", 5)
 
     def project_up(self, coarse, fine: Optional[np.ndarray] = None) -> np.ndarray:
         coarse = np.ascontiguousarray(coarse, np.uint32)
@@ -169,22 +165,6 @@ class CoarseGraph:
         self._host = None
         self.sparsify_stats = stats
         return stats
-
-    def close(self):
-        if getattr(self, "_g", None):
-            _lib().kmp_coarse_destroy(self._g)  # frees on the handle's stream: the handle must still exist
-            self._g = None
-            k = self._keepalive
-            if k is not None:
-                k._children -= 1
-                if k._close_pending and k._children == 0:
-                    k.close()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 def sparsification_target(prev_m: int, prev_n: int, c_n: int, density_target_factor: float = 0.5,
@@ -226,7 +206,7 @@ def contract_on_handle(handle: lp.LPHandle, clustering: Optional[np.ndarray]) ->
     out = C.c_void_p()
     stats = ContractionStats()
     lp._check(_lib().kmp_contract_clustering(handle._h, lp._ptr(cl), C.byref(out), C.byref(stats)))
-    return CoarseGraph(out, stats, keepalive=handle)
+    return CoarseGraph(out, stats, handle)
 
 
 def overlay_level(handle: lp.LPHandle, level: int, ctx: Optional[OverlayClusterCoarseningContext],

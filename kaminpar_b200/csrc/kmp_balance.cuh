@@ -469,14 +469,6 @@ int bal_evaluate(kmp_lp_handle *h, uint32_t k, uint32_t nc, uint32_t base_tie, b
   return KMP_OK;
 }
 
-template <typename Fn> int bal_cub(kmp_lp_handle *h, Fn &&call) {
-  size_t bytes = 0;
-  KMP_CUDA(call(static_cast<void *>(nullptr), bytes));
-  KMP_CUDA(h->cub_tmp.ensure(bytes));
-  KMP_CUDA(call(static_cast<void *>(h->cub_tmp.p), bytes));
-  return KMP_OK;
-}
-
 // The end of a round of either balancer, after its selection left ns sort words (block << 32 | desc key bits) and
 // candidate indices in bal_sk_a / bal_sv_a: sort them by (block, key desc), scan the weights per block, propose the
 // candidates whose preceding weight in their block is below the block's quota bal_over[b], and commit the proposals
@@ -490,22 +482,16 @@ int bal_round_tail(kmp_lp_handle *h, BalKind kind, uint32_t k, uint32_t ns, uint
     ++end_bit;
   }
   cudaStream_t st = h->stream;
-  int rc = bal_cub(h, [&](void *tmp, size_t &bytes) {
+  KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
     return cub::DeviceRadixSort::SortPairs(tmp, bytes, h->bal_sk_a.p, h->bal_sk_b.p, h->bal_sv_a.p, h->bal_sv_b.p,
                                            static_cast<int>(ns), 0, static_cast<int>(end_bit), st);
-  });
-  if (rc != KMP_OK) {
-    return rc;
-  }
+  }));
   bal_sorted_weights<<<capped(h, grid_for(ns, 256)), 256, 0, st>>>(ns, h->bal_sk_b.p, h->bal_sv_b.p, h->bal_cand.p, h->vwgt,
                                                                    h->bal_blk.p, h->bal_wt.p);
-  rc = bal_cub(h, [&](void *tmp, size_t &bytes) {
+  KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
     return cub::DeviceScan::ExclusiveSumByKey(tmp, bytes, h->bal_blk.p, h->bal_wt.p, h->bal_prefix.p,
                                               static_cast<int>(ns), cub::Equality(), st);
-  });
-  if (rc != KMP_OK) {
-    return rc;
-  }
+  }));
   const bool under = kind == BalKind::Underload;
   uint32_t *mover_count = h->bal_ctr32.p;
   if (under) {
@@ -526,7 +512,7 @@ int bal_round_tail(kmp_lp_handle *h, BalKind kind, uint32_t k, uint32_t ns, uint
   ca.moved_count = h->bal_ctr32.p + 4 + r;
   ca.base_commit = sync_base(h->cfg.seed, call, r, under ? SALT_UBAL_COMMIT : SALT_BAL_COMMIT);
   ca.stamp = 0;
-  rc = launch_commit_refine(h, ca, GatheredArgs{nullptr, 1, 0, nullptr}, 1, ns);
+  const int rc = launch_commit_refine(h, ca, GatheredArgs{nullptr, 1, 0, nullptr}, 1, ns);
   if (rc != KMP_OK) {
     return rc;
   }
@@ -543,21 +529,15 @@ int bal_round_begin(kmp_lp_handle *h, uint32_t k, unsigned long long *host_ctrl,
   KMP_CUDA(cudaMemsetAsync(h->bal_ctrl.p, 0, 3 * sizeof(unsigned long long), st));
   bal_block_stats<<<capped(h, grid_for(k, 256)), 256, 0, st>>>(k, h->weight.p, h->maxw.p, h->bal_pbw.p, h->bal_over.p,
                                                                h->bal_flag.p, h->bal_ctrl.p);
-  int rc = bal_cub(h, [&](void *tmp, size_t &bytes) {
+  KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
     return cub::DeviceSelect::Flagged(tmp, bytes, thrust::counting_iterator<uint32_t>(0), h->bal_flag.p, h->bal_under.p,
                                       h->bal_ctrl.p + 2, static_cast<int>(k), st);
-  });
-  if (rc != KMP_OK) {
-    return rc;
-  }
+  }));
   bal_vertex_flags<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, h->label.p, h->bal_over.p, h->bal_flag.p);
-  rc = bal_cub(h, [&](void *tmp, size_t &bytes) {
+  KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
     return cub::DeviceSelect::Flagged(tmp, bytes, thrust::counting_iterator<uint32_t>(0), h->bal_flag.p, h->bal_cand.p,
                                       h->bal_ctrl.p + 1, static_cast<int>(n), st);
-  });
-  if (rc != KMP_OK) {
-    return rc;
-  }
+  }));
   h->kernel_launches += 4;
   KMP_CUDA(cudaMemcpyAsync(host_ctrl, h->bal_ctrl.p, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
   KMP_CUDA(cudaMemcpyAsync(host_proposals, h->bal_ctr32.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));

@@ -23,70 +23,9 @@
 // ceil(2b/8) radix passes of 24 B each.
 #pragma once
 
-#include <mutex>
-
 #include <cub/block/block_scan.cuh>
 #include <cub/device/device_reduce.cuh>
 #include <cub/device/device_run_length_encode.cuh>
-
-// Output arrays come from the device's stream-ordered memory pool (cudaMallocAsync): a coarsening
-// loop allocates and frees coarse graphs of hundreds of MB per level, and cudaMalloc / cudaFree of that
-// size cost milliseconds and serialise the device. The pool keeps freed blocks (release threshold set
-// in contract_impl), so after the first level an allocation is a pointer bump.
-// A PRIVATE pool per device (never the device's default pool, which the host application or torch's
-// cudaMallocAsync backend may share -- ADVICE r1): freed blocks stay in it until kmp_lp_free_scratch trims it.
-inline cudaMemPool_t kmp_private_pool(int device) {
-  static std::mutex mu;
-  static cudaMemPool_t pools[64] = {};
-  std::lock_guard<std::mutex> lock(mu);
-  if (device < 0 || device >= 64) {
-    return nullptr;
-  }
-  if (pools[device] == nullptr) {
-    cudaMemPoolProps props{};
-    props.allocType = cudaMemAllocationTypePinned;
-    props.handleTypes = cudaMemHandleTypeNone;
-    props.location.type = cudaMemLocationTypeDevice;
-    props.location.id = device;
-    cudaMemPool_t pool = nullptr;
-    if (cudaMemPoolCreate(&pool, &props) == cudaSuccess) {
-      unsigned long long keep = ~0ull;
-      cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
-      pools[device] = pool;
-    }
-  }
-  return pools[device];
-}
-
-template <typename T> struct PoolBuf {
-  T *p = nullptr;
-  size_t cap = 0;
-  cudaStream_t stream = nullptr; // the stream the block was allocated on: it is freed there, too
-  cudaError_t alloc(size_t n, cudaStream_t st, int device) {
-    release();
-    cudaMemPool_t pool = kmp_private_pool(device);
-    if (pool == nullptr) {
-      return cudaErrorMemoryAllocation;
-    }
-    cudaError_t e = cudaMallocFromPoolAsync(reinterpret_cast<void **>(&p), std::max<size_t>(n, 1) * sizeof(T), pool, st);
-    if (e == cudaSuccess) {
-      cap = std::max<size_t>(n, 1);
-      stream = st;
-    } else {
-      p = nullptr;
-    }
-    return e;
-  }
-  // stream-ordered: a later user of the arrays (e.g. the next level's LP handle) must have synchronised with
-  // `stream` before the coarse graph is destroyed (kmp_coarse_destroy documents it)
-  void release() {
-    if (p != nullptr) {
-      cudaFreeAsync(p, stream);
-    }
-    p = nullptr;
-    cap = 0;
-  }
-};
 
 struct kmp_coarse_graph {
   int device = 0;
@@ -96,14 +35,6 @@ struct kmp_coarse_graph {
 };
 
 namespace {
-
-// scratch that lives for one call (DevBuf itself has no destructor: handle members are released explicitly)
-template <typename T> struct ScratchBuf : DevBuf<T> {
-  ScratchBuf() = default;
-  ScratchBuf(const ScratchBuf &) = delete;
-  ScratchBuf &operator=(const ScratchBuf &) = delete;
-  ~ScratchBuf() { this->release(); }
-};
 
 constexpr int kTileEdges = 2048;  // fine edges per CTA in the key pass (256 threads x 8)
 constexpr int kTileVerts = 2304;  // xadj entries of a tile staged in shared memory (else: global search)
@@ -270,7 +201,6 @@ int contract_impl(kmp_lp_handle *h, const uint32_t *clustering, kmp_coarse_graph
   const uint32_t n = h->n, m = h->m;
   cudaStream_t st = h->stream;
   uint32_t launches = 0;
-  cg->device = h->device;
   cg->fine_n = n;
   KMP_CUDA(cg->mapping.alloc(n, st, h->device));
   if (n == 0) {
@@ -289,22 +219,15 @@ int contract_impl(kmp_lp_handle *h, const uint32_t *clustering, kmp_coarse_graph
   } else {
     cl = h->label.p; // kmp_contract_clustering refused labels of another graph
   }
-  // a dedicated event pair (the handle's own pair may bracket an open stepping call -- ADVICE r1)
-  if (h->ev_ct0 == nullptr) {
-    KMP_CUDA(cudaEventCreate(&h->ev_ct0));
-    KMP_CUDA(cudaEventCreate(&h->ev_ct1));
-  }
-  cudaEvent_t ev0 = h->ev_ct0, ev1 = h->ev_ct1;
-  KMP_CUDA(cudaEventRecord(ev0, st));
+  KMP_CUDA(call_clock_start(h, st));
   // ---- 1. mapping ------------------------------------------------------------------------------
   KMP_CUDA(flags.ensure(static_cast<size_t>(n) + 1)); // flags[n]: out-of-range marker
   KMP_CUDA(rank.ensure(n));
   KMP_CUDA(cudaMemsetAsync(flags.p, 0, (static_cast<size_t>(n) + 1) * 4, st));
   k_flag_leaders<<<grid_for(n, 256), 256, 0, st>>>(n, cl, flags.p, flags.p + n);
-  size_t tmp_bytes = 0;
-  KMP_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, flags.p, rank.p, static_cast<int>(n), st));
-  KMP_CUDA(h->cub_tmp.ensure(std::max<size_t>(tmp_bytes, 1)));
-  KMP_CUDA(cub::DeviceScan::InclusiveSum(h->cub_tmp.p, tmp_bytes, flags.p, rank.p, static_cast<int>(n), st));
+  KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
+    return cub::DeviceScan::InclusiveSum(tmp, bytes, flags.p, rank.p, static_cast<int>(n), st);
+  }));
   uint32_t host2[2] = {0, 0};
   KMP_CUDA(cudaMemcpyAsync(&host2[0], rank.p + (n - 1), 4, cudaMemcpyDeviceToHost, st));
   KMP_CUDA(cudaMemcpyAsync(&host2[1], flags.p + n, 4, cudaMemcpyDeviceToHost, st));
@@ -362,27 +285,26 @@ int contract_impl(kmp_lp_handle *h, const uint32_t *clustering, kmp_coarse_graph
     int32_t *uw = nullptr;            // their weights
     if (h->adjwgt != nullptr) {
       cub::DoubleBuffer<int32_t> dv(vals_a.p, vals_b.p);
-      KMP_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, dk, dv, items, 0, static_cast<int>(bits), st));
-      KMP_CUDA(h->cub_tmp.ensure(std::max<size_t>(tmp_bytes, 1)));
-      KMP_CUDA(cub::DeviceRadixSort::SortPairs(h->cub_tmp.p, tmp_bytes, dk, dv, items, 0, static_cast<int>(bits), st));
+      KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
+        return cub::DeviceRadixSort::SortPairs(tmp, bytes, dk, dv, items, 0, static_cast<int>(bits), st);
+      }));
       uk = dk.Alternate();
       uw = dv.Alternate();
-      KMP_CUDA(cub::DeviceReduce::ReduceByKey(nullptr, tmp_bytes, dk.Current(), uk, dv.Current(), uw, num_runs,
-                                              cub::Sum(), items, st));
-      KMP_CUDA(h->cub_tmp.ensure(std::max<size_t>(tmp_bytes, 1)));
-      KMP_CUDA(cub::DeviceReduce::ReduceByKey(h->cub_tmp.p, tmp_bytes, dk.Current(), uk, dv.Current(), uw, num_runs,
-                                              cub::Sum(), items, st));
+      KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
+        return cub::DeviceReduce::ReduceByKey(tmp, bytes, dk.Current(), uk, dv.Current(), uw, num_runs, cub::Sum(),
+                                              items, st);
+      }));
     } else {
       // unit edge weights (the finest, i.e. largest, level): sort the keys alone (8 instead of 12 bytes per
       // item and pass); the weight of a coarse edge is the length of its run
-      KMP_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tmp_bytes, dk, items, 0, static_cast<int>(bits), st));
-      KMP_CUDA(h->cub_tmp.ensure(std::max<size_t>(tmp_bytes, 1)));
-      KMP_CUDA(cub::DeviceRadixSort::SortKeys(h->cub_tmp.p, tmp_bytes, dk, items, 0, static_cast<int>(bits), st));
+      KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
+        return cub::DeviceRadixSort::SortKeys(tmp, bytes, dk, items, 0, static_cast<int>(bits), st);
+      }));
       uk = dk.Alternate();
       uw = vals_b.p;
-      KMP_CUDA(cub::DeviceRunLengthEncode::Encode(nullptr, tmp_bytes, dk.Current(), uk, uw, num_runs, items, st));
-      KMP_CUDA(h->cub_tmp.ensure(std::max<size_t>(tmp_bytes, 1)));
-      KMP_CUDA(cub::DeviceRunLengthEncode::Encode(h->cub_tmp.p, tmp_bytes, dk.Current(), uk, uw, num_runs, items, st));
+      KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
+        return cub::DeviceRunLengthEncode::Encode(tmp, bytes, dk.Current(), uk, uw, num_runs, items, st);
+      }));
     }
     KMP_CUDA(cudaMemcpyAsync(&c_m, num_runs, 4, cudaMemcpyDeviceToHost, st));
     KMP_CUDA(cudaStreamSynchronize(st));
@@ -400,10 +322,9 @@ int contract_impl(kmp_lp_handle *h, const uint32_t *clustering, kmp_coarse_graph
     KMP_CUDA(cg->adjwgt.alloc(1, st, h->device));
   }
   cg->c_m = c_m;
-  KMP_CUDA(cudaEventRecord(ev1, st));
+  KMP_CUDA(call_clock_stop(h, st));
   KMP_CUDA(cudaStreamSynchronize(st));
-  float ms = 0.f;
-  cudaEventElapsedTime(&ms, ev0, ev1);
+  const float ms = call_clock_ms(h);
   if (stats != nullptr) {
     stats->c_n = c_n;
     stats->c_m = c_m;
@@ -435,17 +356,7 @@ int kmp_contract_clustering(kmp_lp_handle *h, const uint32_t *clustering, kmp_co
   if (stats != nullptr) {
     std::memset(stats, 0, sizeof(*stats));
   }
-  kmp_coarse_graph *cg = new (std::nothrow) kmp_coarse_graph();
-  if (cg == nullptr) {
-    return fail(KMP_ERR_ALLOC, "out of host memory");
-  }
-  rc = contract_impl(h, clustering, cg, stats);
-  if (rc != KMP_OK) {
-    kmp_coarse_destroy(cg);
-    return rc;
-  }
-  *out = cg;
-  return KMP_OK;
+  return make_result(h, out, [&](kmp_coarse_graph *cg) { return contract_impl(h, clustering, cg, stats); });
 }
 
 uint32_t kmp_coarse_n(const kmp_coarse_graph *g) { return g != nullptr ? g->c_n : 0; }
@@ -458,21 +369,11 @@ int kmp_coarse_download(const kmp_coarse_graph *g, uint32_t *xadj, uint32_t *adj
     return fail(KMP_ERR_INVALID, "null argument");
   }
   KMP_CUDA(cudaSetDevice(g->device));
-  if (xadj != nullptr) {
-    KMP_CUDA(cudaMemcpy(xadj, g->xadj.p, (static_cast<size_t>(g->c_n) + 1) * 4, cudaMemcpyDeviceToHost));
-  }
-  if (adjncy != nullptr && g->c_m > 0) {
-    KMP_CUDA(cudaMemcpy(adjncy, g->adjncy.p, static_cast<size_t>(g->c_m) * 4, cudaMemcpyDeviceToHost));
-  }
-  if (vwgt != nullptr && g->c_n > 0) {
-    KMP_CUDA(cudaMemcpy(vwgt, g->vwgt.p, static_cast<size_t>(g->c_n) * 4, cudaMemcpyDeviceToHost));
-  }
-  if (adjwgt != nullptr && g->c_m > 0) {
-    KMP_CUDA(cudaMemcpy(adjwgt, g->adjwgt.p, static_cast<size_t>(g->c_m) * 4, cudaMemcpyDeviceToHost));
-  }
-  if (mapping != nullptr && g->fine_n > 0) {
-    KMP_CUDA(cudaMemcpy(mapping, g->mapping.p, static_cast<size_t>(g->fine_n) * 4, cudaMemcpyDeviceToHost));
-  }
+  KMP_CUDA(copy_out(xadj, g->xadj, static_cast<size_t>(g->c_n) + 1));
+  KMP_CUDA(copy_out(adjncy, g->adjncy, g->c_m));
+  KMP_CUDA(copy_out(vwgt, g->vwgt, g->c_n));
+  KMP_CUDA(copy_out(adjwgt, g->adjwgt, g->c_m));
+  KMP_CUDA(copy_out(mapping, g->mapping, g->fine_n));
   return KMP_OK;
 }
 
@@ -481,21 +382,11 @@ int kmp_coarse_device_arrays(const kmp_coarse_graph *g, const uint32_t **d_xadj,
   if (g == nullptr) {
     return fail(KMP_ERR_INVALID, "null argument");
   }
-  if (d_xadj != nullptr) {
-    *d_xadj = g->xadj.p;
-  }
-  if (d_adjncy != nullptr) {
-    *d_adjncy = g->adjncy.p;
-  }
-  if (d_vwgt != nullptr) {
-    *d_vwgt = g->vwgt.p;
-  }
-  if (d_adjwgt != nullptr) {
-    *d_adjwgt = g->adjwgt.p;
-  }
-  if (d_mapping != nullptr) {
-    *d_mapping = g->mapping.p;
-  }
+  hand_out(d_xadj, g->xadj);
+  hand_out(d_adjncy, g->adjncy);
+  hand_out(d_vwgt, g->vwgt);
+  hand_out(d_adjwgt, g->adjwgt);
+  hand_out(d_mapping, g->mapping);
   return KMP_OK;
 }
 
@@ -507,7 +398,7 @@ int kmp_coarse_project_up(const kmp_coarse_graph *g, const uint32_t *coarse, uin
     return KMP_OK;
   }
   KMP_CUDA(cudaSetDevice(g->device));
-  ScratchBuf<uint32_t> d_c, d_f;
+  DevBuf<uint32_t> d_c, d_f;
   KMP_CUDA(d_c.ensure(g->c_n));
   KMP_CUDA(d_f.ensure(g->fine_n));
   KMP_CUDA(cudaMemcpy(d_c.p, coarse, static_cast<size_t>(g->c_n) * 4, cudaMemcpyHostToDevice));
@@ -525,7 +416,7 @@ int kmp_coarse_project_down(const kmp_coarse_graph *g, const uint32_t *fine, uin
     return KMP_OK;
   }
   KMP_CUDA(cudaSetDevice(g->device));
-  ScratchBuf<uint32_t> d_c, d_f;
+  DevBuf<uint32_t> d_c, d_f;
   KMP_CUDA(d_c.ensure(g->c_n));
   KMP_CUDA(d_f.ensure(g->fine_n));
   KMP_CUDA(cudaMemcpy(d_f.p, fine, static_cast<size_t>(g->fine_n) * 4, cudaMemcpyHostToDevice));
@@ -540,12 +431,7 @@ void kmp_coarse_destroy(kmp_coarse_graph *g) {
   if (g == nullptr) {
     return;
   }
-  cudaSetDevice(g->device);
-  g->xadj.release();
-  g->adjncy.release();
-  g->mapping.release();
-  g->vwgt.release();
-  g->adjwgt.release();
+  cudaSetDevice(g->device); // the arrays free themselves on this device's pool
   delete g;
 }
 

@@ -14,8 +14,11 @@
 #include <chrono>
 #include <cstdio>
 #include <cstring>
+#include <memory>
+#include <mutex>
 #include <new>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include <cstdlib>
@@ -108,8 +111,97 @@ template <typename T> struct DevBuf {
 
 } // namespace
 
-cudaMemPool_t kmp_private_pool(int device); // kmp_contract.cuh
+// The result objects of the graph operations (coarse, prepared and subgraph arrays) and their per-call scratch come
+// from the device's stream-ordered memory pool (cudaMallocAsync): a coarsening loop allocates and frees coarse graphs
+// of hundreds of MB per level, and cudaMalloc / cudaFree of that size cost milliseconds and serialise the device. The
+// pool keeps freed blocks (its release threshold is unbounded), so after the first level an allocation is a pointer
+// bump. A PRIVATE pool per device (never the device's default pool, which the host application or torch's
+// cudaMallocAsync backend may share): freed blocks stay in it until kmp_lp_free_scratch trims it.
+inline cudaMemPool_t kmp_private_pool(int device) {
+  static std::mutex mu;
+  static cudaMemPool_t pools[64] = {};
+  std::lock_guard<std::mutex> lock(mu);
+  if (device < 0 || device >= 64) {
+    return nullptr;
+  }
+  if (pools[device] == nullptr) {
+    cudaMemPoolProps props{};
+    props.allocType = cudaMemAllocationTypePinned;
+    props.handleTypes = cudaMemHandleTypeNone;
+    props.location.type = cudaMemLocationTypeDevice;
+    props.location.id = device;
+    cudaMemPool_t pool = nullptr;
+    if (cudaMemPoolCreate(&pool, &props) == cudaSuccess) {
+      unsigned long long keep = ~0ull;
+      cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
+      pools[device] = pool;
+    }
+  }
+  return pools[device];
+}
+
+// An owned block of kmp_private_pool. It is freed stream-ordered, on the stream it was allocated on, when the owner is
+// destroyed, reallocated or assigned another block: a later user of the arrays on another stream (e.g. the next
+// level's LP handle) must have synchronised with `stream` before then (kmp_coarse_destroy documents it).
+template <typename T> struct PoolBuf {
+  T *p = nullptr;
+  size_t cap = 0;
+  cudaStream_t stream = nullptr;
+  PoolBuf() = default;
+  PoolBuf(const PoolBuf &) = delete;
+  PoolBuf &operator=(const PoolBuf &) = delete;
+  PoolBuf(PoolBuf &&o) noexcept : p(std::exchange(o.p, nullptr)), cap(std::exchange(o.cap, 0)), stream(o.stream) {}
+  PoolBuf &operator=(PoolBuf &&o) noexcept {
+    if (this != &o) {
+      release();
+      p = std::exchange(o.p, nullptr);
+      cap = std::exchange(o.cap, 0);
+      stream = o.stream;
+    }
+    return *this;
+  }
+  ~PoolBuf() { release(); }
+  cudaError_t alloc(size_t n, cudaStream_t st, int device) {
+    release();
+    cudaMemPool_t pool = kmp_private_pool(device);
+    if (pool == nullptr) {
+      return cudaErrorMemoryAllocation;
+    }
+    cudaError_t e = cudaMallocFromPoolAsync(reinterpret_cast<void **>(&p), std::max<size_t>(n, 1) * sizeof(T), pool, st);
+    if (e == cudaSuccess) {
+      cap = std::max<size_t>(n, 1);
+      stream = st;
+    } else {
+      p = nullptr;
+    }
+    return e;
+  }
+  void release() {
+    if (p != nullptr) {
+      cudaFreeAsync(p, stream);
+    }
+    p = nullptr;
+    cap = 0;
+  }
+};
+
 namespace {
+// D2H copy of the first `count` elements of a result array; a null destination, an unallocated array (unit weights)
+// or count 0 copies nothing
+template <typename T> cudaError_t copy_out(T *dst, const PoolBuf<T> &buf, size_t count) {
+  if (dst == nullptr || buf.p == nullptr || count == 0) {
+    return cudaSuccess;
+  }
+  return cudaMemcpy(dst, buf.p, count * sizeof(T), cudaMemcpyDeviceToHost);
+}
+
+// the device pointer of a result array (null: unallocated) to a caller's non-null slot
+template <typename T> void hand_out(const T **dst, const PoolBuf<T> &buf) {
+  if (dst != nullptr) {
+    *dst = buf.p;
+  }
+}
+
 struct OverlayState; // kmp_overlay.cuh
 
 // What one LP run (a clustering or a refinement) passes to its sweeps and commits.
@@ -133,7 +225,7 @@ struct kmp_lp_handle {
   cudaStream_t side_stream[3] = {nullptr, nullptr, nullptr};
   cudaEvent_t ev_fork = nullptr, ev_join[3] = {nullptr, nullptr, nullptr};
   cudaEvent_t ev_begin = nullptr, ev_end = nullptr;
-  cudaEvent_t ev_ct0 = nullptr, ev_ct1 = nullptr; // contraction timing (kmp_contract.cuh), created on first use
+  cudaEvent_t ev_ct0 = nullptr, ev_ct1 = nullptr; // graph-operation timing (call_clock_start), created on first use
   bool timing = false;
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> sweep_events;
   std::vector<int> sweep_event_group;
@@ -288,6 +380,56 @@ struct kmp_lp_handle {
 
 namespace {
 void overlay_release(kmp_lp_handle *h, bool scratch); // kmp_overlay.cuh
+
+// A CUB device-wide call in its two phases: call(nullptr, bytes) asks for the temporary storage, call(tmp, bytes) runs
+// on h->cub_tmp grown to it (CUB never asks for 0 bytes, so tmp is never null and the second call is never a query).
+template <typename Fn> cudaError_t cub_call(kmp_lp_handle *h, Fn &&call) {
+  size_t bytes = 0;
+  cudaError_t e = call(static_cast<void *>(nullptr), bytes);
+  if (e == cudaSuccess) {
+    e = h->cub_tmp.ensure(bytes);
+  }
+  return e != cudaSuccess ? e : call(static_cast<void *>(h->cub_tmp.p), bytes);
+}
+
+// Device time of one graph-operation call (contraction, sparsification, overlay, preparation, subgraph extraction) on
+// the handle's event pair ev_ct0 / ev_ct1, created on first use. None of these calls runs inside another, and the pair
+// is not ev_begin / ev_end, which may bracket an open stepping call.
+cudaError_t call_clock_start(kmp_lp_handle *h, cudaStream_t st) {
+  if (h->ev_ct0 == nullptr) {
+    cudaError_t e = cudaEventCreate(&h->ev_ct0);
+    if (e == cudaSuccess) {
+      e = cudaEventCreate(&h->ev_ct1);
+    }
+    if (e != cudaSuccess) {
+      return e;
+    }
+  }
+  return cudaEventRecord(h->ev_ct0, st);
+}
+cudaError_t call_clock_stop(kmp_lp_handle *h, cudaStream_t st) { return cudaEventRecord(h->ev_ct1, st); }
+// after the caller has waited for the stop event (on the event or on its stream)
+float call_clock_ms(const kmp_lp_handle *h) {
+  float ms = 0.f;
+  cudaEventElapsedTime(&ms, h->ev_ct0, h->ev_ct1);
+  return ms;
+}
+
+// A new result object T of a call on h (kmp_coarse_graph, kmp_prepared_graph, kmp_subgraphs), filled by impl(obj) and
+// handed to *out only if impl succeeds. A refused call leaves *out untouched and frees what impl allocated; obj->device
+// is set before impl allocates anything.
+template <typename T, typename Impl> int make_result(const kmp_lp_handle *h, T **out, Impl &&impl) {
+  std::unique_ptr<T> obj(new (std::nothrow) T());
+  if (obj == nullptr) {
+    return fail(KMP_ERR_ALLOC, "out of host memory");
+  }
+  obj->device = h->device;
+  const int rc = impl(obj.get());
+  if (rc == KMP_OK) {
+    *out = obj.release();
+  }
+  return rc;
+}
 } // namespace
 
 namespace kmp {
@@ -906,13 +1048,11 @@ int ensure_lists(kmp_lp_handle *h) {
                                                         h->adjwgt != nullptr ? kHubMinDegree : kHubMinDegreeUnit,
                                                         h->sort_keys_in.p, h->sort_vals_in.p, h->ctr32.p, h->ctr32.p + 300);
   KMP_CUDA(cudaGetLastError());
-  size_t tmp_bytes = 0;
-  KMP_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, h->sort_keys_in.p, h->sort_keys_out.p,
-                                           h->sort_vals_in.p, h->order.p, static_cast<int>(n), 0, 8, h->stream));
-  KMP_CUDA(h->cub_tmp.ensure(tmp_bytes));
   if (n > 0) {
-    KMP_CUDA(cub::DeviceRadixSort::SortPairs(h->cub_tmp.p, tmp_bytes, h->sort_keys_in.p, h->sort_keys_out.p,
-                                             h->sort_vals_in.p, h->order.p, static_cast<int>(n), 0, 8, h->stream));
+    KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
+      return cub::DeviceRadixSort::SortPairs(tmp, bytes, h->sort_keys_in.p, h->sort_keys_out.p, h->sort_vals_in.p,
+                                             h->order.p, static_cast<int>(n), 0, 8, h->stream);
+    }));
   }
   std::vector<uint32_t> hist(512);
   KMP_CUDA(cudaMemcpyAsync(hist.data(), h->ctr32.p, 512 * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
@@ -1821,13 +1961,11 @@ int cluster_post_passes(kmp_lp_handle *h, int32_t max_w, uint32_t num_clusters, 
   const int iso = h->cfg.isolated_nodes_strategy;
   const bool iso_match = iso == KMP_ISOLATED_MATCH || (iso == KMP_ISOLATED_MATCH_DURING_TWO_HOP && two_hop);
   const bool iso_cluster = iso == KMP_ISOLATED_CLUSTER || (iso == KMP_ISOLATED_CLUSTER_DURING_TWO_HOP && two_hop);
-  auto sort_pairs = [&](uint32_t cnt, int bits) -> int { // pairs_a -> pairs_b, ascending
-    size_t tmp = 0;
-    KMP_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tmp, h->pairs_a.p, h->pairs_b.p, static_cast<int>(cnt), 0, bits, h->stream));
-    KMP_CUDA(h->cub_tmp.ensure(tmp));
-    KMP_CUDA(cub::DeviceRadixSort::SortKeys(h->cub_tmp.p, tmp, h->pairs_a.p, h->pairs_b.p, static_cast<int>(cnt), 0, bits,
-                                            h->stream));
-    return KMP_OK;
+  auto sort_pairs = [&](uint32_t cnt, int bits) { // pairs_a -> pairs_b, ascending
+    return cub_call(h, [&](void *tmp, size_t &bytes) {
+      return cub::DeviceRadixSort::SortKeys(tmp, bytes, h->pairs_a.p, h->pairs_b.p, static_cast<int>(cnt), 0, bits,
+                                            h->stream);
+    });
   };
   if ((iso_match || iso_cluster) && h->num_isolated > 1) {
     KMP_CUDA(h->pairs_a.ensure(h->num_isolated));
@@ -1838,10 +1976,7 @@ int cluster_post_passes(kmp_lp_handle *h, int32_t max_w, uint32_t num_clusters, 
     KMP_CUDA(cudaMemcpyAsync(&iso_cnt, h->ctr32.p + 2, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
     KMP_CUDA(cudaStreamSynchronize(h->stream));
     if (iso_cnt > 1) {
-      const int rc = sort_pairs(iso_cnt, 32); // key 0: ascending vertex id
-      if (rc != KMP_OK) {
-        return rc;
-      }
+      KMP_CUDA(sort_pairs(iso_cnt, 32)); // key 0: ascending vertex id
       if (iso_match) {
         k_match_isolated<<<grid_for(iso_cnt / 2 + 1, 256), 256, 0, h->stream>>>(iso_cnt, h->pairs_b.p, h->label.p, h->weight.p, max_w);
       } else {
@@ -1866,10 +2001,7 @@ int cluster_post_passes(kmp_lp_handle *h, int32_t max_w, uint32_t num_clusters, 
   KMP_CUDA(cudaMemcpyAsync(&cnt, h->ctr32.p + 2, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
   KMP_CUDA(cudaStreamSynchronize(h->stream));
   if (cnt > 1) {
-    const int rc = sort_pairs(cnt, 64);
-    if (rc != KMP_OK) {
-      return rc;
-    }
+    KMP_CUDA(sort_pairs(cnt, 64));
     if (h->cfg.two_hop_strategy == KMP_TWO_HOP_CLUSTER_THREADWISE) {
       k_next_fit<<<grid_for(static_cast<uint64_t>(cnt) * 32, 256, kSMs * 8), 256, 0, h->stream>>>(cnt, h->pairs_b.p, h->label.p,
                                                                                                  h->weight.p, max_w);
@@ -1879,10 +2011,9 @@ int cluster_post_passes(kmp_lp_handle *h, int32_t max_w, uint32_t num_clusters, 
       uint32_t *head_in = reinterpret_cast<uint32_t *>(h->pairs_a.p);
       uint32_t *head_out = head_in + cnt;
       k_two_hop_heads<<<grid_for(cnt, 256), 256, 0, h->stream>>>(cnt, h->pairs_b.p, head_in);
-      size_t tmp2 = 0;
-      KMP_CUDA(cub::DeviceScan::InclusiveScan(nullptr, tmp2, head_in, head_out, MaxOp(), static_cast<int>(cnt), h->stream));
-      KMP_CUDA(h->cub_tmp.ensure(tmp2));
-      KMP_CUDA(cub::DeviceScan::InclusiveScan(h->cub_tmp.p, tmp2, head_in, head_out, MaxOp(), static_cast<int>(cnt), h->stream));
+      KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
+        return cub::DeviceScan::InclusiveScan(tmp, bytes, head_in, head_out, MaxOp(), static_cast<int>(cnt), h->stream);
+      }));
       k_match_two_hop<<<grid_for(cnt, 256), 256, 0, h->stream>>>(cnt, h->pairs_b.p, head_out, h->label.p, h->weight.p);
       h->kernel_launches += 5;
     }

@@ -32,12 +32,9 @@ void overlay_release(kmp_lp_handle *h, bool scratch) {
   if (h->ov == nullptr) {
     return;
   }
-  for (PoolBuf<uint32_t> &b : h->ov->stash) {
-    b.release(); // stream-ordered: later than any work of the handle that still reads it
-  }
-  h->ov->stash.clear();
+  h->ov->stash.clear(); // stream-ordered: later than any work of the handle that still reads it
   if (scratch) {
-    delete h->ov; // the DevBufs free themselves
+    delete h->ov;
     h->ov = nullptr;
   }
 }
@@ -97,10 +94,9 @@ template <typename Then> int overlay_ranks(kmp_lp_handle *h, const uint32_t *lab
   KMP_CUDA(rank.ensure(n));
   KMP_CUDA(cudaMemsetAsync(flags.p, 0, (static_cast<size_t>(n) + 1) * 4, st));
   k_flag_leaders<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, labels, flags.p, flags.p + n);
-  size_t tmp_bytes = 0;
-  KMP_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, flags.p, rank.p, static_cast<int>(n), st));
-  KMP_CUDA(h->cub_tmp.ensure(std::max<size_t>(tmp_bytes, 1)));
-  KMP_CUDA(cub::DeviceScan::InclusiveSum(h->cub_tmp.p, tmp_bytes, flags.p, rank.p, static_cast<int>(n), st));
+  KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
+    return cub::DeviceScan::InclusiveSum(tmp, bytes, flags.p, rank.p, static_cast<int>(n), st);
+  }));
   int rc = then(rank.p, flags.p + n);
   if (rc != KMP_OK) {
     return rc;
@@ -142,19 +138,17 @@ int overlay_pair(kmp_lp_handle *h, const uint32_t *a, const uint32_t *b, uint32_
   cnt->sort_bits = std::max(cnt->sort_bits, bits);
   cub::DoubleBuffer<unsigned long long> dk(keys_a.p, keys_b.p);
   cub::DoubleBuffer<uint32_t> dv(ov.vals_a.p, ov.vals_b.p);
-  size_t tmp_bytes = 0;
   if (bits > 0) { // bits == 0 only for n == 1: one pair is sorted
-    KMP_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, dk, dv, static_cast<int>(n), 0, static_cast<int>(bits), st));
-    KMP_CUDA(h->cub_tmp.ensure(std::max<size_t>(tmp_bytes, 1)));
-    KMP_CUDA(cub::DeviceRadixSort::SortPairs(h->cub_tmp.p, tmp_bytes, dk, dv, static_cast<int>(n), 0,
-                                             static_cast<int>(bits), st));
+    KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
+      return cub::DeviceRadixSort::SortPairs(tmp, bytes, dk, dv, static_cast<int>(n), 0, static_cast<int>(bits), st);
+    }));
   }
   // ---- 4. heads + scan; 5. scatter. The leader flags and ranks are dead: P reuses the flags, seg the ranks ------------
   uint32_t *P = h->ct_flags.p, *seg = h->ct_rank.p;
   k_overlay_heads<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, dk.Current(), nb, P, seg);
-  KMP_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, P, P, static_cast<int>(n), st));
-  KMP_CUDA(h->cub_tmp.ensure(std::max<size_t>(tmp_bytes, 1)));
-  KMP_CUDA(cub::DeviceScan::InclusiveSum(h->cub_tmp.p, tmp_bytes, P, P, static_cast<int>(n), st));
+  KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
+    return cub::DeviceScan::InclusiveSum(tmp, bytes, P, P, static_cast<int>(n), st);
+  }));
   k_overlay_scatter<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, dk.Current(), dv.Current(), P, seg, nb, out);
   cnt->launches += 2; // + the sort and the scans inside CUB
   KMP_CUDA(cudaGetLastError());
@@ -228,18 +222,14 @@ int overlay_finish(kmp_lp_handle *h, uint32_t count, uint32_t *clustering_out, k
   float ms = 0.f;
   if (n > 0) {
     KMP_CUDA(h->label.ensure(n));
-    if (h->ev_ct0 == nullptr) {
-      KMP_CUDA(cudaEventCreate(&h->ev_ct0));
-      KMP_CUDA(cudaEventCreate(&h->ev_ct1));
-    }
-    KMP_CUDA(cudaEventRecord(h->ev_ct0, st));
+    KMP_CUDA(call_clock_start(h, st));
     const int rc = overlay_tree(h, count, h->label.p, &cnt);
     if (rc != KMP_OK) {
       return rc;
     }
-    KMP_CUDA(cudaEventRecord(h->ev_ct1, st));
+    KMP_CUDA(call_clock_stop(h, st));
     KMP_CUDA(cudaEventSynchronize(h->ev_ct1));
-    cudaEventElapsedTime(&ms, h->ev_ct0, h->ev_ct1);
+    ms = call_clock_ms(h);
     if (clustering_out != nullptr) {
       KMP_CUDA(cudaMemcpyAsync(clustering_out, h->label.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, st));
       KMP_CUDA(cudaStreamSynchronize(st));

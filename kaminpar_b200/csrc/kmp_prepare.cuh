@@ -28,14 +28,6 @@ constexpr uint32_t kPrepTileVerts = 4096; // vertices per CTA of passes 1 and 2 
 constexpr uint32_t kPrepBuckets = 33;     // kNumberOfDegreeBuckets<uint32_t> (degree_buckets.h:17)
 constexpr uint32_t kPrepIsolated = 32;    // the bucket of a degree-0 vertex
 
-// scratch of one call, from the device's pool and freed stream-ordered when the call returns
-template <typename T> struct CallBuf : PoolBuf<T> {
-  CallBuf() = default;
-  CallBuf(const CallBuf &) = delete;
-  CallBuf &operator=(const CallBuf &) = delete;
-  ~CallBuf() { this->release(); }
-};
-
 __device__ __forceinline__ uint32_t prep_bucket(uint32_t d) { // degree_buckets.h:24-26, permutator.h:105-107
   return d == 0 ? kPrepIsolated : 32u - __clz(d);
 }
@@ -288,12 +280,7 @@ int prepare_impl(kmp_lp_handle *h, uint32_t n, uint32_t m, const uint32_t *xadj,
   const cudaStream_t st = h->stream;
   const int dev = h->device;
   uint32_t launches = 0;
-  if (h->ev_ct0 == nullptr) { // the contraction's event pair: neither call runs inside the other
-    KMP_CUDA(cudaEventCreate(&h->ev_ct0));
-    KMP_CUDA(cudaEventCreate(&h->ev_ct1));
-  }
-  KMP_CUDA(cudaEventRecord(h->ev_ct0, st));
-  g->device = dev;
+  KMP_CUDA(call_clock_start(h, st));
   g->n = n;
   g->m = m;
   KMP_CUDA(g->xadj.alloc(static_cast<size_t>(n) + 1, st, dev));
@@ -309,17 +296,16 @@ int prepare_impl(kmp_lp_handle *h, uint32_t n, uint32_t m, const uint32_t *xadj,
   // ---- 1. validate, bucket, histogram -----------------------------------------------------------------------
   const uint32_t tiles = std::max<uint32_t>(1, (n + kPrepTileVerts - 1) / kPrepTileVerts);
   const size_t cells = static_cast<size_t>(kPrepBuckets) * tiles;
-  CallBuf<uint32_t> hist, base, deg, bad;
+  PoolBuf<uint32_t> hist, base, deg, bad; // scratch of this call
   KMP_CUDA(hist.alloc(cells, st, dev));
   KMP_CUDA(base.alloc(cells, st, dev));
   KMP_CUDA(bad.alloc(2, st, dev));
   KMP_CUDA(cudaMemsetAsync(bad.p, 0, 8, st));
   k_prep_count<<<tiles, 256, 0, st>>>(n, m, xadj, tiles, hist.p, bad.p);
   ++launches;
-  size_t tmp_bytes = 0;
-  KMP_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, hist.p, base.p, static_cast<int>(cells), st));
-  KMP_CUDA(h->cub_tmp.ensure(std::max<size_t>(tmp_bytes, 1)));
-  KMP_CUDA(cub::DeviceScan::ExclusiveSum(h->cub_tmp.p, tmp_bytes, hist.p, base.p, static_cast<int>(cells), st));
+  KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
+    return cub::DeviceScan::ExclusiveSum(tmp, bytes, hist.p, base.p, static_cast<int>(cells), st);
+  }));
   uint32_t host[2] = {0, 0};
   KMP_CUDA(cudaMemcpyAsync(&host[0], bad.p, 4, cudaMemcpyDeviceToHost, st));
   KMP_CUDA(cudaMemcpyAsync(&host[1], base.p + static_cast<size_t>(kPrepIsolated) * tiles, 4, cudaMemcpyDeviceToHost, st));
@@ -335,9 +321,9 @@ int prepare_impl(kmp_lp_handle *h, uint32_t n, uint32_t m, const uint32_t *xadj,
     k_prep_scatter<<<tiles, 256, 0, st>>>(n, xadj, vwgt, tiles, base.p, g->old_to_new.p, g->new_to_old.p, deg.p,
                                           g->vwgt.p);
     ++launches;
-    KMP_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, deg.p, g->xadj.p + 1, static_cast<int>(n), st));
-    KMP_CUDA(h->cub_tmp.ensure(std::max<size_t>(tmp_bytes, 1)));
-    KMP_CUDA(cub::DeviceScan::InclusiveSum(h->cub_tmp.p, tmp_bytes, deg.p, g->xadj.p + 1, static_cast<int>(n), st));
+    KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
+      return cub::DeviceScan::InclusiveSum(tmp, bytes, deg.p, g->xadj.p + 1, static_cast<int>(n), st);
+    }));
   }
   // ---- 3. edge copy -----------------------------------------------------------------------------------------
   if (m > 0) {
@@ -355,20 +341,18 @@ int prepare_impl(kmp_lp_handle *h, uint32_t n, uint32_t m, const uint32_t *xadj,
   }
   KMP_CUDA(cudaGetLastError());
   KMP_CUDA(cudaMemcpyAsync(&host[0], bad.p + 1, 4, cudaMemcpyDeviceToHost, st));
-  KMP_CUDA(cudaEventRecord(h->ev_ct1, st));
+  KMP_CUDA(call_clock_stop(h, st));
   KMP_CUDA(cudaStreamSynchronize(st));
   if (host[0] != 0) {
     return fail(KMP_ERR_INVALID, "adjncy holds a target >= n");
   }
   if (stats != nullptr) {
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, h->ev_ct0, h->ev_ct1);
     stats->n = n;
     stats->n_nonisolated = g->np;
     stats->num_isolated = n - g->np;
     stats->m = m;
     stats->kernel_launches = launches;
-    stats->device_ms = ms;
+    stats->device_ms = call_clock_ms(h);
   }
   return KMP_OK;
 }
@@ -390,14 +374,9 @@ int prepare_checked(kmp_lp_handle *h, uint32_t n, uint32_t m, const uint32_t *xa
   if (stats != nullptr) {
     std::memset(stats, 0, sizeof(*stats));
   }
-  kmp_prepared_graph *g = new (std::nothrow) kmp_prepared_graph();
-  if (g == nullptr) {
-    return fail(KMP_ERR_ALLOC, "out of host memory");
-  }
-  int rc = KMP_OK;
-  {
-    CallBuf<uint32_t> d_xadj, d_adj;
-    CallBuf<int32_t> d_vw, d_ew;
+  return make_result(h, out, [&](kmp_prepared_graph *g) {
+    PoolBuf<uint32_t> d_xadj, d_adj;
+    PoolBuf<int32_t> d_vw, d_ew;
     if (host_input) { // copies on the handle's stream, freed stream-ordered behind the kernels that read them
       const cudaStream_t st = h->stream;
       auto up = [&](auto &buf, const auto *src, size_t count) -> cudaError_t {
@@ -418,24 +397,16 @@ int prepare_checked(kmp_lp_handle *h, uint32_t n, uint32_t m, const uint32_t *xa
         e = up(d_ew, adjwgt, m);
       }
       if (e != cudaSuccess) {
-        rc = fail(e == cudaErrorMemoryAllocation ? KMP_ERR_ALLOC : KMP_ERR_CUDA,
-                  std::string("uploading the graph: ") + cudaGetErrorString(e));
+        return fail(e == cudaErrorMemoryAllocation ? KMP_ERR_ALLOC : KMP_ERR_CUDA,
+                    std::string("uploading the graph: ") + cudaGetErrorString(e));
       }
       xadj = d_xadj.p;
       adjncy = d_adj.p;
       vwgt = vwgt != nullptr ? d_vw.p : nullptr;
       adjwgt = adjwgt != nullptr ? d_ew.p : nullptr;
     }
-    if (rc == KMP_OK) {
-      rc = prepare_impl(h, n, m, xadj, adjncy, vwgt, adjwgt, g, stats);
-    }
-  }
-  if (rc != KMP_OK) {
-    kmp_prepared_destroy(g);
-    return rc;
-  }
-  *out = g;
-  return KMP_OK;
+    return prepare_impl(h, n, m, xadj, adjncy, vwgt, adjwgt, g, stats);
+  });
 }
 
 int finish_impl(kmp_lp_handle *h, const kmp_prepared_graph *g, uint32_t k, const int32_t *max_block_weights,
@@ -443,10 +414,10 @@ int finish_impl(kmp_lp_handle *h, const kmp_prepared_graph *g, uint32_t k, const
   const cudaStream_t st = h->stream;
   const int dev = h->device;
   const uint32_t n = g->n, np = g->np, ni = n - np;
-  CallBuf<uint32_t> d_part, start, out;
-  CallBuf<int32_t> bw, maxw, bw_out;
-  CallBuf<unsigned long long> bad;
-  CallBuf<long long> w, S;
+  PoolBuf<uint32_t> d_part, start, out; // scratch of this call
+  PoolBuf<int32_t> bw, maxw, bw_out;
+  PoolBuf<unsigned long long> bad;
+  PoolBuf<long long> w, S;
   const uint32_t *part = h->label.p;
   if (partition != nullptr) {
     KMP_CUDA(d_part.alloc(np, st, dev));
@@ -476,10 +447,9 @@ int finish_impl(kmp_lp_handle *h, const kmp_prepared_graph *g, uint32_t k, const
     KMP_CUDA(S.alloc(static_cast<size_t>(ni) + 1, st, dev));
     KMP_CUDA(cudaMemsetAsync(S.p, 0, 8, st));
     k_prep_iso_weights<<<grid_for(ni, 256), 256, 0, st>>>(ni, g->vwgt.p + np, w.p);
-    size_t tmp_bytes = 0;
-    KMP_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, w.p, S.p + 1, static_cast<int>(ni), st));
-    KMP_CUDA(h->cub_tmp.ensure(std::max<size_t>(tmp_bytes, 1)));
-    KMP_CUDA(cub::DeviceScan::InclusiveSum(h->cub_tmp.p, tmp_bytes, w.p, S.p + 1, static_cast<int>(ni), st));
+    KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
+      return cub::DeviceScan::InclusiveSum(tmp, bytes, w.p, S.p + 1, static_cast<int>(ni), st);
+    }));
     s_ptr = S.p;
   }
   KMP_CUDA(maxw.alloc(k, st, dev));
@@ -526,24 +496,12 @@ int kmp_prepared_device_arrays(const kmp_prepared_graph *g, const uint32_t **d_x
   if (g == nullptr) {
     return fail(KMP_ERR_INVALID, "null argument");
   }
-  if (d_xadj != nullptr) {
-    *d_xadj = g->xadj.p;
-  }
-  if (d_adjncy != nullptr) {
-    *d_adjncy = g->adjncy.p;
-  }
-  if (d_vwgt != nullptr) {
-    *d_vwgt = g->vwgt.p;
-  }
-  if (d_adjwgt != nullptr) {
-    *d_adjwgt = g->adjwgt.p;
-  }
-  if (d_old_to_new != nullptr) {
-    *d_old_to_new = g->old_to_new.p;
-  }
-  if (d_new_to_old != nullptr) {
-    *d_new_to_old = g->new_to_old.p;
-  }
+  hand_out(d_xadj, g->xadj);
+  hand_out(d_adjncy, g->adjncy);
+  hand_out(d_vwgt, g->vwgt);
+  hand_out(d_adjwgt, g->adjwgt);
+  hand_out(d_old_to_new, g->old_to_new);
+  hand_out(d_new_to_old, g->new_to_old);
   return KMP_OK;
 }
 
@@ -553,21 +511,11 @@ int kmp_prepared_download(const kmp_prepared_graph *g, uint32_t *xadj, uint32_t 
     return fail(KMP_ERR_INVALID, "null argument");
   }
   KMP_CUDA(cudaSetDevice(g->device));
-  if (xadj != nullptr) {
-    KMP_CUDA(cudaMemcpy(xadj, g->xadj.p, (static_cast<size_t>(g->n) + 1) * 4, cudaMemcpyDeviceToHost));
-  }
-  if (adjncy != nullptr && g->m > 0) {
-    KMP_CUDA(cudaMemcpy(adjncy, g->adjncy.p, static_cast<size_t>(g->m) * 4, cudaMemcpyDeviceToHost));
-  }
-  if (vwgt != nullptr && g->vwgt.p != nullptr && g->n > 0) {
-    KMP_CUDA(cudaMemcpy(vwgt, g->vwgt.p, static_cast<size_t>(g->n) * 4, cudaMemcpyDeviceToHost));
-  }
-  if (adjwgt != nullptr && g->adjwgt.p != nullptr && g->m > 0) {
-    KMP_CUDA(cudaMemcpy(adjwgt, g->adjwgt.p, static_cast<size_t>(g->m) * 4, cudaMemcpyDeviceToHost));
-  }
-  if (old_to_new != nullptr && g->n > 0) {
-    KMP_CUDA(cudaMemcpy(old_to_new, g->old_to_new.p, static_cast<size_t>(g->n) * 4, cudaMemcpyDeviceToHost));
-  }
+  KMP_CUDA(copy_out(xadj, g->xadj, static_cast<size_t>(g->n) + 1));
+  KMP_CUDA(copy_out(adjncy, g->adjncy, g->m));
+  KMP_CUDA(copy_out(vwgt, g->vwgt, g->n));
+  KMP_CUDA(copy_out(adjwgt, g->adjwgt, g->m));
+  KMP_CUDA(copy_out(old_to_new, g->old_to_new, g->n));
   return KMP_OK;
 }
 
@@ -613,13 +561,7 @@ void kmp_prepared_destroy(kmp_prepared_graph *g) {
   if (g == nullptr) {
     return;
   }
-  cudaSetDevice(g->device);
-  g->xadj.release();
-  g->adjncy.release();
-  g->old_to_new.release();
-  g->new_to_old.release();
-  g->vwgt.release();
-  g->adjwgt.release();
+  cudaSetDevice(g->device); // the arrays free themselves on this device's pool
   delete g;
 }
 

@@ -193,18 +193,14 @@ __global__ void sp_scatter(uint32_t m, const uint32_t *__restrict__ pos, const u
 
 namespace {
 
-// The new arrays go to `out` (the caller frees them if this fails); g is not modified here.
+// The new arrays go to `out` (they free themselves if this fails); g is not modified here.
 int sparsify_impl(kmp_lp_handle *h, const kmp_coarse_graph *g, uint32_t target_m, uint64_t seed, kmp_coarse_graph *out,
                   kmp_sparsify_stats *stats) {
   using namespace kmp;
   const uint32_t c_n = g->c_n, m = g->c_m;
   cudaStream_t st = h->stream;
   uint32_t launches = 0;
-  if (h->ev_ct0 == nullptr) {
-    KMP_CUDA(cudaEventCreate(&h->ev_ct0));
-    KMP_CUDA(cudaEventCreate(&h->ev_ct1));
-  }
-  KMP_CUDA(cudaEventRecord(h->ev_ct0, st));
+  KMP_CUDA(call_clock_start(h, st));
   KMP_CUDA(out->xadj.alloc(static_cast<size_t>(c_n) + 1, st, h->device));
   int32_t threshold = 0;
   uint32_t smaller = 0, equal = 0, kept = 0, equal_kept = 0;
@@ -259,17 +255,16 @@ int sparsify_impl(kmp_lp_handle *h, const kmp_coarse_graph *g, uint32_t target_m
     // selection's read-back, so that the kept count is read only with the call's final synchronisation.
     KMP_CUDA(out->adjncy.alloc(m - smaller, st, h->device));
     KMP_CUDA(out->adjwgt.alloc(m - smaller, st, h->device));
-    size_t tmp_bytes = 0;
-    KMP_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, pos.p, m + 1, st));
-    KMP_CUDA(h->cub_tmp.ensure(std::max<size_t>(tmp_bytes, 1)));
-    KMP_CUDA(cub::DeviceScan::ExclusiveSum(h->cub_tmp.p, tmp_bytes, pos.p, m + 1, st));
+    KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
+      return cub::DeviceScan::ExclusiveSum(tmp, bytes, pos.p, m + 1, st);
+    }));
     sp_offsets<<<capped(h, grid_for(static_cast<uint64_t>(c_n) + 1, 256)), 256, 0, st>>>(c_n, g->xadj.p, pos.p,
                                                                                          out->xadj.p);
     sp_scatter<<<capped(h, grid_for(m, 256)), 256, 0, st>>>(m, pos.p, g->adjncy.p, w, out->adjncy.p, out->adjwgt.p);
     launches += 3; // + the scan inside CUB
     KMP_CUDA(cudaGetLastError());
   }
-  KMP_CUDA(cudaEventRecord(h->ev_ct1, st));
+  KMP_CUDA(call_clock_stop(h, st));
   if (target_m >= 2) {
     KMP_CUDA(cudaMemcpyAsync(&counts[0], h->ct_rank.p + m, 4, cudaMemcpyDeviceToHost, st));
     KMP_CUDA(cudaMemcpyAsync(&counts[1], h->sp_ctl.p + kSpEqualKept, 4, cudaMemcpyDeviceToHost, st));
@@ -277,8 +272,7 @@ int sparsify_impl(kmp_lp_handle *h, const kmp_coarse_graph *g, uint32_t target_m
   KMP_CUDA(cudaStreamSynchronize(st));
   kept = counts[0];
   equal_kept = counts[1];
-  float ms = 0.f;
-  cudaEventElapsedTime(&ms, h->ev_ct0, h->ev_ct1);
+  const float ms = call_clock_ms(h);
   out->c_m = kept;
   if (stats != nullptr) {
     stats->c_m_before = m;
@@ -323,18 +317,12 @@ int kmp_coarse_sparsify(kmp_lp_handle *h, kmp_coarse_graph *g, uint32_t target_m
   kmp_coarse_graph out;
   const int rc = sparsify_impl(h, g, target_m, seed, &out, stats);
   if (rc != KMP_OK) {
-    out.xadj.release();
-    out.adjncy.release();
-    out.adjwgt.release();
     return rc;
   }
   // the stream is idle (sparsify_impl synchronised it): the old arrays are unused when they are freed
-  g->xadj.release();
-  g->adjncy.release();
-  g->adjwgt.release();
-  g->xadj = out.xadj;
-  g->adjncy = out.adjncy;
-  g->adjwgt = out.adjwgt;
+  g->xadj = std::move(out.xadj);
+  g->adjncy = std::move(out.adjncy);
+  g->adjwgt = std::move(out.adjwgt);
   g->c_m = out.c_m;
   return KMP_OK;
 }

@@ -1,7 +1,7 @@
 // kaminpar_b200: block-induced subgraph extraction and the copy-back of sub-partitions on the device + their C ABI
 // (include/kaminpar_b200_subgraph.h, DESIGN.md §16). Included at the end of kmp_lp.cu after kmp_prepare.cuh: the
 // edge passes find the vertex that owns an edge with the contraction's tile owners (k_tile_owners, owner_of_edge),
-// labels >= k and the k' block weights go through the refiner's bal_block_weights, scratch is CallBuf.
+// labels >= k and the k' block weights go through the refiner's bal_block_weights, scratch is PoolBuf.
 //
 // What it restates (see the header): graph::lazy_extract_subgraphs_preprocessing + graph::extract_subgraph
 // (graphutils/subgraph_extractor.cc:181-324) and graph::copy_subgraph_partitions (:492-533).
@@ -302,8 +302,8 @@ int extract_impl(kmp_lp_handle *h, uint32_t k, kmp_subgraphs *g, kmp_subgraph_st
   uint32_t launches = 0;
   // ---- labels >= k are refused before any [k] array is indexed by one ---------------------------------------
   {
-    CallBuf<int32_t> bw;
-    CallBuf<unsigned long long> bad;
+    PoolBuf<int32_t> bw;
+    PoolBuf<unsigned long long> bad;
     KMP_CUDA(bw.alloc(k, st, dev));
     KMP_CUDA(bad.alloc(1, st, dev));
     KMP_CUDA(cudaMemsetAsync(bw.p, 0, static_cast<size_t>(k) * 4, st));
@@ -334,8 +334,7 @@ int extract_impl(kmp_lp_handle *h, uint32_t k, kmp_subgraphs *g, kmp_subgraph_st
     KMP_CUDA(g->vwgt.alloc(n, st, dev));
   }
   const uint32_t tiles = (m + kTileEdges - 1) / kTileEdges;
-  CallBuf<uint32_t> tile_lo, tile_cnt, tile_base, deg, first_rank, iota, deg_new, edge_pos, delta;
-  size_t tmp_bytes = 0;
+  PoolBuf<uint32_t> tile_lo, tile_cnt, tile_base, deg, first_rank, iota, deg_new, edge_pos, delta;
   // ---- 1. count ---------------------------------------------------------------------------------------------
   KMP_CUDA(deg.alloc(n, st, dev));
   KMP_CUDA(cudaMemsetAsync(deg.p, 0, static_cast<size_t>(n) * 4, st));
@@ -349,10 +348,9 @@ int extract_impl(kmp_lp_handle *h, uint32_t k, kmp_subgraphs *g, kmp_subgraph_st
                                                                                 part, tile_cnt.p, deg.p);
     launches += 2;
     KMP_CUDA(cudaMemsetAsync(tile_cnt.p + tiles, 0, 4, st));
-    KMP_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, tile_cnt.p, tile_base.p, static_cast<int>(tiles) + 1, st));
-    KMP_CUDA(h->cub_tmp.ensure(std::max<size_t>(tmp_bytes, 1)));
-    KMP_CUDA(cub::DeviceScan::ExclusiveSum(h->cub_tmp.p, tmp_bytes, tile_cnt.p, tile_base.p, static_cast<int>(tiles) + 1,
-                                           st));
+    KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
+      return cub::DeviceScan::ExclusiveSum(tmp, bytes, tile_cnt.p, tile_base.p, static_cast<int>(tiles) + 1, st);
+    }));
   }
   // ---- 2. vertex order, offsets, local xadj -----------------------------------------------------------------
   KMP_CUDA(deg_new.alloc(static_cast<size_t>(n) + 1, st, dev));
@@ -362,11 +360,10 @@ int extract_impl(kmp_lp_handle *h, uint32_t k, kmp_subgraphs *g, kmp_subgraph_st
     KMP_CUDA(iota.alloc(n, st, dev));
     bal_iota<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, iota.p);
     const int bits = static_cast<int>(std::max<uint32_t>(1, sub_ceil_log2(k)));
-    KMP_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, part, g->blk.p, iota.p, g->block_nodes.p,
-                                             static_cast<int>(n), 0, bits, st));
-    KMP_CUDA(h->cub_tmp.ensure(std::max<size_t>(tmp_bytes, 1)));
-    KMP_CUDA(cub::DeviceRadixSort::SortPairs(h->cub_tmp.p, tmp_bytes, part, g->blk.p, iota.p, g->block_nodes.p,
-                                             static_cast<int>(n), 0, bits, st));
+    KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
+      return cub::DeviceRadixSort::SortPairs(tmp, bytes, part, g->blk.p, iota.p, g->block_nodes.p, static_cast<int>(n),
+                                             0, bits, st);
+    }));
     k_sub_node_off<<<capped(h, grid_for(static_cast<uint64_t>(k) + 1, 256)), 256, 0, st>>>(n, k, g->blk.p,
                                                                                             g->node_off.p);
     k_sub_map<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, g->blk.p, g->block_nodes.p, g->node_off.p, h->vwgt, deg.p,
@@ -374,12 +371,12 @@ int extract_impl(kmp_lp_handle *h, uint32_t k, kmp_subgraphs *g, kmp_subgraph_st
     launches += 3;
     KMP_CUDA(cudaMemsetAsync(deg_new.p + n, 0, 4, st));
     KMP_CUDA(first_rank.alloc(n, st, dev));
-    KMP_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, deg.p, first_rank.p, static_cast<int>(n), st));
-    KMP_CUDA(h->cub_tmp.ensure(std::max<size_t>(tmp_bytes, 1)));
-    KMP_CUDA(cub::DeviceScan::ExclusiveSum(h->cub_tmp.p, tmp_bytes, deg.p, first_rank.p, static_cast<int>(n), st));
-    KMP_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, deg_new.p, edge_pos.p, static_cast<int>(n) + 1, st));
-    KMP_CUDA(h->cub_tmp.ensure(std::max<size_t>(tmp_bytes, 1)));
-    KMP_CUDA(cub::DeviceScan::ExclusiveSum(h->cub_tmp.p, tmp_bytes, deg_new.p, edge_pos.p, static_cast<int>(n) + 1, st));
+    KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
+      return cub::DeviceScan::ExclusiveSum(tmp, bytes, deg.p, first_rank.p, static_cast<int>(n), st);
+    }));
+    KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
+      return cub::DeviceScan::ExclusiveSum(tmp, bytes, deg_new.p, edge_pos.p, static_cast<int>(n) + 1, st);
+    }));
   } else {
     KMP_CUDA(cudaMemsetAsync(g->node_off.p, 0, (static_cast<size_t>(k) + 1) * 4, st));
   }
@@ -408,17 +405,15 @@ int extract_impl(kmp_lp_handle *h, uint32_t k, kmp_subgraphs *g, kmp_subgraph_st
     ++launches;
   }
   KMP_CUDA(cudaGetLastError());
-  KMP_CUDA(cudaEventRecord(h->ev_ct1, st));
+  KMP_CUDA(call_clock_stop(h, st));
   KMP_CUDA(cudaStreamSynchronize(st));
   if (stats != nullptr) {
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, h->ev_ct0, h->ev_ct1);
     stats->n = n;
     stats->k = k;
     stats->m = m;
     stats->m_internal = m_int;
     stats->kernel_launches = launches;
-    stats->device_ms = ms;
+    stats->device_ms = call_clock_ms(h);
   }
   return KMP_OK;
 }
@@ -445,8 +440,8 @@ int copy_back_impl(kmp_lp_handle *h, const kmp_subgraphs *g, uint32_t k_prime, u
     return fail(KMP_ERR_INVALID, "the sub-block counts do not add up to k_prime (k must be a power of two when "
                                  "k_prime == input_k)");
   }
-  CallBuf<uint32_t> d_k0, d_sub, out;
-  CallBuf<unsigned long long> bad;
+  PoolBuf<uint32_t> d_k0, d_sub, out; // scratch of this call
+  PoolBuf<unsigned long long> bad;
   KMP_CUDA(d_k0.alloc(k0.size(), st, dev));
   KMP_CUDA(cudaMemcpyAsync(d_k0.p, k0.data(), k0.size() * 4, cudaMemcpyHostToDevice, st));
   if (host_sub) {
@@ -546,28 +541,13 @@ int kmp_extract_subgraphs(kmp_lp_handle *h, uint32_t k, const uint32_t *partitio
   if (stats != nullptr) {
     std::memset(stats, 0, sizeof(*stats));
   }
-  if (h->ev_ct0 == nullptr) { // the contraction's event pair: neither call runs inside the other
-    KMP_CUDA(cudaEventCreate(&h->ev_ct0));
-    KMP_CUDA(cudaEventCreate(&h->ev_ct1));
-  }
-  KMP_CUDA(cudaEventRecord(h->ev_ct0, h->stream));
+  KMP_CUDA(call_clock_start(h, h->stream));
   if (partition != nullptr) { // loaded as the handle's labels, as load_partition does
     KMP_CUDA(h->label.ensure(h->n));
     KMP_CUDA(cudaMemcpyAsync(h->label.p, partition, static_cast<size_t>(h->n) * 4, cudaMemcpyHostToDevice, h->stream));
     h->labels_valid = true;
   }
-  kmp_subgraphs *g = new (std::nothrow) kmp_subgraphs();
-  if (g == nullptr) {
-    return fail(KMP_ERR_ALLOC, "out of host memory");
-  }
-  g->device = h->device; // kmp_subgraphs_destroy of a refused call selects this device
-  const int rc = extract_impl(h, k, g, stats);
-  if (rc != KMP_OK) {
-    kmp_subgraphs_destroy(g);
-    return rc;
-  }
-  *out = g;
-  return KMP_OK;
+  return make_result(h, out, [&](kmp_subgraphs *g) { return extract_impl(h, k, g, stats); });
 }
 
 uint32_t kmp_subgraphs_k(const kmp_subgraphs *g) { return g != nullptr ? g->k : 0; }
@@ -579,13 +559,8 @@ int kmp_subgraphs_offsets(const kmp_subgraphs *g, uint32_t *node_off, uint32_t *
     return fail(KMP_ERR_INVALID, "null argument");
   }
   KMP_CUDA(cudaSetDevice(g->device));
-  const size_t bytes = (static_cast<size_t>(g->k) + 1) * 4;
-  if (node_off != nullptr) {
-    KMP_CUDA(cudaMemcpy(node_off, g->node_off.p, bytes, cudaMemcpyDeviceToHost));
-  }
-  if (edge_off != nullptr) {
-    KMP_CUDA(cudaMemcpy(edge_off, g->edge_off.p, bytes, cudaMemcpyDeviceToHost));
-  }
+  KMP_CUDA(copy_out(node_off, g->node_off, static_cast<size_t>(g->k) + 1));
+  KMP_CUDA(copy_out(edge_off, g->edge_off, static_cast<size_t>(g->k) + 1));
   return KMP_OK;
 }
 
@@ -595,25 +570,12 @@ int kmp_subgraphs_download(const kmp_subgraphs *g, uint32_t *xadj, uint32_t *adj
     return fail(KMP_ERR_INVALID, "null argument");
   }
   KMP_CUDA(cudaSetDevice(g->device));
-  const size_t n4 = static_cast<size_t>(g->n) * 4, m4 = static_cast<size_t>(g->m) * 4;
-  if (xadj != nullptr) {
-    KMP_CUDA(cudaMemcpy(xadj, g->xadj.p, (static_cast<size_t>(g->n) + g->k) * 4, cudaMemcpyDeviceToHost));
-  }
-  if (adjncy != nullptr && m4 > 0) {
-    KMP_CUDA(cudaMemcpy(adjncy, g->adjncy.p, m4, cudaMemcpyDeviceToHost));
-  }
-  if (vwgt != nullptr && g->vwgt.p != nullptr && n4 > 0) {
-    KMP_CUDA(cudaMemcpy(vwgt, g->vwgt.p, n4, cudaMemcpyDeviceToHost));
-  }
-  if (adjwgt != nullptr && g->adjwgt.p != nullptr && m4 > 0) {
-    KMP_CUDA(cudaMemcpy(adjwgt, g->adjwgt.p, m4, cudaMemcpyDeviceToHost));
-  }
-  if (mapping != nullptr && n4 > 0) {
-    KMP_CUDA(cudaMemcpy(mapping, g->mapping.p, n4, cudaMemcpyDeviceToHost));
-  }
-  if (block_nodes != nullptr && n4 > 0) {
-    KMP_CUDA(cudaMemcpy(block_nodes, g->block_nodes.p, n4, cudaMemcpyDeviceToHost));
-  }
+  KMP_CUDA(copy_out(xadj, g->xadj, static_cast<size_t>(g->n) + g->k));
+  KMP_CUDA(copy_out(adjncy, g->adjncy, g->m));
+  KMP_CUDA(copy_out(vwgt, g->vwgt, g->n));
+  KMP_CUDA(copy_out(adjwgt, g->adjwgt, g->m));
+  KMP_CUDA(copy_out(mapping, g->mapping, g->n));
+  KMP_CUDA(copy_out(block_nodes, g->block_nodes, g->n));
   return KMP_OK;
 }
 
@@ -624,17 +586,14 @@ int kmp_subgraphs_device_arrays(const kmp_subgraphs *g, const uint32_t **d_xadj,
   if (g == nullptr) {
     return fail(KMP_ERR_INVALID, "null argument");
   }
-  const void *src[8] = {g->xadj.p, g->adjncy.p, g->vwgt.p, g->adjwgt.p, g->mapping.p, g->block_nodes.p, g->node_off.p,
-                        g->edge_off.p};
-  const void **dst[8] = {reinterpret_cast<const void **>(d_xadj),      reinterpret_cast<const void **>(d_adjncy),
-                         reinterpret_cast<const void **>(d_vwgt),      reinterpret_cast<const void **>(d_adjwgt),
-                         reinterpret_cast<const void **>(d_mapping),   reinterpret_cast<const void **>(d_block_nodes),
-                         reinterpret_cast<const void **>(d_node_off),  reinterpret_cast<const void **>(d_edge_off)};
-  for (int i = 0; i < 8; ++i) {
-    if (dst[i] != nullptr) {
-      *dst[i] = src[i];
-    }
-  }
+  hand_out(d_xadj, g->xadj);
+  hand_out(d_adjncy, g->adjncy);
+  hand_out(d_vwgt, g->vwgt);
+  hand_out(d_adjwgt, g->adjwgt);
+  hand_out(d_mapping, g->mapping);
+  hand_out(d_block_nodes, g->block_nodes);
+  hand_out(d_node_off, g->node_off);
+  hand_out(d_edge_off, g->edge_off);
   return KMP_OK;
 }
 
@@ -654,16 +613,7 @@ void kmp_subgraphs_destroy(kmp_subgraphs *g) {
   if (g == nullptr) {
     return;
   }
-  cudaSetDevice(g->device);
-  g->xadj.release();
-  g->adjncy.release();
-  g->mapping.release();
-  g->block_nodes.release();
-  g->blk.release();
-  g->node_off.release();
-  g->edge_off.release();
-  g->vwgt.release();
-  g->adjwgt.release();
+  cudaSetDevice(g->device); // the arrays free themselves on this device's pool
   delete g;
 }
 

@@ -85,13 +85,10 @@ int ubal_round_begin(kmp_lp_handle *h, uint32_t k, unsigned long long *host_ctrl
                                                                 h->ubal_tmask.p, h->bal_ctrl.p);
   ubal_vertex_flags<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, h->label.p, h->vwgt, h->weight.p, h->minw.p,
                                                                  h->ubal_tmask.p, h->bal_flag.p);
-  int rc = bal_cub(h, [&](void *tmp, size_t &bytes) {
+  KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
     return cub::DeviceSelect::Flagged(tmp, bytes, thrust::counting_iterator<uint32_t>(0), h->bal_flag.p, h->bal_cand.p,
                                       h->bal_ctrl.p + 1, static_cast<int>(n), st);
-  });
-  if (rc != KMP_OK) {
-    return rc;
-  }
+  }));
   h->kernel_launches += 3;
   KMP_CUDA(cudaMemcpyAsync(host_ctrl, h->bal_ctrl.p, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
   KMP_CUDA(cudaMemcpyAsync(host_proposals, h->bal_ctr32.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
@@ -115,13 +112,10 @@ int ubal_select(kmp_lp_handle *h, uint32_t k, uint32_t nc, uint32_t call, uint32
   // away costs one select and a read-back, where sorting them into a zero-deficit segment would cost radix passes
   // over nearly every vertex.
   uint32_t *list = h->bal_lists.p; // free again after the evaluation
-  rc = bal_cub(h, [&](void *tmp, size_t &bytes) {
+  KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
     return cub::DeviceSelect::If(tmp, bytes, thrust::counting_iterator<uint32_t>(0), list, h->bal_ctrl.p + 5,
                                  static_cast<int>(nc), UbalHasTarget{h->bal_cand.p, h->label.p, h->bal_target.p}, st);
-  });
-  if (rc != KMP_OK) {
-    return rc;
-  }
+  }));
   unsigned long long nt64 = 0;
   KMP_CUDA(cudaMemcpyAsync(&nt64, h->bal_ctrl.p + 5, sizeof(nt64), cudaMemcpyDeviceToHost, st));
   KMP_CUDA(cudaStreamSynchronize(st));

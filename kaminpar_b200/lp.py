@@ -361,13 +361,23 @@ class LPHandle:
     def __init__(self, cfg: KmpConfig):
         self._lib = load_library()
         self._h = C.c_void_p()
-        # coarse graphs contracted on this handle free their arrays on its stream (kmp_coarse_destroy): while any
-        # is open, close() is deferred to the last one's close -- also when the garbage collector finalises a
-        # reference cycle holding both in arbitrary order
+        # results made on this handle (DeviceResult) free their arrays on its stream: while any is open, close() is
+        # deferred to the last one's close -- also when the garbage collector finalises a reference cycle holding
+        # both in arbitrary order
         self._children = 0
         self._close_pending = False
         _check(self._lib.kmp_lp_create(C.byref(cfg), C.byref(self._h)))
         self._graph_id = None
+
+    def _adopt(self):
+        """A DeviceResult of this handle opened: the handle outlives it."""
+        self._children += 1
+
+    def _release_child(self):
+        """A DeviceResult of this handle closed: a deferred close() runs after the last one."""
+        self._children -= 1
+        if self._close_pending and self._children == 0:
+            self.close()
 
     def close(self):
         if getattr(self, "_children", 0) > 0:
@@ -551,6 +561,38 @@ class LPHandle:
 
     def free_scratch(self):
         _check(self._lib.kmp_lp_free_scratch(self._h))
+
+
+class DeviceResult:
+    """A result object of a graph operation on an LPHandle (a coarse graph, a prepared graph, extracted subgraphs).
+    It owns device memory of the handle's pool, freed on the handle's stream when it closes, so the handle stays open
+    until the last of its results is closed. A subclass names the C symbol that destroys it in `_destroy`."""
+
+    _destroy: str
+
+    def __init__(self, ptr, stats, handle: LPHandle):
+        self._g = ptr
+        self.stats = stats
+        self._handle = handle
+        handle._adopt()
+
+    def _device_ptrs(self, symbol: str, count: int):
+        """The `count` device pointers `symbol` hands out, as integers (0: absent)."""
+        ptrs = [C.c_void_p() for _ in range(count)]
+        _check(getattr(load_library(), symbol)(self._g, *[C.byref(p) for p in ptrs]))
+        return tuple(int(p.value or 0) for p in ptrs)
+
+    def close(self):
+        if getattr(self, "_g", None):
+            getattr(load_library(), self._destroy)(self._g)  # frees on the handle's stream: the handle must still exist
+            self._g = None
+            self._handle._release_child()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 _SCHEDULES = {"sync": 0, "seq_strict": 1}

@@ -54,17 +54,15 @@ def _lib():
     return lib
 
 
-class PreparedGraph:
+class PreparedGraph(lp.DeviceResult):
     """The caller's graph rearranged by degree bucket on the device, its isolated vertices last. The LP sees the
     first `n` (non-isolated) vertices: `set_on(handle)`; `finish(...)` maps a partition of them back to the caller's
     ids with the isolated vertices placed. Owns device memory of the preparing handle's pool, freed on its stream."""
 
-    def __init__(self, ptr, stats: PrepareStats, keepalive: lp.LPHandle):
-        self._g = ptr
-        self.stats = stats
-        self._keepalive = keepalive  # the handle that prepared the graph (owns the stream the arrays are freed on)
-        keepalive._children += 1
-        self._has_vwgt = self._has_adjwgt = False
+    _destroy = "kmp_prepared_destroy"
+
+    def __init__(self, ptr, stats: PrepareStats, handle: lp.LPHandle):
+        super().__init__(ptr, stats, handle)
         ptrs = self.device_arrays()
         self._has_vwgt, self._has_adjwgt = ptrs[2] != 0, ptrs[3] != 0
         self._host = None
@@ -113,9 +111,7 @@ class PreparedGraph:
     def device_arrays(self):
         """(d_xadj, d_adjncy, d_vwgt, d_adjwgt, d_old_to_new, d_new_to_old) as integers (0: absent); valid while this
         object lives."""
-        ptrs = [C.c_void_p() for _ in range(6)]
-        lp._check(_lib().kmp_prepared_device_arrays(self._g, *[C.byref(p) for p in ptrs]))
-        return tuple(int(p.value or 0) for p in ptrs)
+        return self._device_ptrs("kmp_prepared_device_arrays", 6)
 
     def set_on(self, handle: lp.LPHandle):
         """kmp_lp_set_graph_prepared: the handle's graph becomes the n' prepared vertices, marked sorted."""
@@ -142,21 +138,6 @@ class PreparedGraph:
         lp._check(_lib().kmp_prepared_finish(handle._h, self._g, C.c_uint32(int(k)), lp._ptr(mbw), lp._ptr(part),
                                              lp._ptr(out), lp._ptr(bw)))
         return out, bw
-
-    def close(self):
-        if getattr(self, "_g", None):
-            _lib().kmp_prepared_destroy(self._g)  # frees on the handle's stream: the handle must still exist
-            self._g = None
-            k = self._keepalive
-            k._children -= 1
-            if k._close_pending and k._children == 0:
-                k.close()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 def rearrange_by_degree_buckets(handle: lp.LPHandle, graph: CSRGraph) -> PreparedGraph:

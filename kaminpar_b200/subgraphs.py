@@ -56,16 +56,15 @@ def _lib():
     return lib
 
 
-class Subgraphs:
+class Subgraphs(lp.DeviceResult):
     """The k block-induced subgraphs of a handle's graph on the device, in one n + k xadj (block b's local xadj at
     node_off[b] + b), one adjncy and the vertex order block_nodes. Owns device memory of the extracting handle's pool,
     freed on its stream."""
 
-    def __init__(self, ptr, stats: SubgraphStats, keepalive: lp.LPHandle):
-        self._g = ptr
-        self.stats = stats
-        self._keepalive = keepalive  # the handle that extracted the blocks (owns the stream the arrays are freed on)
-        keepalive._children += 1
+    _destroy = "kmp_subgraphs_destroy"
+
+    def __init__(self, ptr, stats: SubgraphStats, handle: lp.LPHandle):
+        super().__init__(ptr, stats, handle)
         ptrs = self.device_arrays()
         self._has_vwgt, self._has_adjwgt = ptrs[2] != 0, ptrs[3] != 0
         self._host = None
@@ -130,9 +129,7 @@ class Subgraphs:
     def device_arrays(self):
         """(d_xadj, d_adjncy, d_vwgt, d_adjwgt, d_mapping, d_block_nodes, d_node_off, d_edge_off) as integers (0:
         absent); valid while this object lives."""
-        ptrs = [C.c_void_p() for _ in range(8)]
-        lp._check(_lib().kmp_subgraphs_device_arrays(self._g, *[C.byref(p) for p in ptrs]))
-        return tuple(int(p.value or 0) for p in ptrs)
+        return self._device_ptrs("kmp_subgraphs_device_arrays", 8)
 
     def device_view(self, b: int):
         """Block b in place as (n_b, m_b, d_xadj, d_adjncy, d_vwgt, d_adjwgt) for LPHandle.set_graph_device: no copy.
@@ -161,21 +158,6 @@ class Subgraphs:
             lp._check(lib.kmp_subgraphs_copy_partitions(handle._h, self._g, C.c_uint32(k_prime), C.c_uint32(input_k),
                                                         lp._ptr(sub), lp._ptr(out), lp._ptr(bw)))
         return out, bw
-
-    def close(self):
-        if getattr(self, "_g", None):
-            _lib().kmp_subgraphs_destroy(self._g)  # frees on the handle's stream: the handle must still exist
-            self._g = None
-            k = self._keepalive
-            k._children -= 1
-            if k._close_pending and k._children == 0:
-                k.close()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 def extract_subgraphs(handle: lp.LPHandle, k: int, partition: Optional[np.ndarray] = None) -> Subgraphs:
