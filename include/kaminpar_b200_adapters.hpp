@@ -23,6 +23,8 @@
 //                      kaminpar-shm/graphutils/permutator.cc:66-91, 236-264, kaminpar.cc:368-445 (DESIGN.md §15)
 //   Subgraphs / extract_subgraphs / copy_subgraph_partitions
 //                      kaminpar-shm/graphutils/subgraph_extractor.cc:181-324, 492-533 (DESIGN.md §16)
+//   GraphReport / validate_graph
+//                      kaminpar-shm/datastructures/csr_graph.cc:266-356 (debug::validate_graph, DESIGN.md §17)
 //
 // Error convention: the reference's path has no error codes (KASSERT aborts); here a non-zero
 // status of the C ABI becomes std::runtime_error. There is no CPU fallback.
@@ -40,6 +42,7 @@
 #include "kaminpar_b200_lp.h"
 #include "kaminpar_b200_prepare.h"
 #include "kaminpar_b200_subgraph.h"
+#include "kaminpar_b200_validate.h"
 
 namespace kaminpar_b200 {
 
@@ -601,6 +604,29 @@ inline void copy_subgraph_partitions(kmp_lp_handle *h, const Subgraphs &subgraph
   }
   detail::check(kmp_subgraphs_copy_partitions(h, subgraphs.device(), k_prime, input_k, sub_partitions.data(),
                                               out.empty() ? nullptr : out.data(), nullptr));
+}
+
+// The report of debug::validate_graph(graph) (csr_graph.cc:266-356) with every edge counted under its first violation
+// and the duplicate neighbours beside it (include/kaminpar_b200_validate.h). valid() is the reference's verdict and
+// message() its warning line for the first violation.
+struct GraphReport : kmp_graph_report {
+  [[nodiscard]] bool is_valid() const { return valid != 0; }
+  [[nodiscard]] std::string message() const {
+    const int len = kmp_graph_report_message(this, nullptr, 0);
+    std::string out(static_cast<std::size_t>(len > 0 ? len : 0) + 1, '\0');
+    kmp_graph_report_message(this, out.data(), out.size());
+    out.resize(out.size() - 1);
+    return out;
+  }
+};
+
+// Validates `graph` on the device, stream and pool of `h` (its graph, labels and call counter are not touched). A
+// malformed graph is a report, not an exception: only a refused call throws.
+inline GraphReport validate_graph(kmp_lp_handle *h, const CSRGraphView &graph) {
+  GraphReport r{};
+  detail::check(kmp_validate_graph(h, graph.n(), graph.m(), graph.nodes.data(), graph.edges.data(),
+                                   graph.edge_weights.empty() ? nullptr : graph.edge_weights.data(), &r));
+  return r;
 }
 
 } // namespace kaminpar_b200

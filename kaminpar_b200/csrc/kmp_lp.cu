@@ -26,11 +26,13 @@
 #include <nccl.h> // types only: the library is dlopen()ed in kmp_lp_dist_init (no link-time dependency)
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
+#include <cub/device/device_segmented_sort.cuh>
 
 #include "../../include/kaminpar_b200_contraction.h"
 #include "../../include/kaminpar_b200_lp.h"
 #include "../../include/kaminpar_b200_prepare.h"
 #include "../../include/kaminpar_b200_subgraph.h"
+#include "../../include/kaminpar_b200_validate.h"
 #include "lp_commit.cuh"
 #include "lp_device.cuh"
 #include "lp_lowgroup.cuh"
@@ -193,6 +195,15 @@ template <typename T> cudaError_t copy_out(T *dst, const PoolBuf<T> &buf, size_t
     return cudaSuccess;
   }
   return cudaMemcpy(dst, buf.p, count * sizeof(T), cudaMemcpyDeviceToHost);
+}
+
+// H2D copy of a caller's host array into a new block of the pool on `st` (count 0: a one-element block, no copy)
+template <typename T> cudaError_t upload(PoolBuf<T> &buf, const T *src, size_t count, cudaStream_t st, int device) {
+  cudaError_t e = buf.alloc(count, st, device);
+  if (e == cudaSuccess && count > 0) {
+    e = cudaMemcpyAsync(buf.p, src, count * sizeof(T), cudaMemcpyHostToDevice, st);
+  }
+  return e;
 }
 
 // the device pointer of a result array (null: unallocated) to a caller's non-null slot
@@ -3118,6 +3129,7 @@ int kmp_lp_step_finish(kmp_lp_handle *h, uint32_t *labels_out, int32_t *block_we
 #include "kmp_underload.cuh"
 #include "kmp_prepare.cuh"
 #include "kmp_subgraph.cuh"
+#include "kmp_validate.cuh"
 
 #ifdef KMP_HUB_PHASE_STAMPS
 // scripts/hub_rate_phases.py: reads (and with reset != 0 zeroes) the rate kernel's 7 phase accumulators

@@ -379,22 +379,15 @@ int prepare_checked(kmp_lp_handle *h, uint32_t n, uint32_t m, const uint32_t *xa
     PoolBuf<int32_t> d_vw, d_ew;
     if (host_input) { // copies on the handle's stream, freed stream-ordered behind the kernels that read them
       const cudaStream_t st = h->stream;
-      auto up = [&](auto &buf, const auto *src, size_t count) -> cudaError_t {
-        cudaError_t e = buf.alloc(count, st, h->device);
-        if (e == cudaSuccess && count > 0) {
-          e = cudaMemcpyAsync(buf.p, src, count * sizeof(*src), cudaMemcpyHostToDevice, st);
-        }
-        return e;
-      };
-      cudaError_t e = up(d_xadj, xadj, static_cast<size_t>(n) + 1);
+      cudaError_t e = upload(d_xadj, xadj, static_cast<size_t>(n) + 1, st, h->device);
       if (e == cudaSuccess) {
-        e = up(d_adj, adjncy, m);
+        e = upload(d_adj, adjncy, m, st, h->device);
       }
       if (e == cudaSuccess && vwgt != nullptr) {
-        e = up(d_vw, vwgt, n);
+        e = upload(d_vw, vwgt, n, st, h->device);
       }
       if (e == cudaSuccess && adjwgt != nullptr) {
-        e = up(d_ew, adjwgt, m);
+        e = upload(d_ew, adjwgt, m, st, h->device);
       }
       if (e != cudaSuccess) {
         return fail(e == cudaErrorMemoryAllocation ? KMP_ERR_ALLOC : KMP_ERR_CUDA,
