@@ -400,7 +400,7 @@ int bal_refuse(kmp_lp_handle *h, BalKind kind) {
   const bool under = kind == BalKind::Underload;
   const char *what = under ? "the underload balancer" : "the overload balancer";
   const char *section = under ? "§12" : "§11";
-  if (h == nullptr || !h->have_graph) {
+  if (h == nullptr || !h->graph.present) {
     return fail(KMP_ERR_INVALID, "no graph set");
   }
   if (h->cfg.schedule == KMP_SCHEDULE_SEQ_STRICT) {
@@ -411,25 +411,25 @@ int bal_refuse(kmp_lp_handle *h, BalKind kind) {
 
 // Scratch of both balancers, grow-only in the handle (kmp_lp_free_scratch releases it).
 int bal_ensure(kmp_lp_handle *h, uint32_t k, uint32_t nc) {
-  const size_t n = std::max<uint32_t>(h->n, 1), kk = std::max<uint32_t>(k, 1), c = std::max<uint32_t>(nc, 1);
-  KMP_CUDA(h->bal_cand.ensure(n));
-  KMP_CUDA(h->bal_flag.ensure(std::max(n, kk)));
-  KMP_CUDA(h->ubal_tmask.ensure(kk));
-  KMP_CUDA(h->bal_over.ensure(kk));
-  KMP_CUDA(h->bal_pbw.ensure(kk));
-  KMP_CUDA(h->bal_under.ensure(kk));
-  KMP_CUDA(h->bal_ctrl.ensure(8));
-  KMP_CUDA(h->bal_ctr32.ensure(4 + kBalMaxRounds));
-  KMP_CUDA(h->bal_target.ensure(c));
-  KMP_CUDA(h->bal_key.ensure(c));
-  KMP_CUDA(h->bal_lists.ensure(2 * c));
-  KMP_CUDA(h->bal_sk_a.ensure(c));
-  KMP_CUDA(h->bal_sk_b.ensure(c));
-  KMP_CUDA(h->bal_sv_a.ensure(c));
-  KMP_CUDA(h->bal_sv_b.ensure(c));
-  KMP_CUDA(h->bal_blk.ensure(c));
-  KMP_CUDA(h->bal_wt.ensure(c));
-  KMP_CUDA(h->bal_prefix.ensure(c));
+  const size_t n = std::max<uint32_t>(h->graph.n, 1), kk = std::max<uint32_t>(k, 1), c = std::max<uint32_t>(nc, 1);
+  KMP_CUDA(h->bal.cand.ensure(n));
+  KMP_CUDA(h->bal.flag.ensure(std::max(n, kk)));
+  KMP_CUDA(h->bal.tmask.ensure(kk));
+  KMP_CUDA(h->bal.over.ensure(kk));
+  KMP_CUDA(h->bal.pbw.ensure(kk));
+  KMP_CUDA(h->bal.under.ensure(kk));
+  KMP_CUDA(h->bal.ctrl.ensure(8));
+  KMP_CUDA(h->bal.ctr32.ensure(4 + kBalMaxRounds));
+  KMP_CUDA(h->bal.target.ensure(c));
+  KMP_CUDA(h->bal.key.ensure(c));
+  KMP_CUDA(h->bal.lists.ensure(2 * c));
+  KMP_CUDA(h->bal.sk_a.ensure(c));
+  KMP_CUDA(h->bal.sk_b.ensure(c));
+  KMP_CUDA(h->bal.sv_a.ensure(c));
+  KMP_CUDA(h->bal.sv_b.ensure(c));
+  KMP_CUDA(h->bal.blk.ensure(c));
+  KMP_CUDA(h->bal.wt.ensure(c));
+  KMP_CUDA(h->bal.prefix.ensure(c));
   return KMP_OK;
 }
 
@@ -438,41 +438,41 @@ int bal_ensure(kmp_lp_handle *h, uint32_t k, uint32_t nc) {
 int bal_evaluate(kmp_lp_handle *h, uint32_t k, uint32_t nc, uint32_t base_tie, bool sort_keys,
                  const uint8_t *tmask = nullptr) {
   BalArgs a{};
-  a.xadj = h->xadj;
-  a.adjncy = h->adjncy;
-  a.vwgt = h->vwgt;
-  a.adjwgt = h->adjwgt;
-  a.label = h->label.p;
-  a.weight = h->weight.p;
-  a.max_w = h->maxw.p;
+  a.xadj = h->graph.xadj;
+  a.adjncy = h->graph.adjncy;
+  a.vwgt = h->graph.vwgt;
+  a.adjwgt = h->graph.adjwgt;
+  a.label = h->lp.label.p;
+  a.weight = h->lp.weight.p;
+  a.max_w = h->lp.maxw.p;
   a.tmask = tmask;
   a.k = k;
   a.base_tie = base_tie;
-  a.cand = h->bal_cand.p;
+  a.cand = h->bal.cand.p;
   a.num_cand = nc;
-  a.warp_list = h->bal_lists.p;
-  a.cta_list = h->bal_lists.p + std::max<uint32_t>(nc, 1);
-  a.tier_count = h->bal_ctr32.p + 2;
-  a.edges = h->bal_ctrl.p + 4;
-  a.target = h->bal_target.p;
-  a.key = h->bal_key.p;
-  a.sort_key = sort_keys ? h->bal_sk_a.p : nullptr;
-  a.sort_val = h->bal_sv_a.p;
-  KMP_CUDA(cudaMemsetAsync(h->bal_ctr32.p + 2, 0, 2 * sizeof(uint32_t), h->stream));
+  a.warp_list = h->bal.lists.p;
+  a.cta_list = h->bal.lists.p + std::max<uint32_t>(nc, 1);
+  a.tier_count = h->bal.ctr32.p + 2;
+  a.edges = h->bal.ctrl.p + 4;
+  a.target = h->bal.target.p;
+  a.key = h->bal.key.p;
+  a.sort_key = sort_keys ? h->bal.sk_a.p : nullptr;
+  a.sort_val = h->bal.sv_a.p;
+  KMP_CUDA(cudaMemsetAsync(h->bal.ctr32.p + 2, 0, 2 * sizeof(uint32_t), h->stream));
   bal_eval_thread<<<capped(h, grid_for(nc, 256)), 256, 0, h->stream>>>(a);
   bal_eval_warp<<<capped(h, grid_for(static_cast<uint64_t>(nc) * 32, kBalWarpsPerCta * 32)), kBalWarpsPerCta * 32, 0,
                   h->stream>>>(a);
   bal_eval_cta<<<capped(h, grid_for(static_cast<uint64_t>(nc) * kBalCtaThreads, kBalCtaThreads, kSMs * 8)), kBalCtaThreads,
                  0, h->stream>>>(a);
-  h->kernel_launches += 3;
+  h->counts.kernel_launches += 3;
   KMP_CUDA(cudaGetLastError());
   return KMP_OK;
 }
 
 // The end of a round of either balancer, after its selection left ns sort words (block << 32 | desc key bits) and
-// candidate indices in bal_sk_a / bal_sv_a: sort them by (block, key desc), scan the weights per block, propose the
-// candidates whose preceding weight in their block is below the block's quota bal_over[b], and commit the proposals
-// with the refiner's ladder, one pass (moves land in bal_ctr32[4 + r]). The overload balancer commits without
+// candidate indices in bal.sk_a / bal.sv_a: sort them by (block, key desc), scan the weights per block, propose the
+// candidates whose preceding weight in their block is below the block's quota bal.over[b], and commit the proposals
+// with the refiner's ladder, one pass (moves land in bal.ctr32[4 + r]). The overload balancer commits without
 // minimum weights: accepted moves never push a target above its maximum. The underload balancer commits with them:
 // the target side keeps every block <= max, the source side keeps every source >= min (targets are underloaded and
 // sources are not, so no block is both).
@@ -483,40 +483,40 @@ int bal_round_tail(kmp_lp_handle *h, BalKind kind, uint32_t k, uint32_t ns, uint
   }
   cudaStream_t st = h->stream;
   KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
-    return cub::DeviceRadixSort::SortPairs(tmp, bytes, h->bal_sk_a.p, h->bal_sk_b.p, h->bal_sv_a.p, h->bal_sv_b.p,
+    return cub::DeviceRadixSort::SortPairs(tmp, bytes, h->bal.sk_a.p, h->bal.sk_b.p, h->bal.sv_a.p, h->bal.sv_b.p,
                                            static_cast<int>(ns), 0, static_cast<int>(end_bit), st);
   }));
-  bal_sorted_weights<<<capped(h, grid_for(ns, 256)), 256, 0, st>>>(ns, h->bal_sk_b.p, h->bal_sv_b.p, h->bal_cand.p, h->vwgt,
-                                                                   h->bal_blk.p, h->bal_wt.p);
+  bal_sorted_weights<<<capped(h, grid_for(ns, 256)), 256, 0, st>>>(ns, h->bal.sk_b.p, h->bal.sv_b.p, h->bal.cand.p, h->graph.vwgt,
+                                                                   h->bal.blk.p, h->bal.wt.p);
   KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
-    return cub::DeviceScan::ExclusiveSumByKey(tmp, bytes, h->bal_blk.p, h->bal_wt.p, h->bal_prefix.p,
+    return cub::DeviceScan::ExclusiveSumByKey(tmp, bytes, h->bal.blk.p, h->bal.wt.p, h->bal.prefix.p,
                                               static_cast<int>(ns), cub::Equality(), st);
   }));
   const bool under = kind == BalKind::Underload;
-  uint32_t *mover_count = h->bal_ctr32.p;
+  uint32_t *mover_count = h->bal.ctr32.p;
   if (under) {
-    ubal_propose<<<capped(h, grid_for(ns, 256)), 256, 0, st>>>(ns, h->bal_blk.p, h->bal_prefix.p, h->bal_over.p,
-                                                               h->bal_sv_b.p, h->bal_cand.p, h->mv_u.p, h->mv_t.p,
+    ubal_propose<<<capped(h, grid_for(ns, 256)), 256, 0, st>>>(ns, h->bal.blk.p, h->bal.prefix.p, h->bal.over.p,
+                                                               h->bal.sv_b.p, h->bal.cand.p, h->commit.mv_u.p, h->commit.mv_t.p,
                                                                mover_count);
   } else {
-    bal_propose<<<capped(h, grid_for(ns, 256)), 256, 0, st>>>(ns, h->bal_blk.p, h->bal_prefix.p, h->bal_over.p,
-                                                              h->bal_sv_b.p, h->bal_cand.p, h->bal_target.p, h->vwgt,
-                                                              h->weight.p, h->maxw.p, h->bal_under.p, h->bal_ctrl.p,
-                                                              sync_base(h->cfg.seed, call, r, SALT_BAL_DRAW), h->mv_u.p,
-                                                              h->mv_t.p, mover_count);
+    bal_propose<<<capped(h, grid_for(ns, 256)), 256, 0, st>>>(ns, h->bal.blk.p, h->bal.prefix.p, h->bal.over.p,
+                                                              h->bal.sv_b.p, h->bal.cand.p, h->bal.target.p, h->graph.vwgt,
+                                                              h->lp.weight.p, h->lp.maxw.p, h->bal.under.p, h->bal.ctrl.p,
+                                                              sync_base(h->cfg.seed, call, r, SALT_BAL_DRAW), h->commit.mv_u.p,
+                                                              h->commit.mv_t.p, mover_count);
   }
   CommitArgs ca = make_commit_args(h, RunCtx{1, k, 0, under, false});
   ca.mover_count = mover_count;
-  ca.next_mover_count = h->bal_ctr32.p + 1; // scratch: nothing reads it
+  ca.next_mover_count = h->bal.ctr32.p + 1; // scratch: nothing reads it
   ca.also_zero = nullptr;
-  ca.moved_count = h->bal_ctr32.p + 4 + r;
+  ca.moved_count = h->bal.ctr32.p + 4 + r;
   ca.base_commit = sync_base(h->cfg.seed, call, r, under ? SALT_UBAL_COMMIT : SALT_BAL_COMMIT);
   ca.stamp = 0;
   const int rc = launch_commit_refine(h, ca, GatheredArgs{nullptr, 1, 0, nullptr}, 1, ns);
   if (rc != KMP_OK) {
     return rc;
   }
-  h->kernel_launches += 5;
+  h->counts.kernel_launches += 5;
   KMP_CUDA(cudaGetLastError());
   return KMP_OK;
 }
@@ -525,22 +525,22 @@ int bal_round_tail(kmp_lp_handle *h, BalKind kind, uint32_t k, uint32_t ns, uint
 // number of proposals of the previous round.
 int bal_round_begin(kmp_lp_handle *h, uint32_t k, unsigned long long *host_ctrl, uint32_t *host_proposals) {
   cudaStream_t st = h->stream;
-  const uint32_t n = h->n;
-  KMP_CUDA(cudaMemsetAsync(h->bal_ctrl.p, 0, 3 * sizeof(unsigned long long), st));
-  bal_block_stats<<<capped(h, grid_for(k, 256)), 256, 0, st>>>(k, h->weight.p, h->maxw.p, h->bal_pbw.p, h->bal_over.p,
-                                                               h->bal_flag.p, h->bal_ctrl.p);
+  const uint32_t n = h->graph.n;
+  KMP_CUDA(cudaMemsetAsync(h->bal.ctrl.p, 0, 3 * sizeof(unsigned long long), st));
+  bal_block_stats<<<capped(h, grid_for(k, 256)), 256, 0, st>>>(k, h->lp.weight.p, h->lp.maxw.p, h->bal.pbw.p, h->bal.over.p,
+                                                               h->bal.flag.p, h->bal.ctrl.p);
   KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
-    return cub::DeviceSelect::Flagged(tmp, bytes, thrust::counting_iterator<uint32_t>(0), h->bal_flag.p, h->bal_under.p,
-                                      h->bal_ctrl.p + 2, static_cast<int>(k), st);
+    return cub::DeviceSelect::Flagged(tmp, bytes, thrust::counting_iterator<uint32_t>(0), h->bal.flag.p, h->bal.under.p,
+                                      h->bal.ctrl.p + 2, static_cast<int>(k), st);
   }));
-  bal_vertex_flags<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, h->label.p, h->bal_over.p, h->bal_flag.p);
+  bal_vertex_flags<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, h->lp.label.p, h->bal.over.p, h->bal.flag.p);
   KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
-    return cub::DeviceSelect::Flagged(tmp, bytes, thrust::counting_iterator<uint32_t>(0), h->bal_flag.p, h->bal_cand.p,
-                                      h->bal_ctrl.p + 1, static_cast<int>(n), st);
+    return cub::DeviceSelect::Flagged(tmp, bytes, thrust::counting_iterator<uint32_t>(0), h->bal.flag.p, h->bal.cand.p,
+                                      h->bal.ctrl.p + 1, static_cast<int>(n), st);
   }));
-  h->kernel_launches += 4;
-  KMP_CUDA(cudaMemcpyAsync(host_ctrl, h->bal_ctrl.p, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-  KMP_CUDA(cudaMemcpyAsync(host_proposals, h->bal_ctr32.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  h->counts.kernel_launches += 4;
+  KMP_CUDA(cudaMemcpyAsync(host_ctrl, h->bal.ctrl.p, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  KMP_CUDA(cudaMemcpyAsync(host_proposals, h->bal.ctr32.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
   KMP_CUDA(cudaStreamSynchronize(st));
   return KMP_OK;
 }
@@ -561,11 +561,11 @@ struct BalResult {
 // balanced weights, min_w: the underload balancer's minimum weights), run rounds until the stop rule, download.
 int bal_run(kmp_lp_handle *h, BalKind kind, uint32_t k, const int32_t *max_w, const int32_t *min_w, const int32_t *pbw,
             uint32_t *partition_inout, int32_t *block_weights_out, BalResult &res) {
-  const uint32_t n = h->n;
+  const uint32_t n = h->graph.n;
   KMP_CUDA(cudaSetDevice(h->device));
-  h->kernel_launches = 0;
+  h->counts.kernel_launches = 0;
   cudaStream_t st = h->stream;
-  KMP_CUDA(cudaEventRecord(h->ev_begin, st));
+  KMP_CUDA(cudaEventRecord(h->streams.ev_begin, st));
   int rc = ensure_scratch(h, 1, k); // the commit's ladder histograms (zeroed), counters, active flags
   if (rc == KMP_OK) {
     rc = prepare_labg(h, k); // the commit writes the packed labels (kmp_lp_refine repacks them on entry)
@@ -580,11 +580,11 @@ int bal_run(kmp_lp_handle *h, BalKind kind, uint32_t k, const int32_t *max_w, co
     return rc;
   }
   if (pbw != nullptr) {
-    KMP_CUDA(cudaMemcpyAsync(h->bal_pbw.p, pbw, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, st));
+    KMP_CUDA(cudaMemcpyAsync(h->bal.pbw.p, pbw, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, st));
   }
-  KMP_CUDA(cudaMemsetAsync(h->bal_ctrl.p, 0, 8 * sizeof(unsigned long long), st));
-  KMP_CUDA(cudaMemsetAsync(h->bal_ctr32.p, 0, (4 + kBalMaxRounds) * sizeof(uint32_t), st));
-  rc = checked_block_weights(h, k, h->bal_ctrl.p + 3);
+  KMP_CUDA(cudaMemsetAsync(h->bal.ctrl.p, 0, 8 * sizeof(unsigned long long), st));
+  KMP_CUDA(cudaMemsetAsync(h->bal.ctr32.p, 0, (4 + kBalMaxRounds) * sizeof(uint32_t), st));
+  rc = checked_block_weights(h, k, h->bal.ctrl.p + 3);
   if (rc != KMP_OK) {
     return rc;
   }
@@ -610,15 +610,15 @@ int bal_run(kmp_lp_handle *h, BalKind kind, uint32_t k, const int32_t *max_w, co
     const uint32_t nc = static_cast<uint32_t>(ctrl[1]);
     res.candidates += nc;
     rc = bal_ensure(h, k, nc);
-    if (rc == KMP_OK && h->mv_u.cap < nc) {
-      KMP_CUDA(h->mv_u.ensure(nc));
-      KMP_CUDA(h->mv_t.ensure(nc));
-      KMP_CUDA(h->acc.ensure(nc));
+    if (rc == KMP_OK && h->commit.mv_u.cap < nc) {
+      KMP_CUDA(h->commit.mv_u.ensure(nc));
+      KMP_CUDA(h->commit.mv_t.ensure(nc));
+      KMP_CUDA(h->commit.acc.ensure(nc));
     }
     if (rc != KMP_OK) {
       return rc;
     }
-    KMP_CUDA(cudaMemsetAsync(h->bal_ctr32.p, 0, sizeof(uint32_t), st)); // this round's proposals
+    KMP_CUDA(cudaMemsetAsync(h->bal.ctr32.p, 0, sizeof(uint32_t), st)); // this round's proposals
     uint32_t ns = nc; // sort words the selection left
     rc = under ? ubal_select(h, k, nc, call, r, &ns)
                : bal_evaluate(h, k, nc, sync_base(h->cfg.seed, call, r, SALT_BAL_TIE), true);
@@ -632,16 +632,16 @@ int bal_run(kmp_lp_handle *h, BalKind kind, uint32_t k, const int32_t *max_w, co
   }
   res.after = ctrl[0];
   if (partition_inout != nullptr && res.before != 0 && n > 0) {
-    KMP_CUDA(cudaMemcpyAsync(partition_inout, h->label.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, st));
+    KMP_CUDA(cudaMemcpyAsync(partition_inout, h->lp.label.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, st));
   }
   if (block_weights_out != nullptr) {
-    KMP_CUDA(cudaMemcpyAsync(block_weights_out, h->weight.p, static_cast<size_t>(k) * 4, cudaMemcpyDeviceToHost, st));
+    KMP_CUDA(cudaMemcpyAsync(block_weights_out, h->lp.weight.p, static_cast<size_t>(k) * 4, cudaMemcpyDeviceToHost, st));
   }
-  KMP_CUDA(cudaMemcpyAsync(res.moved, h->bal_ctr32.p + 4, sizeof(res.moved), cudaMemcpyDeviceToHost, st));
-  KMP_CUDA(cudaMemcpyAsync(&res.edges, h->bal_ctrl.p + 4, sizeof(res.edges), cudaMemcpyDeviceToHost, st));
-  KMP_CUDA(cudaEventRecord(h->ev_end, st));
+  KMP_CUDA(cudaMemcpyAsync(res.moved, h->bal.ctr32.p + 4, sizeof(res.moved), cudaMemcpyDeviceToHost, st));
+  KMP_CUDA(cudaMemcpyAsync(&res.edges, h->bal.ctrl.p + 4, sizeof(res.edges), cudaMemcpyDeviceToHost, st));
+  KMP_CUDA(cudaEventRecord(h->streams.ev_end, st));
   KMP_CUDA(cudaStreamSynchronize(st));
-  cudaEventElapsedTime(&res.device_ms, h->ev_begin, h->ev_end);
+  cudaEventElapsedTime(&res.device_ms, h->streams.ev_begin, h->streams.ev_end);
   return KMP_OK;
 }
 
@@ -659,7 +659,7 @@ int bal_select_all(kmp_lp_handle *h, BalKind kind, uint32_t k, const uint32_t *l
       target_out == nullptr || key_out == nullptr) {
     return fail(KMP_ERR_INVALID, "null argument");
   }
-  const uint32_t n = h->n;
+  const uint32_t n = h->graph.n;
   for (uint32_t u = 0; u < n; ++u) {
     if (labels[u] >= k) {
       return fail(KMP_ERR_INVALID, "labels >= k: not a k-way partition");
@@ -671,37 +671,37 @@ int bal_select_all(kmp_lp_handle *h, BalKind kind, uint32_t k, const uint32_t *l
   if (rc != KMP_OK) {
     return rc;
   }
-  KMP_CUDA(h->label.ensure(n));
-  KMP_CUDA(h->weight.ensure(k));
-  KMP_CUDA(h->maxw.ensure(k));
+  KMP_CUDA(h->lp.label.ensure(n));
+  KMP_CUDA(h->lp.weight.ensure(k));
+  KMP_CUDA(h->lp.maxw.ensure(k));
   if (n > 0) {
-    KMP_CUDA(cudaMemcpyAsync(h->label.p, labels, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, st));
+    KMP_CUDA(cudaMemcpyAsync(h->lp.label.p, labels, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, st));
   }
-  KMP_CUDA(cudaMemcpyAsync(h->weight.p, block_weights, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, st));
-  KMP_CUDA(cudaMemcpyAsync(h->maxw.p, max_w, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, st));
-  KMP_CUDA(cudaMemsetAsync(h->bal_ctrl.p, 0, 8 * sizeof(unsigned long long), st));
+  KMP_CUDA(cudaMemcpyAsync(h->lp.weight.p, block_weights, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, st));
+  KMP_CUDA(cudaMemcpyAsync(h->lp.maxw.p, max_w, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, st));
+  KMP_CUDA(cudaMemsetAsync(h->bal.ctrl.p, 0, 8 * sizeof(unsigned long long), st));
   if (under) { // the target mask
-    KMP_CUDA(h->minw.ensure(k));
-    KMP_CUDA(cudaMemcpyAsync(h->minw.p, min_w, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, st));
-    ubal_block_stats<<<capped(h, grid_for(k, 256)), 256, 0, st>>>(k, h->weight.p, h->minw.p, h->bal_over.p,
-                                                                  h->ubal_tmask.p, h->bal_ctrl.p);
+    KMP_CUDA(h->lp.minw.ensure(k));
+    KMP_CUDA(cudaMemcpyAsync(h->lp.minw.p, min_w, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, st));
+    ubal_block_stats<<<capped(h, grid_for(k, 256)), 256, 0, st>>>(k, h->lp.weight.p, h->lp.minw.p, h->bal.over.p,
+                                                                  h->bal.tmask.p, h->bal.ctrl.p);
   }
   if (n > 0) {
-    bal_iota<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, h->bal_cand.p);
+    bal_iota<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, h->bal.cand.p);
     rc = bal_evaluate(h, k, n, sync_base(h->cfg.seed, call_index, round, under ? SALT_UBAL_TIE : SALT_BAL_TIE), false,
-                      under ? h->ubal_tmask.p : nullptr);
+                      under ? h->bal.tmask.p : nullptr);
     if (rc != KMP_OK) {
       return rc;
     }
     if (under) { // a vertex that may not leave its block keeps it
-      ubal_vertex_flags<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, h->label.p, h->vwgt, h->weight.p, h->minw.p,
-                                                                     h->ubal_tmask.p, h->bal_flag.p);
-      ubal_keep_sources<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, h->bal_flag.p, h->label.p, h->vwgt,
-                                                                     h->bal_target.p, h->bal_key.p);
+      ubal_vertex_flags<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, h->lp.label.p, h->graph.vwgt, h->lp.weight.p, h->lp.minw.p,
+                                                                     h->bal.tmask.p, h->bal.flag.p);
+      ubal_keep_sources<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, h->bal.flag.p, h->lp.label.p, h->graph.vwgt,
+                                                                     h->bal.target.p, h->bal.key.p);
       KMP_CUDA(cudaGetLastError());
     }
-    KMP_CUDA(cudaMemcpyAsync(target_out, h->bal_target.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, st));
-    KMP_CUDA(cudaMemcpyAsync(key_out, h->bal_key.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, st));
+    KMP_CUDA(cudaMemcpyAsync(target_out, h->bal.target.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, st));
+    KMP_CUDA(cudaMemcpyAsync(key_out, h->bal.key.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, st));
   }
   KMP_CUDA(cudaStreamSynchronize(st));
   return KMP_OK;
@@ -743,7 +743,7 @@ int kmp_overload_balance(kmp_lp_handle *h, uint32_t k, const int32_t *max_block_
     stats->overload_after = static_cast<int64_t>(res.after);
     stats->candidates = res.candidates;
     stats->edges_scanned = res.edges;
-    stats->kernel_launches = h->kernel_launches;
+    stats->kernel_launches = h->counts.kernel_launches;
     stats->device_ms = res.device_ms;
   }
   return KMP_OK;

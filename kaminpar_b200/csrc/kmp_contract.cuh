@@ -198,7 +198,7 @@ uint32_t ceil_log2_u32(uint32_t x) { // smallest b with 2^b >= x (x >= 1)
 }
 
 int contract_impl(kmp_lp_handle *h, const uint32_t *clustering, kmp_coarse_graph *cg, kmp_contraction_stats *stats) {
-  const uint32_t n = h->n, m = h->m;
+  const uint32_t n = h->graph.n, m = h->graph.m;
   cudaStream_t st = h->stream;
   uint32_t launches = 0;
   cg->fine_n = n;
@@ -210,14 +210,14 @@ int contract_impl(kmp_lp_handle *h, const uint32_t *clustering, kmp_coarse_graph
     return KMP_OK;
   }
   // scratch lives in the handle (grow-only): no cudaMalloc / cudaFree on the timed path after the first call
-  DevBuf<uint32_t> &d_cl = h->ct_cl, &flags = h->ct_flags, &rank = h->ct_rank;
+  DevBuf<uint32_t> &d_cl = h->ops.ct_cl, &flags = h->ops.ct_flags, &rank = h->ops.ct_rank;
   const uint32_t *cl = nullptr;
   if (clustering != nullptr) {
     KMP_CUDA(d_cl.ensure(n));
     KMP_CUDA(cudaMemcpyAsync(d_cl.p, clustering, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, st));
     cl = d_cl.p;
   } else {
-    cl = h->label.p; // kmp_contract_clustering refused labels of another graph
+    cl = h->lp.label.p; // kmp_contract_clustering refused labels of another graph
   }
   KMP_CUDA(call_clock_start(h, st));
   // ---- 1. mapping ------------------------------------------------------------------------------
@@ -239,29 +239,29 @@ int contract_impl(kmp_lp_handle *h, const uint32_t *clustering, kmp_coarse_graph
   cg->c_n = c_n;
   KMP_CUDA(cg->vwgt.alloc(c_n, st, h->device));
   KMP_CUDA(cudaMemsetAsync(cg->vwgt.p, 0, static_cast<size_t>(c_n) * 4, st));
-  k_map_and_weigh<<<grid_for(n, 256), 256, 0, st>>>(n, cl, rank.p, h->vwgt, cg->mapping.p, cg->vwgt.p);
+  k_map_and_weigh<<<grid_for(n, 256), 256, 0, st>>>(n, cl, rank.p, h->graph.vwgt, cg->mapping.p, cg->vwgt.p);
   launches += 4;
   // ---- 2. edge keys ----------------------------------------------------------------------------
   const uint32_t shift = std::max<uint32_t>(1, ceil_log2_u32(c_n));
   const uint32_t bits = shift + std::max<uint32_t>(1, ceil_log2_u32(c_n));
   unsigned long long cut = 0;
-  DevBuf<unsigned long long> &keys_a = h->pairs_a, &keys_b = h->pairs_b, &counter = h->ct_counter;
-  DevBuf<int32_t> &vals_a = h->ct_vals_a, &vals_b = h->ct_vals_b;
+  DevBuf<unsigned long long> &keys_a = h->ops.pairs_a, &keys_b = h->ops.pairs_b, &counter = h->ops.ct_counter;
+  DevBuf<int32_t> &vals_a = h->ops.ct_vals_a, &vals_b = h->ops.ct_vals_b;
   KMP_CUDA(counter.ensure(2));
   KMP_CUDA(cudaMemsetAsync(counter.p, 0, 16, st));
   if (m > 0) {
     KMP_CUDA(keys_a.ensure(m));
-    if (h->adjwgt != nullptr) {
+    if (h->graph.adjwgt != nullptr) {
       KMP_CUDA(vals_a.ensure(m));
     }
     const uint32_t tiles = (m + kTileEdges - 1) / kTileEdges;
     KMP_CUDA(flags.ensure(static_cast<size_t>(tiles) + 1)); // the leader flags are dead: reuse as tile_lo
-    k_tile_owners<<<grid_for(static_cast<uint64_t>(tiles) + 1, 256), 256, 0, st>>>(n, m, h->xadj, tiles, flags.p);
-    if (h->adjwgt != nullptr) {
-      k_contract_edge_keys<true><<<tiles, 256, 0, st>>>(n, m, h->xadj, flags.p, h->adjncy, h->adjwgt, cg->mapping.p,
+    k_tile_owners<<<grid_for(static_cast<uint64_t>(tiles) + 1, 256), 256, 0, st>>>(n, m, h->graph.xadj, tiles, flags.p);
+    if (h->graph.adjwgt != nullptr) {
+      k_contract_edge_keys<true><<<tiles, 256, 0, st>>>(n, m, h->graph.xadj, flags.p, h->graph.adjncy, h->graph.adjwgt, cg->mapping.p,
                                                         shift, keys_a.p, vals_a.p, counter.p);
     } else {
-      k_contract_edge_keys<false><<<tiles, 256, 0, st>>>(n, m, h->xadj, flags.p, h->adjncy, nullptr, cg->mapping.p,
+      k_contract_edge_keys<false><<<tiles, 256, 0, st>>>(n, m, h->graph.xadj, flags.p, h->graph.adjncy, nullptr, cg->mapping.p,
                                                          shift, keys_a.p, vals_a.p, counter.p);
     }
     launches += 2;
@@ -283,7 +283,7 @@ int contract_impl(kmp_lp_handle *h, const uint32_t *clustering, kmp_coarse_graph
     uint32_t *num_runs = reinterpret_cast<uint32_t *>(counter.p + 1);
     unsigned long long *uk = nullptr; // unique keys: the idle half of the key double buffer
     int32_t *uw = nullptr;            // their weights
-    if (h->adjwgt != nullptr) {
+    if (h->graph.adjwgt != nullptr) {
       cub::DoubleBuffer<int32_t> dv(vals_a.p, vals_b.p);
       KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
         return cub::DeviceRadixSort::SortPairs(tmp, bytes, dk, dv, items, 0, static_cast<int>(bits), st);
@@ -345,7 +345,7 @@ int kmp_contract_clustering(kmp_lp_handle *h, const uint32_t *clustering, kmp_co
   if (h == nullptr || out == nullptr) {
     return fail(KMP_ERR_INVALID, "null argument");
   }
-  if (!h->have_graph) {
+  if (!h->graph.present) {
     return fail(KMP_ERR_INVALID, "no graph set");
   }
   int rc = clustering == nullptr ? refuse_without_labels(h) : KMP_OK;

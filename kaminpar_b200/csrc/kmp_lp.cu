@@ -88,6 +88,15 @@ template <typename T> struct DevBuf {
   DevBuf() = default;
   DevBuf(const DevBuf &) = delete;
   DevBuf &operator=(const DevBuf &) = delete;
+  DevBuf(DevBuf &&o) noexcept : p(std::exchange(o.p, nullptr)), cap(std::exchange(o.cap, 0)) {}
+  DevBuf &operator=(DevBuf &&o) noexcept {
+    if (this != &o) {
+      release();
+      p = std::exchange(o.p, nullptr);
+      cap = std::exchange(o.cap, 0);
+    }
+    return *this;
+  }
   ~DevBuf() { release(); }
   cudaError_t ensure(size_t n) {
     if (n <= cap) {
@@ -213,7 +222,12 @@ template <typename T> void hand_out(const T **dst, const PoolBuf<T> &buf) {
   }
 }
 
-struct OverlayState; // kmp_overlay.cuh
+// The overlay's state on the handle (kmp_overlay.cuh): the stashed clusterings of the last overlay call (pool blocks,
+// kept between calls) and the sort's values
+struct OverlayState {
+  std::vector<PoolBuf<uint32_t>> stash;
+  DevBuf<uint32_t> vals_a, vals_b;
+};
 
 // What one LP run (a clustering or a refinement) passes to its sweeps and commits.
 struct RunCtx {
@@ -225,140 +239,50 @@ struct RunCtx {
 };
 } // namespace
 
+// The handle's buffers are grouped by owner. kmp_lp_free_scratch resets the groups marked "released" (the next call
+// that needs a grow-only buffer allocates it again); it keeps the groups marked "kept" and everything outside the
+// groups, the call counters included.
 struct kmp_lp_handle {
   kmp_lp_config cfg{};
   int device = 0;
   cudaStream_t stream = nullptr;       // stream all work is issued on
-  cudaStream_t owned_stream = nullptr; // the stream this handle created (destroyed with it)
   // The kernel tiers of one sub-round of degree group 3 are independent of each other: they are launched on
   // side streams (fork / join by events) so that their tails and latency-bound phases overlap.
   cudaStream_t sweep_stream = nullptr; // stream the running sweep launch goes to
-  cudaStream_t side_stream[3] = {nullptr, nullptr, nullptr};
-  cudaEvent_t ev_fork = nullptr, ev_join[3] = {nullptr, nullptr, nullptr};
-  cudaEvent_t ev_begin = nullptr, ev_end = nullptr;
-  cudaEvent_t ev_ct0 = nullptr, ev_ct1 = nullptr; // graph-operation timing (call_clock_start), created on first use
+  // the streams and events this handle created, destroyed with it
+  struct Streams {
+    cudaStream_t owned = nullptr; // the handle's stream unless kmp_lp_set_stream replaced it
+    cudaStream_t side[3] = {nullptr, nullptr, nullptr};
+    cudaEvent_t ev_fork = nullptr, ev_join[3] = {nullptr, nullptr, nullptr};
+    cudaEvent_t ev_begin = nullptr, ev_end = nullptr;
+    cudaEvent_t ev_ct0 = nullptr, ev_ct1 = nullptr; // graph-operation timing (call_clock_start), created on first use
+    std::vector<std::pair<cudaEvent_t, cudaEvent_t>> sweep_events; // timing mode (timed_begin), created on first use
+    std::vector<int> sweep_event_group;
+    Streams() = default;
+    Streams(const Streams &) = delete;
+    Streams &operator=(const Streams &) = delete;
+    ~Streams() {
+      for (cudaEvent_t e : {ev_fork, ev_join[0], ev_join[1], ev_join[2], ev_begin, ev_end, ev_ct0, ev_ct1}) {
+        if (e != nullptr) {
+          cudaEventDestroy(e);
+        }
+      }
+      for (auto &p : sweep_events) {
+        cudaEventDestroy(p.first);
+        cudaEventDestroy(p.second);
+      }
+      for (cudaStream_t s : {side[0], side[1], side[2], owned}) {
+        if (s != nullptr) {
+          cudaStreamDestroy(s);
+        }
+      }
+    }
+  } streams;
   bool timing = false;
-  std::vector<std::pair<cudaEvent_t, cudaEvent_t>> sweep_events;
-  std::vector<int> sweep_event_group;
-  uint64_t group_launches[kStatTiers] = {};
   uint32_t grid_cap = 0;        // KMP_GRID_CAP: most CTAs of any launch inside an LP round (0: no cap)
-  // packed (label, stamp) gather array of the sweeps (lp_device.cuh): 4 B per vertex while labels fit 24 bits
-  // (n <= 2^24 clusterer / k <= 2^24 refiner), else 8 B
-  DevBuf<unsigned char> labg;
-  bool p64 = false;
   bool force_p64 = false;
-  bool stamps_ok = false;        // 4 * S sub-rounds fit the stamp code (else push activation only)
-  bool pull_this = true, pull_next = true; // activation mode of the running / the next LP round
-  uint32_t moved_hist[2] = {0xFFFFFFFFu, 0xFFFFFFFFu}; // accepted moves of the two previous rounds
-  uint32_t visited_total = 0;    // vertices on the work lists
-  DevBuf<uint32_t> queue;        // work-queue cursors of the team kernels: [tier][sub-round], zeroed per round
-  DevBuf<uint32_t> t4_hit;       // hub tier: per list entry "a neighbour moved since the last visit"
-  DevBuf<uint32_t> t4_tmp_deg, t4_tmp_beg, t4_tmp_ids; // list building scratch
-  size_t sweep_events_used = 0;
-
-  // graph
-  uint32_t n = 0, m = 0;
-  const uint32_t *xadj = nullptr;
-  const uint32_t *adjncy = nullptr;
-  const int32_t *vwgt = nullptr;
-  const int32_t *adjwgt = nullptr;
-  bool adjncy_16b = true; // adjncy starts on a 16-byte boundary: the hub tier may stage it with bulk copies
-  DevBuf<uint32_t> own_xadj, own_adjncy;
-  DevBuf<int32_t> own_vwgt, own_adjwgt;
-  bool have_graph = false;
-  uint64_t graph_epoch = 0; // counts set_graph calls: a kmp_subgraphs knows which graph it was extracted from
-  uint32_t max_degree = 0;
-  uint32_t num_isolated = 0;
-
-  // work lists: order[] holds the vertices of (group g, sub-round s) contiguously
-  DevBuf<uint32_t> order;
-  std::vector<uint32_t> list_off; // kNumGroups*S + 1 (+1 tail bucket for unvisited vertices)
-  uint32_t max_list = 0;
-  uint32_t lists_S = 0, lists_G = 0, lists_thr = 0;
-  int lists_seed = 0;
-  bool lists_valid = false;
-
-  // state
-  DevBuf<uint32_t> label, favored, communities;
-  // label[] belongs to the current graph: set by a completed clustering, kmp_lp_upload_partition and a refine or
-  // balancer call given a partition; cleared by a new graph and by kmp_lp_free_scratch. The calls that read the
-  // labels on the device (a NULL partition or clustering) refuse while it is clear.
-  bool labels_valid = false;
-  DevBuf<int32_t> weight, maxw, minw;
-  DevBuf<uint8_t> active;
-  // scratch
-  DevBuf<uint32_t> mv_u, mv_t, cslot, slotmap;
-  DevBuf<uint8_t> acc;
-  DevBuf<int32_t> incoming, chist, hist, jmin, out_cur, out_delta, ohist, ojmin;
-  DevBuf<uint32_t> ctr32; // [0] mover_count [1] moved_count (per iteration) [2] misc
-  DevBuf<unsigned long long> ctr64; // [0] edges [1] nodes [2] proposals
-  // hub tier ("t4" in these names is historical): per list entry its first bucket (wave-relative), the
-  // (entry, chunk) work items of the scatter pass and the (entry, bucket) items of the select pass; all per sub-round
-  DevBuf<uint32_t> t4_table_off, t4_item_entry, t4_item_chunk, t4_sel_entry, t4_sel_piece, t4_sel_begin;
-  DevBuf<uint32_t> t4_item_u, t4_item_beg, t4_item_deg; // static per item: vertex, xadj[u], degree
-  std::vector<uint32_t> t4_item_off, t4_sel_off; // S + 1
-  // A sub-round's hubs are processed in waves whose bucket regions together stay below hub_wave_slots entries
-  // (a memory bound: every wave reuses the same regions, cursors and overflow list).
-  struct HubWave {
-    uint32_t item_lo, item_hi, sel_lo, sel_hi; // absolute ranges in the t4_item_* / t4_sel_* arrays
-  };
-  std::vector<HubWave> t4_waves;
-  std::vector<uint32_t> t4_wave_off; // S + 1
   uint64_t hub_wave_slots = 1ull << 28; // 2 GiB of packed entries (KMP_HUB_WAVE_SLOTS overrides, for experiments)
-  DevBuf<Cand> t4_part_best, t4_part_fav;
-  uint64_t t4_max_slots = 0;
-  uint64_t t4_max_wave_edges = 0; // largest adjacency volume of a wave = capacity of the overflow list
   uint32_t hub_bucket_cap = kBucketCap, hub_sel_limit = 0; // KMP_HUB_BUCKET_CAP / KMP_HUB_SEL_LIMIT (tests: force the overflow paths)
-  DevBuf<unsigned long long> hub_tab; // bucket regions: kBucketCap packed (key << 32 | rating) entries each
-  DevBuf<uint32_t> hub_cursor;        // per bucket: entries appended in the running sub-round
-  DevBuf<HubOverflow> hub_ovf;
-  // clusterer hub path (gather + rate): per list entry the start of its row in hub_lab (sub-round-relative) and its
-  // first rate item result; the (entry, hash class) rate items of each sub-round, largest degree first
-  DevBuf<uint32_t> t4_lab_off, t4_rate_begin, t4_rate_entry, t4_rate_cls;
-  // unit edge weights: per list entry the start of its chunks' class offsets in hub_cls (sub-round-relative)
-  DevBuf<uint32_t> t4_cls_off;
-  uint64_t t4_max_subround_cls = 0;
-  DevBuf<uint16_t> hub_cls; // class offsets of the running sub-round's staged chunks (hub_sort_classes + 1 each)
-  std::vector<uint32_t> t4_rate_off; // S + 1
-  uint64_t t4_max_subround_edges = 0;
-  DevBuf<uint32_t> hub_lab; // staged neighbour labels of the running sub-round's hubs (4 B per edge)
-  uint32_t mover_cap = 0;
-  uint32_t cur_subround = 0; // hashed class of the running sub-round
-  uint32_t cur_sg = 0;       // running sub-round index in [0, 4 * S): queue cursor and stamp code
-  DevBuf<uint8_t> sort_keys_in, sort_keys_out;
-  DevBuf<uint32_t> sort_vals_in;
-  DevBuf<unsigned char> cub_tmp;
-  DevBuf<unsigned long long> pairs_a, pairs_b; // two-hop sort; contraction: edge keys (double buffer)
-  // contraction scratch (kmp_contract.cuh), grow-only like the rest
-  DevBuf<int32_t> ct_vals_a, ct_vals_b;
-  DevBuf<uint32_t> ct_flags, ct_rank, ct_cl;
-  DevBuf<unsigned long long> ct_counter;
-  DevBuf<uint32_t> sp_ctl; // sparsification (kmp_sparsify.cuh): radix-select bins, select state, kept counter
-  // overlay (kmp_overlay.cuh): the stashed clusterings of the last overlay call and the sort's values. The stash is
-  // released by set_graph and kmp_lp_free_scratch, the rest by kmp_lp_free_scratch.
-  OverlayState *ov = nullptr;
-  bool slot_state_clean = false; // incoming/slotmap/chist zeroed for current n
-
-  // schedule KMP_SCHEDULE_SEQ_STRICT (lp_strict.cuh): sequential engine state
-  bool graph_sorted = false; // CSRGraph::sorted() of the current graph (kmp_lp_set_graph_sorted)
-  bool strict_seeded = false;
-  DevBuf<int32_t> st_slot, st_ent_val, st_slot2, st_ent2_val, st_concurrent;
-  DevBuf<uint32_t> st_ent_key, st_ent2_key, st_used, st_second, st_tie_best, st_tie_fav, st_chunks, st_sub_perm,
-      st_match, st_buckets;
-  DevBuf<kmp_strict::Rng> st_rng;
-  DevBuf<kmp_strict::Stats> st_stats;
-
-  uint32_t call_counter = 0;
-  uint64_t kernel_launches = 0, sweep_launches = 0;
-  uint32_t pull_rounds = 0, push_rounds = 0;
-  // frontier sharding (one process per GPU): this rank sweeps slice `rank` of `world` of every list
-  uint32_t rank = 0, world = 1;
-  // NCCL communicator of the sharded run (kmp_lp_dist_init): proposals are all-gathered per sub-round on
-  // the handle's stream, inside kmp_lp_cluster / kmp_lp_refine
-  ncclComm_t comm = nullptr;
-  DevBuf<uint32_t> dist_send, dist_recv;
-  uint32_t *direct_send = nullptr; // set while the sweeps of a sharded sub-round write into the send buffer
-  uint32_t direct_cap = 0;
   // cooperative single-launch commit of a sub-round (lp_commit.cuh commit_cluster_fused / commit_refine_fused)
   DevBuf<unsigned> grid_bar; // [0] arrivals, [1] generation
   int fused_blocks = 0;      // co-resident CTAs of the clusterer's kernel
@@ -368,61 +292,217 @@ struct kmp_lp_handle {
   // resident CTAs of each sweep_team instantiation on the device, [MODE][EW][P64][team size 32 / 128 / 512 / 1024]:
   // a larger grid only adds CTAs that start after the work queue is drained
   uint32_t team_grid[2][2][2][4] = {};
-  // stepping API state: the open run (between kmp_lp_step_begin_* and kmp_lp_step_finish) and its LP round
-  RunCtx step{};
-  bool step_open = false;
-  uint32_t step_iter = 0;
-  uint32_t mover_parity = 0; // proposal counter in use: ctr32[0] (parity 0) or ctr32[3] (parity 1)
-  bool stepping = false; // proposals are accumulated by kmp_lp_step_commit, not by the sweep kernels
+
+  uint32_t call_counter = 0; // clusterings computed on this handle: the sync schedule's call index
   // overload and underload balancers (kmp_balance.cuh, kmp_underload.cuh): one call counter each, so that LP calls
-  // and either balancer hash the same with or without the other; one set of scratch
+  // and either balancer hash the same with or without the other
   uint32_t bal_calls = 0, ubal_calls = 0;
-  DevBuf<uint32_t> bal_cand, bal_under, bal_ctr32, bal_target, bal_lists, bal_sv_a, bal_sv_b, bal_blk;
-  // bal_over[b]: the quota a block's segment of sorted candidates is selected against (overload of b, or the
-  // underload balancer's deficit of target b)
-  DevBuf<int32_t> bal_over, bal_pbw, bal_wt, bal_prefix;
-  DevBuf<uint8_t> bal_flag, ubal_tmask;
-  DevBuf<float> bal_key;
-  // bal_ctrl: [0] total over- / underload [1] candidates [2] |U| (underloaded blocks) [3] bad labels [4] edges
-  //           [5] candidates with a target
-  // bal_ctr32: [0] movers [1] scratch [2..3] tier counts [4 + r] moved in round r
-  DevBuf<unsigned long long> bal_ctrl, bal_sk_a, bal_sk_b;
+
+  // per-call counters of kmp_lp_stats, reset by begin_call
+  struct CallCounters {
+    uint64_t kernel_launches = 0, sweep_launches = 0;
+    uint32_t pull_rounds = 0, push_rounds = 0;
+    size_t sweep_events_used = 0;
+    uint64_t group_launches[kStatTiers] = {};
+  } counts;
+
+  // the graph: the caller's device arrays or the handle's own copies (own_*); kept
+  struct Graph {
+    uint32_t n = 0, m = 0;
+    const uint32_t *xadj = nullptr;
+    const uint32_t *adjncy = nullptr;
+    const int32_t *vwgt = nullptr;
+    const int32_t *adjwgt = nullptr;
+    bool adjncy_16b = true; // adjncy starts on a 16-byte boundary: the hub tier may stage it with bulk copies
+    DevBuf<uint32_t> own_xadj, own_adjncy;
+    DevBuf<int32_t> own_vwgt, own_adjwgt;
+    bool present = false;
+    uint64_t epoch = 0; // counts set_graph calls: a kmp_subgraphs knows which graph it was extracted from
+    uint32_t max_degree = 0;
+    uint32_t num_isolated = 0;
+    bool sorted = false; // CSRGraph::sorted() of the current graph (kmp_lp_set_graph_sorted)
+  } graph;
+
+  // the graph's work lists (ensure_lists): order[] holds the vertices of (group g, sub-round s) contiguously; kept
+  struct WorkLists {
+    DevBuf<uint32_t> order;
+    std::vector<uint32_t> off; // kNumGroups*S + 1 (+1 tail bucket for unvisited vertices)
+    DevBuf<uint32_t> queue;    // work-queue cursors of the team kernels: [tier][sub-round], zeroed per round
+    uint32_t max_list = 0;
+    uint32_t mover_cap = 0;
+    uint32_t visited_total = 0; // vertices on the work lists
+    bool stamps_ok = false;     // 4 * S sub-rounds fit the stamp code (else push activation only)
+    // the sync_subrounds, sync_granule_log2, large_degree_threshold and seed they were built for
+    uint32_t S = 0, G = 0, thr = 0;
+    int seed = 0;
+    bool valid = false;
+  } lists;
+
+  // temporaries of ensure_lists: the list-key sort and the hub degrees; released
+  struct ListScratch {
+    DevBuf<uint8_t> sort_keys_in, sort_keys_out;
+    DevBuf<uint32_t> sort_vals_in;
+    DevBuf<uint32_t> hub_deg, hub_beg, hub_ids;
+  } list_tmp;
+
+  // hub tier metadata of the work lists (build_hub_meta): per list entry its first bucket (wave-relative), the
+  // (entry, chunk) work items of the scatter pass and the (entry, bucket) items of the select pass; all per sub-round.
+  // Kept.
+  struct HubMeta {
+    DevBuf<uint32_t> hit; // per list entry "a neighbour moved since the last visit"
+    DevBuf<uint32_t> table_off, item_entry, item_chunk, sel_entry, sel_piece, sel_begin;
+    DevBuf<uint32_t> item_u, item_beg, item_deg; // static per item: vertex, xadj[u], degree
+    std::vector<uint32_t> item_off, sel_off;     // S + 1
+    // A sub-round's hubs are processed in waves whose bucket regions together stay below hub_wave_slots entries
+    // (a memory bound: every wave reuses the same regions, cursors and overflow list).
+    struct Wave {
+      uint32_t item_lo, item_hi, sel_lo, sel_hi; // absolute ranges in the item_* / sel_* arrays
+    };
+    std::vector<Wave> waves;
+    std::vector<uint32_t> wave_off; // S + 1
+    DevBuf<Cand> part_best, part_fav;
+    uint64_t max_slots = 0;
+    uint64_t max_wave_edges = 0; // largest adjacency volume of a wave = capacity of the overflow list
+    // clusterer hub path (gather + rate): per list entry the start of its row in hub_tmp.lab (sub-round-relative) and
+    // its first rate item result; the (entry, hash class) rate items of each sub-round, largest degree first
+    DevBuf<uint32_t> lab_off, rate_begin, rate_entry, rate_cls;
+    // unit edge weights: per list entry the start of its chunks' class offsets in hub_tmp.cls (sub-round-relative)
+    DevBuf<uint32_t> cls_off;
+    uint64_t max_subround_cls = 0;
+    std::vector<uint32_t> rate_off; // S + 1
+    uint64_t max_subround_edges = 0;
+  } hub;
+
+  // hub tier scratch of the running sub-round; released
+  struct HubScratch {
+    DevBuf<unsigned long long> tab; // bucket regions: kBucketCap packed (key << 32 | rating) entries each
+    DevBuf<uint32_t> cursor;        // per bucket: entries appended in the running sub-round
+    DevBuf<HubOverflow> ovf;
+    DevBuf<uint16_t> cls; // class offsets of the running sub-round's staged chunks (hub_sort_classes + 1 each)
+    DevBuf<uint32_t> lab; // staged neighbour labels of the running sub-round's hubs (4 B per edge)
+  } hub_tmp;
+
+  // LP labels and weights; released
+  struct LpState {
+    DevBuf<uint32_t> label, favored, communities;
+    // label[] belongs to the current graph: set by a completed clustering, kmp_lp_upload_partition and a refine or
+    // balancer call given a partition; cleared by a new graph and by kmp_lp_free_scratch. The calls that read the
+    // labels on the device (a NULL partition or clustering) refuse while it is clear.
+    bool labels_valid = false;
+    DevBuf<int32_t> weight, maxw, minw;
+    DevBuf<uint8_t> active;
+    // packed (label, stamp) gather array of the sweeps (lp_device.cuh): 4 B per vertex while labels fit 24 bits
+    // (n <= 2^24 clusterer / k <= 2^24 refiner), else 8 B (round.p64)
+    DevBuf<unsigned char> labg;
+  } lp;
+
+  // LP commit scratch, and the temporary storage of every CUB call (cub_call); released
+  struct CommitScratch {
+    DevBuf<uint32_t> mv_u, mv_t, cslot, slotmap;
+    DevBuf<uint8_t> acc;
+    DevBuf<int32_t> incoming, chist, hist, jmin, out_cur, out_delta, ohist, ojmin;
+    DevBuf<uint32_t> ctr32; // [0] mover_count [1] moved_count (per iteration) [2] misc
+    DevBuf<unsigned long long> ctr64; // [0] edges [1] nodes [2] proposals
+    DevBuf<unsigned char> cub_tmp;
+    bool slot_state_clean = false; // incoming/slotmap/chist zeroed for current n
+  } commit;
+
+  // the running LP round; kept
+  struct Round {
+    bool p64 = false;
+    bool pull_this = true, pull_next = true; // activation mode of the running / the next LP round
+    uint32_t moved_hist[2] = {0xFFFFFFFFu, 0xFFFFFFFFu}; // accepted moves of the two previous rounds
+    uint32_t cur_subround = 0; // hashed class of the running sub-round
+    uint32_t cur_sg = 0;       // running sub-round index in [0, 4 * S): queue cursor and stamp code
+    uint32_t mover_parity = 0; // proposal counter in use: ctr32[0] (parity 0) or ctr32[3] (parity 1)
+    bool stepping = false; // proposals are accumulated by kmp_lp_step_commit, not by the sweep kernels
+  } round;
+
+  // scratch of the graph operations (contraction, sparsification, overlay; pairs_a/b also the two-hop sort); released
+  struct OpScratch {
+    DevBuf<unsigned long long> pairs_a, pairs_b; // two-hop sort; contraction: edge keys (double buffer)
+    DevBuf<int32_t> ct_vals_a, ct_vals_b; // contraction (kmp_contract.cuh)
+    DevBuf<uint32_t> ct_flags, ct_rank, ct_cl;
+    DevBuf<unsigned long long> ct_counter;
+    DevBuf<uint32_t> sp_ctl; // sparsification (kmp_sparsify.cuh): radix-select bins, select state, kept counter
+    OverlayState ov;         // set_graph releases its stash, which belongs to the previous graph
+  } ops;
+
+  // scratch of both balancers (kmp_balance.cuh, kmp_underload.cuh); released
+  struct BalScratch {
+    DevBuf<uint32_t> cand, under, ctr32, target, lists, sv_a, sv_b, blk;
+    // over[b]: the quota a block's segment of sorted candidates is selected against (overload of b, or the
+    // underload balancer's deficit of target b)
+    DevBuf<int32_t> over, pbw, wt, prefix;
+    DevBuf<uint8_t> flag, tmask; // tmask: the underload balancer's allowed targets
+    DevBuf<float> key;
+    // ctrl: [0] total over- / underload [1] candidates [2] |U| (underloaded blocks) [3] bad labels [4] edges
+    //       [5] candidates with a target
+    // ctr32: [0] movers [1] scratch [2..3] tier counts [4 + r] moved in round r
+    DevBuf<unsigned long long> ctrl, sk_a, sk_b;
+  } bal;
+
+  // schedule KMP_SCHEDULE_SEQ_STRICT (lp_strict.cuh): sequential engine state and its per-object RNG; kept
+  struct Strict {
+    bool seeded = false;
+    DevBuf<int32_t> slot, ent_val, slot2, ent2_val, concurrent;
+    DevBuf<uint32_t> ent_key, ent2_key, used, second, tie_best, tie_fav, chunks, sub_perm, match, buckets;
+    DevBuf<kmp_strict::Rng> rng;
+    DevBuf<kmp_strict::Stats> stats;
+  } strict;
+
+  // frontier sharding (one process per GPU): this rank sweeps slice `rank` of `world` of every list. The NCCL
+  // communicator of the sharded run (kmp_lp_dist_init) all-gathers the proposals per sub-round on the handle's
+  // stream, inside kmp_lp_cluster / kmp_lp_refine. Kept.
+  struct Dist {
+    uint32_t rank = 0, world = 1;
+    ncclComm_t comm = nullptr;
+    DevBuf<uint32_t> send, recv;
+    uint32_t *direct_send = nullptr; // set while the sweeps of a sharded sub-round write into the send buffer
+    uint32_t direct_cap = 0;
+  } dist;
+
+  // stepping API: the open run (between kmp_lp_step_begin_* and kmp_lp_step_finish) and its LP round
+  struct Stepping {
+    RunCtx run{};
+    bool open = false;
+    uint32_t iter = 0;
+  } step;
 };
 
 namespace {
-void overlay_release(kmp_lp_handle *h, bool scratch); // kmp_overlay.cuh
 
 // A CUB device-wide call in its two phases: call(nullptr, bytes) asks for the temporary storage, call(tmp, bytes) runs
-// on h->cub_tmp grown to it (CUB never asks for 0 bytes, so tmp is never null and the second call is never a query).
+// on h->commit.cub_tmp grown to it (CUB never asks for 0 bytes, so tmp is never null and the second call is never a query).
 template <typename Fn> cudaError_t cub_call(kmp_lp_handle *h, Fn &&call) {
   size_t bytes = 0;
   cudaError_t e = call(static_cast<void *>(nullptr), bytes);
   if (e == cudaSuccess) {
-    e = h->cub_tmp.ensure(bytes);
+    e = h->commit.cub_tmp.ensure(bytes);
   }
-  return e != cudaSuccess ? e : call(static_cast<void *>(h->cub_tmp.p), bytes);
+  return e != cudaSuccess ? e : call(static_cast<void *>(h->commit.cub_tmp.p), bytes);
 }
 
 // Device time of one graph-operation call (contraction, sparsification, overlay, preparation, subgraph extraction) on
 // the handle's event pair ev_ct0 / ev_ct1, created on first use. None of these calls runs inside another, and the pair
 // is not ev_begin / ev_end, which may bracket an open stepping call.
 cudaError_t call_clock_start(kmp_lp_handle *h, cudaStream_t st) {
-  if (h->ev_ct0 == nullptr) {
-    cudaError_t e = cudaEventCreate(&h->ev_ct0);
+  if (h->streams.ev_ct0 == nullptr) {
+    cudaError_t e = cudaEventCreate(&h->streams.ev_ct0);
     if (e == cudaSuccess) {
-      e = cudaEventCreate(&h->ev_ct1);
+      e = cudaEventCreate(&h->streams.ev_ct1);
     }
     if (e != cudaSuccess) {
       return e;
     }
   }
-  return cudaEventRecord(h->ev_ct0, st);
+  return cudaEventRecord(h->streams.ev_ct0, st);
 }
-cudaError_t call_clock_stop(kmp_lp_handle *h, cudaStream_t st) { return cudaEventRecord(h->ev_ct1, st); }
+cudaError_t call_clock_stop(kmp_lp_handle *h, cudaStream_t st) { return cudaEventRecord(h->streams.ev_ct1, st); }
 // after the caller has waited for the stop event (on the event or on its stream)
 float call_clock_ms(const kmp_lp_handle *h) {
   float ms = 0.f;
-  cudaEventElapsedTime(&ms, h->ev_ct0, h->ev_ct1);
+  cudaEventElapsedTime(&ms, h->streams.ev_ct0, h->streams.ev_ct1);
   return ms;
 }
 
@@ -874,71 +954,71 @@ template <int MODE, bool EW, bool P64> cudaError_t launch_sweep_t(kmp_lp_handle 
     break;
   default: {
     HubArgs hb{};
-    const uint32_t s_idx = h->cur_subround;
-    const uint32_t S = h->lists_S;
-    const uint32_t first = h->list_off[kHubTier * S + s_idx] - h->list_off[kHubTier * S];
+    const uint32_t s_idx = h->round.cur_subround;
+    const uint32_t S = h->lists.S;
+    const uint32_t first = h->lists.off[kHubTier * S + s_idx] - h->lists.off[kHubTier * S];
     hb.sel_limit = h->hub_sel_limit;
-    hb.rank = h->rank;
-    hb.world = h->world;
-    hb.hit = h->t4_hit.p + first;
+    hb.rank = h->dist.rank;
+    hb.world = h->dist.world;
+    hb.hit = h->hub.hit.p + first;
     if constexpr (MODE == 0) {
       // gather the labels of the sub-round's hub edges once, then rate every (hub, hash class) item in one CTA
-      const uint32_t ilo = h->t4_item_off[s_idx], ihi = h->t4_item_off[s_idx + 1];
-      hb.item_entry = h->t4_item_entry.p + ilo;
-      hb.item_chunk = h->t4_item_chunk.p + ilo;
-      hb.item_u = h->t4_item_u.p + ilo;
-      hb.item_beg = h->t4_item_beg.p + ilo;
-      hb.item_deg = h->t4_item_deg.p + ilo;
+      const uint32_t ilo = h->hub.item_off[s_idx], ihi = h->hub.item_off[s_idx + 1];
+      hb.item_entry = h->hub.item_entry.p + ilo;
+      hb.item_chunk = h->hub.item_chunk.p + ilo;
+      hb.item_u = h->hub.item_u.p + ilo;
+      hb.item_beg = h->hub.item_beg.p + ilo;
+      hb.item_deg = h->hub.item_deg.p + ilo;
       hb.num_items = ihi - ilo;
-      hb.lab = h->hub_lab.p;
-      hb.lab_off = h->t4_lab_off.p + first;
+      hb.lab = h->hub_tmp.lab.p;
+      hb.lab_off = h->hub.lab_off.p + first;
       if constexpr (!EW) {
-        hb.cls = h->hub_cls.p;
-        hb.cls_off = h->t4_cls_off.p + first;
+        hb.cls = h->hub_tmp.cls.p;
+        hb.cls_off = h->hub.cls_off.p + first;
       }
       sweep_hub_gather<P64><<<capped(h, std::min<uint32_t>(hb.num_items, kSMs * 8)), 256, 0, h->sweep_stream>>>(a, hb);
-      const uint32_t rlo = h->t4_rate_off[s_idx], rhi = h->t4_rate_off[s_idx + 1];
-      hb.item_entry = h->t4_rate_entry.p + rlo;
-      hb.item_cls = h->t4_rate_cls.p + rlo;
+      const uint32_t rlo = h->hub.rate_off[s_idx], rhi = h->hub.rate_off[s_idx + 1];
+      hb.item_entry = h->hub.rate_entry.p + rlo;
+      hb.item_cls = h->hub.rate_cls.p + rlo;
       hb.num_items = rhi - rlo;
-      hb.sel_begin = h->t4_rate_begin.p + first;
-      hb.part_best = h->t4_part_best.p;
-      hb.part_fav = h->t4_part_fav.p;
-      hb.queue = h->ctr32.p + 64 + s_idx; // zeroed with the other per-round counters
+      hb.sel_begin = h->hub.rate_begin.p + first;
+      hb.part_best = h->hub.part_best.p;
+      hb.part_fav = h->hub.part_fav.p;
+      hb.queue = h->commit.ctr32.p + 64 + s_idx; // zeroed with the other per-round counters
       sweep_hub_rate<EW><<<capped(h, std::min<uint32_t>(hb.num_items, kSMs)), kRateThreads, rate_smem<EW>(), h->sweep_stream>>>(a, hb);
-      h->kernel_launches += 2;
+      h->counts.kernel_launches += 2;
     } else {
-      hb.table_off = h->t4_table_off.p + first;
-      hb.g_tab = h->hub_tab.p;
-      hb.cursor = h->hub_cursor.p;
-      hb.ovf = h->hub_ovf.p;
-      hb.ovf_cap = static_cast<uint32_t>(std::min<uint64_t>(h->t4_max_wave_edges, 0xFFFFFFFFull));
+      hb.table_off = h->hub.table_off.p + first;
+      hb.g_tab = h->hub_tmp.tab.p;
+      hb.cursor = h->hub_tmp.cursor.p;
+      hb.ovf = h->hub_tmp.ovf.p;
+      hb.ovf_cap = static_cast<uint32_t>(std::min<uint64_t>(h->hub.max_wave_edges, 0xFFFFFFFFull));
       hb.bucket_cap = h->hub_bucket_cap;
-      hb.stage_adjncy = h->adjncy_16b ? 1u : 0u;
-      hb.sel_begin = h->t4_sel_begin.p + first;
+      hb.stage_adjncy = h->graph.adjncy_16b ? 1u : 0u;
+      hb.sel_begin = h->hub.sel_begin.p + first;
       // one scatter + select pair per wave; all waves share the bucket memory (cursors reset by the select)
-      for (uint32_t w = h->t4_wave_off[s_idx]; w < h->t4_wave_off[s_idx + 1]; ++w) {
-        const kmp_lp_handle::HubWave &wv = h->t4_waves[w];
-        hb.item_entry = h->t4_item_entry.p + wv.item_lo;
-        hb.item_chunk = h->t4_item_chunk.p + wv.item_lo;
-        hb.item_u = h->t4_item_u.p + wv.item_lo;
-        hb.item_beg = h->t4_item_beg.p + wv.item_lo;
-        hb.item_deg = h->t4_item_deg.p + wv.item_lo;
+      for (uint32_t w = h->hub.wave_off[s_idx]; w < h->hub.wave_off[s_idx + 1]; ++w) {
+        const kmp_lp_handle::HubMeta::Wave &wv = h->hub.waves[w];
+        hb.item_entry = h->hub.item_entry.p + wv.item_lo;
+        hb.item_chunk = h->hub.item_chunk.p + wv.item_lo;
+        hb.item_u = h->hub.item_u.p + wv.item_lo;
+        hb.item_beg = h->hub.item_beg.p + wv.item_lo;
+        hb.item_deg = h->hub.item_deg.p + wv.item_lo;
         hb.num_items = wv.item_hi - wv.item_lo;
-        hb.queue = h->ctr32.p + 64 + w; // zeroed with the other per-round counters
-        hb.ovf_count = h->ctr32.p + 512 + w;
-        sweep_hub_scatter<MODE, EW, P64><<<capped(h, std::min<uint32_t>(hb.num_items, kSMs * 4)), kHubThreads, kHubScatterSmem, h->sweep_stream>>>(a, hb, h->m);
-        hb.sel_entry = h->t4_sel_entry.p + wv.sel_lo;
-        hb.sel_piece = h->t4_sel_piece.p + wv.sel_lo;
+        hb.queue = h->commit.ctr32.p + 64 + w; // zeroed with the other per-round counters
+        hb.ovf_count = h->commit.ctr32.p + 512 + w;
+        sweep_hub_scatter<MODE, EW, P64><<<capped(h, std::min<uint32_t>(hb.num_items, kSMs * 4)), kHubThreads, kHubScatterSmem, h->sweep_stream>>>(a, hb, h->graph.m);
+        hb.sel_entry = h->hub.sel_entry.p + wv.sel_lo;
+        hb.sel_piece = h->hub.sel_piece.p + wv.sel_lo;
         hb.num_sel_items = wv.sel_hi - wv.sel_lo;
-        hb.part_best = h->t4_part_best.p + (wv.sel_lo - h->t4_sel_off[s_idx]);
-        hb.part_fav = h->t4_part_fav.p + (wv.sel_lo - h->t4_sel_off[s_idx]);
+        hb.part_best = h->hub.part_best.p + (wv.sel_lo - h->hub.sel_off[s_idx]);
+        hb.part_fav = h->hub.part_fav.p + (wv.sel_lo - h->hub.sel_off[s_idx]);
         sweep_hub_select<MODE><<<capped(h, std::min<uint32_t>((hb.num_sel_items + kSelWarps - 1) / kSelWarps, kSMs * 6)), kSelWarps * 32, 0, h->sweep_stream>>>(a, hb);
-        h->kernel_launches += 2;
+        h->counts.kernel_launches += 2;
       }
     }
-    hb.part_best = h->t4_part_best.p;
-    hb.part_fav = h->t4_part_fav.p;
+    hb.part_best = h->hub.part_best.p;
+    hb.part_fav = h->hub.part_fav.p;
     sweep_hub_final<MODE><<<capped(h, grid_for(static_cast<uint64_t>(a.list_size) * 32, 256)), 256, 0, h->sweep_stream>>>(a, hb);
     break;
   }
@@ -955,21 +1035,21 @@ int timed_begin(kmp_lp_handle *h, int tag, cudaStream_t st = nullptr) {
   if (st == nullptr) {
     st = h->stream;
   }
-  if (h->sweep_events_used == h->sweep_events.size()) {
+  if (h->counts.sweep_events_used == h->streams.sweep_events.size()) {
     cudaEvent_t x, y;
     cudaEventCreate(&x);
     cudaEventCreate(&y);
-    h->sweep_events.emplace_back(x, y);
-    h->sweep_event_group.push_back(0);
+    h->streams.sweep_events.emplace_back(x, y);
+    h->streams.sweep_event_group.push_back(0);
   }
-  const int idx = static_cast<int>(h->sweep_events_used++);
-  h->sweep_event_group[idx] = tag;
-  cudaEventRecord(h->sweep_events[idx].first, st);
+  const int idx = static_cast<int>(h->counts.sweep_events_used++);
+  h->streams.sweep_event_group[idx] = tag;
+  cudaEventRecord(h->streams.sweep_events[idx].first, st);
   return idx;
 }
 void timed_end(kmp_lp_handle *h, int idx, cudaStream_t st = nullptr) {
   if (idx >= 0) {
-    cudaEventRecord(h->sweep_events[idx].second, st == nullptr ? h->stream : st);
+    cudaEventRecord(h->streams.sweep_events[idx].second, st == nullptr ? h->stream : st);
   }
 }
 
@@ -979,14 +1059,14 @@ cudaError_t launch_sweep(kmp_lp_handle *h, int mode, int tier, const SweepArgs &
     return cudaSuccess;
   }
   SweepArgs a = a_in;
-  a.counters = h->ctr64.p + tier;
-  a.queue = h->queue.p + static_cast<size_t>(tier) * kNumGroups * h->lists_S + h->cur_sg;
+  a.counters = h->commit.ctr64.p + tier;
+  a.queue = h->lists.queue.p + static_cast<size_t>(tier) * kNumGroups * h->lists.S + h->round.cur_sg;
   if (h->sweep_stream == nullptr) {
     h->sweep_stream = h->stream;
   }
   const int ev = timed_begin(h, tier, h->sweep_stream);
-  const bool ew = h->adjwgt != nullptr;
-  const int variant = (mode << 2) | (ew ? 2 : 0) | (h->p64 ? 1 : 0);
+  const bool ew = h->graph.adjwgt != nullptr;
+  const int variant = (mode << 2) | (ew ? 2 : 0) | (h->round.p64 ? 1 : 0);
   cudaError_t e;
   switch (variant) {
   case 0: e = launch_sweep_t<0, false, false>(h, tier, a); break;
@@ -999,9 +1079,9 @@ cudaError_t launch_sweep(kmp_lp_handle *h, int mode, int tier, const SweepArgs &
   default: e = launch_sweep_t<1, true, true>(h, tier, a); break;
   }
   timed_end(h, ev, h->sweep_stream);
-  ++h->kernel_launches;
-  ++h->sweep_launches;
-  ++h->group_launches[tier];
+  ++h->counts.kernel_launches;
+  ++h->counts.sweep_launches;
+  ++h->counts.group_launches[tier];
   return e;
 }
 
@@ -1017,241 +1097,250 @@ struct TraceClock { // KMP_TRACE=1: wall-clock stages of set_graph on stderr (di
   }
 };
 
+// The hub tier metadata of the work lists just built with S sub-rounds (kmp_lp_handle::HubMeta): bucket regions, chunk
+// work items and (entry, bucket) selection items per sub-round.
+int build_hub_meta(kmp_lp_handle *h, uint32_t S) {
+  const uint32_t hub_begin = h->lists.off[kHubTier * S], hub_end = h->lists.off[(kHubTier + 1) * S];
+  const uint32_t hub_cnt = hub_end - hub_begin;
+  h->hub.item_off.assign(S + 1, 0);
+  h->hub.wave_off.assign(S + 1, 0);
+  h->hub.waves.clear();
+  h->hub.max_slots = 0;
+  h->hub.max_wave_edges = 0;
+  h->hub.max_subround_edges = 0;
+  h->hub.max_subround_cls = 0;
+  if (hub_cnt > 0) {
+    DevBuf<uint32_t> &d_deg = h->list_tmp.hub_deg, &d_beg = h->list_tmp.hub_beg, &d_ids = h->list_tmp.hub_ids; // grow-only
+    KMP_CUDA(d_deg.ensure(hub_cnt));
+    KMP_CUDA(d_beg.ensure(hub_cnt));
+    KMP_CUDA(d_ids.ensure(hub_cnt));
+    k_gather_degrees<<<grid_for(hub_cnt, 256), 256, 0, h->stream>>>(hub_cnt, h->lists.order.p + hub_begin, h->graph.xadj, d_deg.p,
+                                                                    d_beg.p, d_ids.p);
+    std::vector<uint32_t> vbeg(hub_cnt), vids(hub_cnt), iu, ibeg, ideg;
+    KMP_CUDA(cudaMemcpyAsync(vbeg.data(), d_beg.p, hub_cnt * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+    KMP_CUDA(cudaMemcpyAsync(vids.data(), d_ids.p, hub_cnt * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+    std::vector<uint32_t> deg(hub_cnt), toff(hub_cnt), sbeg(hub_cnt), ient, ichk, sent, spiece;
+    h->hub.sel_off.assign(S + 1, 0);
+    size_t max_sel = 0;
+    KMP_CUDA(cudaMemcpyAsync(deg.data(), d_deg.p, hub_cnt * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+    KMP_CUDA(cudaStreamSynchronize(h->stream));
+    // at most kMaxHubWaves work-queue cursors exist per LP round: coarsen the waves if necessary
+    // (the degrees must be on the host before this sum -- ADVICE r1)
+    uint64_t wave_slots = h->hub_wave_slots;
+    {
+      uint64_t total = 0;
+      for (uint32_t i = 0; i < hub_cnt; ++i) {
+        total += static_cast<uint64_t>(hub_buckets(deg[i])) * kBucketCap;
+      }
+      wave_slots = std::max<uint64_t>(wave_slots, total / (kMaxHubWaves / 2 - S) + 1);
+    }
+    for (uint32_t sr = 0; sr < S; ++sr) {
+      const uint32_t lo = h->lists.off[kHubTier * S + sr] - hub_begin, hi = h->lists.off[kHubTier * S + sr + 1] - hub_begin;
+      uint64_t slots = 0, wave_edges = 0;
+      kmp_lp_handle::HubMeta::Wave wave{static_cast<uint32_t>(ient.size()), 0, static_cast<uint32_t>(sent.size()), 0};
+      auto close_wave = [&]() {
+        wave.item_hi = static_cast<uint32_t>(ient.size());
+        wave.sel_hi = static_cast<uint32_t>(sent.size());
+        if (wave.item_hi > wave.item_lo) {
+          h->hub.waves.push_back(wave);
+        }
+        wave.item_lo = wave.item_hi;
+        wave.sel_lo = wave.sel_hi;
+        h->hub.max_slots = std::max(h->hub.max_slots, slots);
+        h->hub.max_wave_edges = std::max(h->hub.max_wave_edges, wave_edges);
+        slots = 0;
+        wave_edges = 0;
+      };
+      for (uint32_t i = lo; i < hi; ++i) {
+        const uint32_t buckets = hub_buckets(deg[i]);
+        const uint64_t cap = static_cast<uint64_t>(buckets) * kBucketCap;
+        if (slots > 0 && slots + cap > wave_slots) {
+          close_wave();
+        }
+        if ((slots + cap) / kBucketCap > 0xFFFFFFFFull) {
+          return fail(KMP_ERR_UNSUPPORTED, "high-degree buckets of one wave exceed 2^32");
+        }
+        toff[i] = static_cast<uint32_t>(slots / kBucketCap); // first bucket of the entry, wave-relative
+        slots += cap;
+        wave_edges += deg[i];
+        const uint32_t chunks = (deg[i] + kChunkEdges - 1) / kChunkEdges;
+        for (uint32_t c = 0; c < chunks; ++c) {
+          ient.push_back(i - lo);
+          ichk.push_back(c);
+          iu.push_back(vids[i]);
+          ibeg.push_back(vbeg[i]);
+          ideg.push_back(deg[i]);
+        }
+        sbeg[i] = static_cast<uint32_t>(sent.size() - h->hub.sel_off[sr]);
+        for (uint32_t c = 0; c < buckets; ++c) { // one selection item per bucket
+          sent.push_back(i - lo);
+          spiece.push_back(c);
+        }
+      }
+      close_wave();
+      h->hub.wave_off[sr + 1] = static_cast<uint32_t>(h->hub.waves.size());
+      h->hub.sel_off[sr + 1] = static_cast<uint32_t>(sent.size());
+      max_sel = std::max<size_t>(max_sel, sent.size() - h->hub.sel_off[sr]);
+      h->hub.item_off[sr + 1] = static_cast<uint32_t>(ient.size());
+    }
+    if (h->hub.waves.size() > kMaxHubWaves) {
+      return fail(KMP_ERR_UNSUPPORTED, "too many high-degree table waves (raise KMP_HUB_WAVE_SLOTS)");
+    }
+    // clusterer: per entry its row in the staged labels and its first result slot, and the (entry, hash class)
+    // rate items of every sub-round, largest degree first (the longest items start first)
+    std::vector<uint32_t> loff(hub_cnt), coff(hub_cnt), rbeg(hub_cnt), rent, rcls, ord;
+    h->hub.rate_off.assign(S + 1, 0);
+    size_t max_rate = 0;
+    for (uint32_t sr = 0; sr < S; ++sr) {
+      const uint32_t lo = h->lists.off[kHubTier * S + sr] - hub_begin, hi = h->lists.off[kHubTier * S + sr + 1] - hub_begin;
+      // edges <= m < 2^32; cls <= (m / 2048 + hubs) * 257 < 2^31 (hubs <= m / 8192)
+      uint64_t edges = 0, cls = 0;
+      uint32_t res = 0;
+      ord.clear();
+      for (uint32_t i = lo; i < hi; ++i) {
+        loff[i] = static_cast<uint32_t>(edges);
+        edges += deg[i];
+        coff[i] = static_cast<uint32_t>(cls);
+        if (h->graph.adjwgt == nullptr) {
+          cls += static_cast<uint64_t>((deg[i] + kChunkEdges - 1) / kChunkEdges) * (hub_sort_classes(deg[i]) + 1);
+        }
+        rbeg[i] = res;
+        res += hub_classes(deg[i]);
+        ord.push_back(i);
+      }
+      std::stable_sort(ord.begin(), ord.end(), [&](uint32_t x, uint32_t y) { return deg[x] > deg[y]; });
+      for (const uint32_t i : ord) {
+        for (uint32_t c = 0; c < hub_classes(deg[i]); ++c) {
+          rent.push_back(i - lo);
+          rcls.push_back(c);
+        }
+      }
+      h->hub.rate_off[sr + 1] = static_cast<uint32_t>(rent.size());
+      max_rate = std::max<size_t>(max_rate, res);
+      h->hub.max_subround_edges = std::max(h->hub.max_subround_edges, edges);
+      h->hub.max_subround_cls = std::max(h->hub.max_subround_cls, cls);
+    }
+    max_sel = std::max(max_sel, max_rate);
+    KMP_CUDA(h->hub.lab_off.ensure(hub_cnt));
+    KMP_CUDA(h->hub.rate_begin.ensure(hub_cnt));
+    KMP_CUDA(h->hub.rate_entry.ensure(rent.size()));
+    KMP_CUDA(h->hub.rate_cls.ensure(rcls.size()));
+    KMP_CUDA(cudaMemcpyAsync(h->hub.lab_off.p, loff.data(), hub_cnt * 4, cudaMemcpyHostToDevice, h->stream));
+    KMP_CUDA(h->hub.cls_off.ensure(hub_cnt));
+    KMP_CUDA(cudaMemcpyAsync(h->hub.cls_off.p, coff.data(), hub_cnt * 4, cudaMemcpyHostToDevice, h->stream));
+    KMP_CUDA(cudaMemcpyAsync(h->hub.rate_begin.p, rbeg.data(), hub_cnt * 4, cudaMemcpyHostToDevice, h->stream));
+    KMP_CUDA(cudaMemcpyAsync(h->hub.rate_entry.p, rent.data(), rent.size() * 4, cudaMemcpyHostToDevice, h->stream));
+    KMP_CUDA(cudaMemcpyAsync(h->hub.rate_cls.p, rcls.data(), rcls.size() * 4, cudaMemcpyHostToDevice, h->stream));
+    KMP_CUDA(h->hub.table_off.ensure(hub_cnt));
+    KMP_CUDA(h->hub.hit.ensure(hub_cnt));
+    KMP_CUDA(cudaMemsetAsync(h->hub.hit.p, 0, static_cast<size_t>(hub_cnt) * 4, h->stream));
+    KMP_CUDA(h->hub.item_entry.ensure(ient.size()));
+    KMP_CUDA(h->hub.item_chunk.ensure(ichk.size()));
+    KMP_CUDA(cudaMemcpyAsync(h->hub.table_off.p, toff.data(), hub_cnt * 4, cudaMemcpyHostToDevice, h->stream));
+    KMP_CUDA(cudaMemcpyAsync(h->hub.item_entry.p, ient.data(), ient.size() * 4, cudaMemcpyHostToDevice, h->stream));
+    KMP_CUDA(cudaMemcpyAsync(h->hub.item_chunk.p, ichk.data(), ichk.size() * 4, cudaMemcpyHostToDevice, h->stream));
+    KMP_CUDA(h->hub.item_u.ensure(iu.size()));
+    KMP_CUDA(h->hub.item_beg.ensure(iu.size()));
+    KMP_CUDA(h->hub.item_deg.ensure(iu.size()));
+    KMP_CUDA(cudaMemcpyAsync(h->hub.item_u.p, iu.data(), iu.size() * 4, cudaMemcpyHostToDevice, h->stream));
+    KMP_CUDA(cudaMemcpyAsync(h->hub.item_beg.p, ibeg.data(), iu.size() * 4, cudaMemcpyHostToDevice, h->stream));
+    KMP_CUDA(cudaMemcpyAsync(h->hub.item_deg.p, ideg.data(), iu.size() * 4, cudaMemcpyHostToDevice, h->stream));
+    KMP_CUDA(h->hub.sel_entry.ensure(sent.size()));
+    KMP_CUDA(h->hub.sel_piece.ensure(spiece.size()));
+    KMP_CUDA(h->hub.sel_begin.ensure(hub_cnt));
+    KMP_CUDA(h->hub.part_best.ensure(max_sel));
+    KMP_CUDA(h->hub.part_fav.ensure(max_sel));
+    KMP_CUDA(cudaMemcpyAsync(h->hub.sel_entry.p, sent.data(), sent.size() * 4, cudaMemcpyHostToDevice, h->stream));
+    KMP_CUDA(cudaMemcpyAsync(h->hub.sel_piece.p, spiece.data(), spiece.size() * 4, cudaMemcpyHostToDevice, h->stream));
+    KMP_CUDA(cudaMemcpyAsync(h->hub.sel_begin.p, sbeg.data(), hub_cnt * 4, cudaMemcpyHostToDevice, h->stream));
+    KMP_CUDA(cudaStreamSynchronize(h->stream));
+  }
+  return KMP_OK;
+}
+
 int ensure_lists(kmp_lp_handle *h) {
   TraceClock tc;
   const uint32_t S = std::max<uint32_t>(1, h->cfg.sync_subrounds);
-  if (h->lists_valid && h->lists_S == S && h->lists_G == h->cfg.sync_granule_log2 &&
-      h->lists_thr == h->cfg.large_degree_threshold && h->lists_seed == h->cfg.seed) {
+  if (h->lists.valid && h->lists.S == S && h->lists.G == h->cfg.sync_granule_log2 &&
+      h->lists.thr == h->cfg.large_degree_threshold && h->lists.seed == h->cfg.seed) {
     return KMP_OK;
   }
   if (S > kMaxSubrounds) {
     return fail(KMP_ERR_INVALID, "sync_subrounds too large (max " + std::to_string(kMaxSubrounds) + ")");
   }
-  h->stamps_ok = kNumGroups * S <= kMaxStampSubrounds; // else: push activation only
-  const uint32_t n = h->n;
+  h->lists.stamps_ok = kNumGroups * S <= kMaxStampSubrounds; // else: push activation only
+  const uint32_t n = h->graph.n;
   const uint32_t nkeys = kNumTiers * S + 1;
-  KMP_CUDA(h->sort_keys_in.ensure(n));
-  KMP_CUDA(h->sort_keys_out.ensure(n));
-  KMP_CUDA(h->sort_vals_in.ensure(n));
-  KMP_CUDA(h->order.ensure(n));
-  KMP_CUDA(h->ctr32.ensure(kCtr32Size));
-  KMP_CUDA(cudaMemsetAsync(h->ctr32.p, 0, kCtr32Size * sizeof(uint32_t), h->stream));
+  KMP_CUDA(h->list_tmp.sort_keys_in.ensure(n));
+  KMP_CUDA(h->list_tmp.sort_keys_out.ensure(n));
+  KMP_CUDA(h->list_tmp.sort_vals_in.ensure(n));
+  KMP_CUDA(h->lists.order.ensure(n));
+  KMP_CUDA(h->commit.ctr32.ensure(kCtr32Size));
+  KMP_CUDA(cudaMemsetAsync(h->commit.ctr32.p, 0, kCtr32Size * sizeof(uint32_t), h->stream));
   tc.lap("lists: buffers");
   const uint32_t base_sr = sync_base(h->cfg.seed, 0, 0, SALT_SUBROUND);
   // Sub-rounds per degree group: S for a group holding >= 1/16 of the visited vertices, S/4 otherwise
   // (a small group has few same-sub-round neighbours; its launches become 4x larger). DESIGN.md §3.
   GroupSubrounds gs{};
   {
-    k_group_counts<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->xadj, h->cfg.large_degree_threshold, h->ctr32.p);
+    k_group_counts<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->graph.xadj, h->cfg.large_degree_threshold, h->commit.ctr32.p);
     uint32_t cnt[4] = {0, 0, 0, 0};
-    KMP_CUDA(cudaMemcpyAsync(cnt, h->ctr32.p, sizeof(cnt), cudaMemcpyDeviceToHost, h->stream));
+    KMP_CUDA(cudaMemcpyAsync(cnt, h->commit.ctr32.p, sizeof(cnt), cudaMemcpyDeviceToHost, h->stream));
     KMP_CUDA(cudaStreamSynchronize(h->stream));
     const uint64_t visited = static_cast<uint64_t>(cnt[0]) + cnt[1] + cnt[2] + cnt[3];
-    h->visited_total = static_cast<uint32_t>(visited);
+    h->lists.visited_total = static_cast<uint32_t>(visited);
     for (int q = 0; q < 4; ++q) {
       gs.s[q] = (16ull * cnt[q] >= visited) ? S : std::max<uint32_t>(1, S / 4);
     }
-    KMP_CUDA(cudaMemsetAsync(h->ctr32.p, 0, kCtr32Size * sizeof(uint32_t), h->stream));
+    KMP_CUDA(cudaMemsetAsync(h->commit.ctr32.p, 0, kCtr32Size * sizeof(uint32_t), h->stream));
   }
   tc.lap("lists: group counts (sync)");
-  k_list_keys<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->xadj, S, gs, h->cfg.sync_granule_log2, base_sr,
+  k_list_keys<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->graph.xadj, S, gs, h->cfg.sync_granule_log2, base_sr,
                                                         h->cfg.large_degree_threshold,
-                                                        h->adjwgt != nullptr ? kHubMinDegree : kHubMinDegreeUnit,
-                                                        h->sort_keys_in.p, h->sort_vals_in.p, h->ctr32.p, h->ctr32.p + 300);
+                                                        h->graph.adjwgt != nullptr ? kHubMinDegree : kHubMinDegreeUnit,
+                                                        h->list_tmp.sort_keys_in.p, h->list_tmp.sort_vals_in.p, h->commit.ctr32.p,
+                                                        h->commit.ctr32.p + 300);
   KMP_CUDA(cudaGetLastError());
   if (n > 0) {
     KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
-      return cub::DeviceRadixSort::SortPairs(tmp, bytes, h->sort_keys_in.p, h->sort_keys_out.p, h->sort_vals_in.p,
-                                             h->order.p, static_cast<int>(n), 0, 8, h->stream);
+      return cub::DeviceRadixSort::SortPairs(tmp, bytes, h->list_tmp.sort_keys_in.p, h->list_tmp.sort_keys_out.p,
+                                             h->list_tmp.sort_vals_in.p, h->lists.order.p, static_cast<int>(n), 0, 8,
+                                             h->stream);
     }));
   }
   std::vector<uint32_t> hist(512);
-  KMP_CUDA(cudaMemcpyAsync(hist.data(), h->ctr32.p, 512 * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+  KMP_CUDA(cudaMemcpyAsync(hist.data(), h->commit.ctr32.p, 512 * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
   KMP_CUDA(cudaStreamSynchronize(h->stream));
   tc.lap("lists: keys + sort (sync)");
-  h->list_off.assign(nkeys + 1, 0);
+  h->lists.off.assign(nkeys + 1, 0);
   for (uint32_t kx = 0; kx < nkeys; ++kx) {
-    h->list_off[kx + 1] = h->list_off[kx] + hist[kx];
+    h->lists.off[kx + 1] = h->lists.off[kx] + hist[kx];
   }
   auto lsize = [&](uint32_t tier, uint32_t sr) { return hist[tier * S + sr]; };
-  h->max_list = 0;
-  h->mover_cap = 1;
+  h->lists.max_list = 0;
+  h->lists.mover_cap = 1;
   for (uint32_t sr = 0; sr < S; ++sr) {
     for (int g = 0; g < kNumGroups; ++g) { // the tiers of a degree group share a sub-round
       uint32_t tot = 0;
       for (int t = first_tier_of_group(g); t <= last_tier_of_group(g); ++t) {
         tot += lsize(static_cast<uint32_t>(t), sr);
       }
-      h->mover_cap = std::max(h->mover_cap, tot);
+      h->lists.mover_cap = std::max(h->lists.mover_cap, tot);
     }
   }
-  KMP_CUDA(h->queue.ensure(static_cast<size_t>(kNumTiers) * kNumGroups * S));
-  h->max_list = h->mover_cap;
-  h->max_degree = hist[300];
-  // ---- hub tier metadata: bucket regions, chunk work items and (entry, bucket) selection items per sub-round --
-  {
-    const uint32_t t4_begin = h->list_off[kHubTier * S], t4_end = h->list_off[(kHubTier + 1) * S];
-    const uint32_t t4_cnt = t4_end - t4_begin;
-    h->t4_item_off.assign(S + 1, 0);
-    h->t4_wave_off.assign(S + 1, 0);
-    h->t4_waves.clear();
-    h->t4_max_slots = 0;
-    h->t4_max_wave_edges = 0;
-    h->t4_max_subround_edges = 0;
-    h->t4_max_subround_cls = 0;
-    if (t4_cnt > 0) {
-      DevBuf<uint32_t> &d_deg = h->t4_tmp_deg, &d_beg = h->t4_tmp_beg, &d_ids = h->t4_tmp_ids; // grow-only
-      KMP_CUDA(d_deg.ensure(t4_cnt));
-      KMP_CUDA(d_beg.ensure(t4_cnt));
-      KMP_CUDA(d_ids.ensure(t4_cnt));
-      k_gather_degrees<<<grid_for(t4_cnt, 256), 256, 0, h->stream>>>(t4_cnt, h->order.p + t4_begin, h->xadj, d_deg.p,
-                                                                      d_beg.p, d_ids.p);
-      std::vector<uint32_t> vbeg(t4_cnt), vids(t4_cnt), iu, ibeg, ideg;
-      KMP_CUDA(cudaMemcpyAsync(vbeg.data(), d_beg.p, t4_cnt * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
-      KMP_CUDA(cudaMemcpyAsync(vids.data(), d_ids.p, t4_cnt * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
-      std::vector<uint32_t> deg(t4_cnt), toff(t4_cnt), sbeg(t4_cnt), ient, ichk, sent, spiece;
-      h->t4_sel_off.assign(S + 1, 0);
-      size_t max_sel = 0;
-      KMP_CUDA(cudaMemcpyAsync(deg.data(), d_deg.p, t4_cnt * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
-      KMP_CUDA(cudaStreamSynchronize(h->stream));
-      // at most kMaxHubWaves work-queue cursors exist per LP round: coarsen the waves if necessary
-      // (the degrees must be on the host before this sum -- ADVICE r1)
-      uint64_t wave_slots = h->hub_wave_slots;
-      {
-        uint64_t total = 0;
-        for (uint32_t i = 0; i < t4_cnt; ++i) {
-          total += static_cast<uint64_t>(hub_buckets(deg[i])) * kBucketCap;
-        }
-        wave_slots = std::max<uint64_t>(wave_slots, total / (kMaxHubWaves / 2 - S) + 1);
-      }
-      for (uint32_t sr = 0; sr < S; ++sr) {
-        const uint32_t lo = h->list_off[kHubTier * S + sr] - t4_begin, hi = h->list_off[kHubTier * S + sr + 1] - t4_begin;
-        uint64_t slots = 0, wave_edges = 0;
-        kmp_lp_handle::HubWave wave{static_cast<uint32_t>(ient.size()), 0, static_cast<uint32_t>(sent.size()), 0};
-        auto close_wave = [&]() {
-          wave.item_hi = static_cast<uint32_t>(ient.size());
-          wave.sel_hi = static_cast<uint32_t>(sent.size());
-          if (wave.item_hi > wave.item_lo) {
-            h->t4_waves.push_back(wave);
-          }
-          wave.item_lo = wave.item_hi;
-          wave.sel_lo = wave.sel_hi;
-          h->t4_max_slots = std::max(h->t4_max_slots, slots);
-          h->t4_max_wave_edges = std::max(h->t4_max_wave_edges, wave_edges);
-          slots = 0;
-          wave_edges = 0;
-        };
-        for (uint32_t i = lo; i < hi; ++i) {
-          const uint32_t buckets = hub_buckets(deg[i]);
-          const uint64_t cap = static_cast<uint64_t>(buckets) * kBucketCap;
-          if (slots > 0 && slots + cap > wave_slots) {
-            close_wave();
-          }
-          if ((slots + cap) / kBucketCap > 0xFFFFFFFFull) {
-            return fail(KMP_ERR_UNSUPPORTED, "high-degree buckets of one wave exceed 2^32");
-          }
-          toff[i] = static_cast<uint32_t>(slots / kBucketCap); // first bucket of the entry, wave-relative
-          slots += cap;
-          wave_edges += deg[i];
-          const uint32_t chunks = (deg[i] + kChunkEdges - 1) / kChunkEdges;
-          for (uint32_t c = 0; c < chunks; ++c) {
-            ient.push_back(i - lo);
-            ichk.push_back(c);
-            iu.push_back(vids[i]);
-            ibeg.push_back(vbeg[i]);
-            ideg.push_back(deg[i]);
-          }
-          sbeg[i] = static_cast<uint32_t>(sent.size() - h->t4_sel_off[sr]);
-          for (uint32_t c = 0; c < buckets; ++c) { // one selection item per bucket
-            sent.push_back(i - lo);
-            spiece.push_back(c);
-          }
-        }
-        close_wave();
-        h->t4_wave_off[sr + 1] = static_cast<uint32_t>(h->t4_waves.size());
-        h->t4_sel_off[sr + 1] = static_cast<uint32_t>(sent.size());
-        max_sel = std::max<size_t>(max_sel, sent.size() - h->t4_sel_off[sr]);
-        h->t4_item_off[sr + 1] = static_cast<uint32_t>(ient.size());
-      }
-      if (h->t4_waves.size() > kMaxHubWaves) {
-        return fail(KMP_ERR_UNSUPPORTED, "too many high-degree table waves (raise KMP_HUB_WAVE_SLOTS)");
-      }
-      // clusterer: per entry its row in the staged labels and its first result slot, and the (entry, hash class)
-      // rate items of every sub-round, largest degree first (the longest items start first)
-      std::vector<uint32_t> loff(t4_cnt), coff(t4_cnt), rbeg(t4_cnt), rent, rcls, ord;
-      h->t4_rate_off.assign(S + 1, 0);
-      size_t max_rate = 0;
-      for (uint32_t sr = 0; sr < S; ++sr) {
-        const uint32_t lo = h->list_off[kHubTier * S + sr] - t4_begin, hi = h->list_off[kHubTier * S + sr + 1] - t4_begin;
-        // edges <= m < 2^32; cls <= (m / 2048 + hubs) * 257 < 2^31 (hubs <= m / 8192)
-        uint64_t edges = 0, cls = 0;
-        uint32_t res = 0;
-        ord.clear();
-        for (uint32_t i = lo; i < hi; ++i) {
-          loff[i] = static_cast<uint32_t>(edges);
-          edges += deg[i];
-          coff[i] = static_cast<uint32_t>(cls);
-          if (h->adjwgt == nullptr) {
-            cls += static_cast<uint64_t>((deg[i] + kChunkEdges - 1) / kChunkEdges) * (hub_sort_classes(deg[i]) + 1);
-          }
-          rbeg[i] = res;
-          res += hub_classes(deg[i]);
-          ord.push_back(i);
-        }
-        std::stable_sort(ord.begin(), ord.end(), [&](uint32_t x, uint32_t y) { return deg[x] > deg[y]; });
-        for (const uint32_t i : ord) {
-          for (uint32_t c = 0; c < hub_classes(deg[i]); ++c) {
-            rent.push_back(i - lo);
-            rcls.push_back(c);
-          }
-        }
-        h->t4_rate_off[sr + 1] = static_cast<uint32_t>(rent.size());
-        max_rate = std::max<size_t>(max_rate, res);
-        h->t4_max_subround_edges = std::max(h->t4_max_subround_edges, edges);
-        h->t4_max_subround_cls = std::max(h->t4_max_subround_cls, cls);
-      }
-      max_sel = std::max(max_sel, max_rate);
-      KMP_CUDA(h->t4_lab_off.ensure(t4_cnt));
-      KMP_CUDA(h->t4_rate_begin.ensure(t4_cnt));
-      KMP_CUDA(h->t4_rate_entry.ensure(rent.size()));
-      KMP_CUDA(h->t4_rate_cls.ensure(rcls.size()));
-      KMP_CUDA(cudaMemcpyAsync(h->t4_lab_off.p, loff.data(), t4_cnt * 4, cudaMemcpyHostToDevice, h->stream));
-      KMP_CUDA(h->t4_cls_off.ensure(t4_cnt));
-      KMP_CUDA(cudaMemcpyAsync(h->t4_cls_off.p, coff.data(), t4_cnt * 4, cudaMemcpyHostToDevice, h->stream));
-      KMP_CUDA(cudaMemcpyAsync(h->t4_rate_begin.p, rbeg.data(), t4_cnt * 4, cudaMemcpyHostToDevice, h->stream));
-      KMP_CUDA(cudaMemcpyAsync(h->t4_rate_entry.p, rent.data(), rent.size() * 4, cudaMemcpyHostToDevice, h->stream));
-      KMP_CUDA(cudaMemcpyAsync(h->t4_rate_cls.p, rcls.data(), rcls.size() * 4, cudaMemcpyHostToDevice, h->stream));
-      KMP_CUDA(h->t4_table_off.ensure(t4_cnt));
-      KMP_CUDA(h->t4_hit.ensure(t4_cnt));
-      KMP_CUDA(cudaMemsetAsync(h->t4_hit.p, 0, static_cast<size_t>(t4_cnt) * 4, h->stream));
-      KMP_CUDA(h->t4_item_entry.ensure(ient.size()));
-      KMP_CUDA(h->t4_item_chunk.ensure(ichk.size()));
-      KMP_CUDA(cudaMemcpyAsync(h->t4_table_off.p, toff.data(), t4_cnt * 4, cudaMemcpyHostToDevice, h->stream));
-      KMP_CUDA(cudaMemcpyAsync(h->t4_item_entry.p, ient.data(), ient.size() * 4, cudaMemcpyHostToDevice, h->stream));
-      KMP_CUDA(cudaMemcpyAsync(h->t4_item_chunk.p, ichk.data(), ichk.size() * 4, cudaMemcpyHostToDevice, h->stream));
-      KMP_CUDA(h->t4_item_u.ensure(iu.size()));
-      KMP_CUDA(h->t4_item_beg.ensure(iu.size()));
-      KMP_CUDA(h->t4_item_deg.ensure(iu.size()));
-      KMP_CUDA(cudaMemcpyAsync(h->t4_item_u.p, iu.data(), iu.size() * 4, cudaMemcpyHostToDevice, h->stream));
-      KMP_CUDA(cudaMemcpyAsync(h->t4_item_beg.p, ibeg.data(), iu.size() * 4, cudaMemcpyHostToDevice, h->stream));
-      KMP_CUDA(cudaMemcpyAsync(h->t4_item_deg.p, ideg.data(), iu.size() * 4, cudaMemcpyHostToDevice, h->stream));
-      KMP_CUDA(h->t4_sel_entry.ensure(sent.size()));
-      KMP_CUDA(h->t4_sel_piece.ensure(spiece.size()));
-      KMP_CUDA(h->t4_sel_begin.ensure(t4_cnt));
-      KMP_CUDA(h->t4_part_best.ensure(max_sel));
-      KMP_CUDA(h->t4_part_fav.ensure(max_sel));
-      KMP_CUDA(cudaMemcpyAsync(h->t4_sel_entry.p, sent.data(), sent.size() * 4, cudaMemcpyHostToDevice, h->stream));
-      KMP_CUDA(cudaMemcpyAsync(h->t4_sel_piece.p, spiece.data(), spiece.size() * 4, cudaMemcpyHostToDevice, h->stream));
-      KMP_CUDA(cudaMemcpyAsync(h->t4_sel_begin.p, sbeg.data(), t4_cnt * 4, cudaMemcpyHostToDevice, h->stream));
-      KMP_CUDA(cudaStreamSynchronize(h->stream));
-    }
+  KMP_CUDA(h->lists.queue.ensure(static_cast<size_t>(kNumTiers) * kNumGroups * S));
+  h->lists.max_list = h->lists.mover_cap;
+  h->graph.max_degree = hist[300];
+  const int rc = build_hub_meta(h, S);
+  if (rc != KMP_OK) {
+    return rc;
   }
   tc.lap("lists: hub metadata");
-  h->lists_S = S;
-  h->lists_G = h->cfg.sync_granule_log2;
-  h->lists_thr = h->cfg.large_degree_threshold;
-  h->lists_seed = h->cfg.seed;
-  h->lists_valid = true;
+  h->lists.S = S;
+  h->lists.G = h->cfg.sync_granule_log2;
+  h->lists.thr = h->cfg.large_degree_threshold;
+  h->lists.seed = h->cfg.seed;
+  h->lists.valid = true;
   // the sort buffers are only needed here
   // The sort buffers stay allocated (grow-only, released by kmp_lp_free_scratch): a cudaFree / cudaMalloc pair per
   // set_graph synchronises the whole device, and waits for the graph upload in flight (scripts/e2e_probe.py).
@@ -1261,46 +1350,47 @@ int ensure_lists(kmp_lp_handle *h) {
 
 // scratch shared by both modes
 int ensure_scratch(kmp_lp_handle *h, int mode, uint32_t num_labels) {
-  const size_t cap = std::max<uint32_t>(h->mover_cap, 1);
-  KMP_CUDA(h->mv_u.ensure(cap));
-  KMP_CUDA(h->mv_t.ensure(cap));
-  KMP_CUDA(h->acc.ensure(cap));
-  KMP_CUDA(h->ctr32.ensure(kCtr32Size));
-  KMP_CUDA(h->ctr64.ensure(kCtrSize));
-  KMP_CUDA(h->active.ensure(h->n));
+  const size_t cap = std::max<uint32_t>(h->lists.mover_cap, 1);
+  KMP_CUDA(h->commit.mv_u.ensure(cap));
+  KMP_CUDA(h->commit.mv_t.ensure(cap));
+  KMP_CUDA(h->commit.acc.ensure(cap));
+  KMP_CUDA(h->commit.ctr32.ensure(kCtr32Size));
+  KMP_CUDA(h->commit.ctr64.ensure(kCtrSize));
+  KMP_CUDA(h->lp.active.ensure(h->graph.n));
   if (mode == 0) {
-    KMP_CUDA(h->cslot.ensure(cap));
-    const bool fresh = h->incoming.cap < h->n || h->slotmap.cap < h->n || h->chist.cap < cap * kLadderLevels;
-    KMP_CUDA(h->incoming.ensure(h->n));
-    KMP_CUDA(h->slotmap.ensure(h->n));
-    KMP_CUDA(h->chist.ensure(cap * kLadderLevels));
-    if (fresh || !h->slot_state_clean) {
-      KMP_CUDA(cudaMemsetAsync(h->incoming.p, 0, h->incoming.cap * sizeof(int32_t), h->stream));
-      KMP_CUDA(cudaMemsetAsync(h->slotmap.p, 0xFF, h->slotmap.cap * sizeof(uint32_t), h->stream));
-      KMP_CUDA(cudaMemsetAsync(h->chist.p, 0, h->chist.cap * sizeof(int32_t), h->stream));
-      h->slot_state_clean = true;
+    KMP_CUDA(h->commit.cslot.ensure(cap));
+    const bool fresh = h->commit.incoming.cap < h->graph.n || h->commit.slotmap.cap < h->graph.n ||
+                       h->commit.chist.cap < cap * kLadderLevels;
+    KMP_CUDA(h->commit.incoming.ensure(h->graph.n));
+    KMP_CUDA(h->commit.slotmap.ensure(h->graph.n));
+    KMP_CUDA(h->commit.chist.ensure(cap * kLadderLevels));
+    if (fresh || !h->commit.slot_state_clean) {
+      KMP_CUDA(cudaMemsetAsync(h->commit.incoming.p, 0, h->commit.incoming.cap * sizeof(int32_t), h->stream));
+      KMP_CUDA(cudaMemsetAsync(h->commit.slotmap.p, 0xFF, h->commit.slotmap.cap * sizeof(uint32_t), h->stream));
+      KMP_CUDA(cudaMemsetAsync(h->commit.chist.p, 0, h->commit.chist.cap * sizeof(int32_t), h->stream));
+      h->commit.slot_state_clean = true;
     }
   } else {
     const size_t kk = std::max<uint32_t>(num_labels, 1);
-    KMP_CUDA(h->hist.ensure(kk * kLadderLevels));
-    KMP_CUDA(h->ohist.ensure(kk * kLadderLevels));
-    KMP_CUDA(h->jmin.ensure(kk));
-    KMP_CUDA(h->ojmin.ensure(kk));
-    KMP_CUDA(h->out_cur.ensure(kk));
-    KMP_CUDA(h->out_delta.ensure(kk));
-    KMP_CUDA(cudaMemsetAsync(h->hist.p, 0, kk * kLadderLevels * sizeof(int32_t), h->stream));
-    KMP_CUDA(cudaMemsetAsync(h->ohist.p, 0, kk * kLadderLevels * sizeof(int32_t), h->stream));
+    KMP_CUDA(h->commit.hist.ensure(kk * kLadderLevels));
+    KMP_CUDA(h->commit.ohist.ensure(kk * kLadderLevels));
+    KMP_CUDA(h->commit.jmin.ensure(kk));
+    KMP_CUDA(h->commit.ojmin.ensure(kk));
+    KMP_CUDA(h->commit.out_cur.ensure(kk));
+    KMP_CUDA(h->commit.out_delta.ensure(kk));
+    KMP_CUDA(cudaMemsetAsync(h->commit.hist.p, 0, kk * kLadderLevels * sizeof(int32_t), h->stream));
+    KMP_CUDA(cudaMemsetAsync(h->commit.ohist.p, 0, kk * kLadderLevels * sizeof(int32_t), h->stream));
   }
   // hub tier scratch: the clusterer stages 4 B per hub edge of the largest sub-round; the refiner has bucket
   // regions, cursors and an overflow list
-  if (mode == 0 && h->t4_max_subround_edges > 0) {
-    KMP_CUDA(h->hub_lab.ensure(h->t4_max_subround_edges));
-    KMP_CUDA(h->hub_cls.ensure(h->t4_max_subround_cls));
+  if (mode == 0 && h->hub.max_subround_edges > 0) {
+    KMP_CUDA(h->hub_tmp.lab.ensure(h->hub.max_subround_edges));
+    KMP_CUDA(h->hub_tmp.cls.ensure(h->hub.max_subround_cls));
   }
-  if (mode == 1 && h->t4_max_slots > 0) {
-    KMP_CUDA(h->hub_tab.ensure(h->t4_max_slots)); // no initialisation: the cursors say how much of a region is valid
-    KMP_CUDA(h->hub_cursor.ensure(h->t4_max_slots / kBucketCap));
-    KMP_CUDA(h->hub_ovf.ensure(std::max<uint64_t>(h->t4_max_wave_edges, 1)));
+  if (mode == 1 && h->hub.max_slots > 0) {
+    KMP_CUDA(h->hub_tmp.tab.ensure(h->hub.max_slots)); // no initialisation: the cursors say how much of a region is valid
+    KMP_CUDA(h->hub_tmp.cursor.ensure(h->hub.max_slots / kBucketCap));
+    KMP_CUDA(h->hub_tmp.ovf.ensure(std::max<uint64_t>(h->hub.max_wave_edges, 1)));
     KMP_CUDA(cudaGetLastError());
   }
   (void)num_labels;
@@ -1309,35 +1399,35 @@ int ensure_scratch(kmp_lp_handle *h, int mode, uint32_t num_labels) {
 
 SweepArgs make_sweep_args(kmp_lp_handle *h, const RunCtx &rc) {
   SweepArgs a{};
-  a.xadj = h->xadj;
-  a.adjncy = h->adjncy;
-  a.vwgt = h->vwgt;
-  a.adjwgt = h->adjwgt;
-  a.label = h->label.p;
-  a.labg = h->labg.p;
+  a.xadj = h->graph.xadj;
+  a.adjncy = h->graph.adjncy;
+  a.vwgt = h->graph.vwgt;
+  a.adjwgt = h->graph.adjwgt;
+  a.label = h->lp.label.p;
+  a.labg = h->lp.labg.p;
   a.pull = false;
   a.window = make_window(0, 0);
-  a.queue = h->queue.p;
-  a.weight = h->weight.p;
-  a.max_w = rc.mode == 1 ? h->maxw.p : nullptr;
-  a.min_w = rc.has_min ? h->minw.p : nullptr;
-  a.communities = rc.has_comm ? h->communities.p : nullptr;
-  a.active = h->active.p;
-  a.favored = h->favored.p;
+  a.queue = h->lists.queue.p;
+  a.weight = h->lp.weight.p;
+  a.max_w = rc.mode == 1 ? h->lp.maxw.p : nullptr;
+  a.min_w = rc.has_min ? h->lp.minw.p : nullptr;
+  a.communities = rc.has_comm ? h->lp.communities.p : nullptr;
+  a.active = h->lp.active.p;
+  a.favored = h->lp.favored.p;
   a.max_cluster_weight = rc.max_cluster_weight;
   a.num_labels = rc.num_labels;
   a.max_num_neighbors = h->cfg.max_num_neighbors;
-  a.mv_u = h->mv_u.p;
-  a.mv_t = h->mv_t.p;
-  a.mover_count = h->ctr32.p + (h->mover_parity ? 3 : 0);
-  if (h->direct_send != nullptr) { // sharded library path: [count, -, -, -, u[cap], t[cap]]
-    a.mover_count = h->direct_send;
-    a.mv_u = h->direct_send + 4;
-    a.mv_t = h->direct_send + 4 + h->direct_cap;
+  a.mv_u = h->commit.mv_u.p;
+  a.mv_t = h->commit.mv_t.p;
+  a.mover_count = h->commit.ctr32.p + (h->round.mover_parity ? 3 : 0);
+  if (h->dist.direct_send != nullptr) { // sharded library path: [count, -, -, -, u[cap], t[cap]]
+    a.mover_count = h->dist.direct_send;
+    a.mv_u = h->dist.direct_send + 4;
+    a.mv_t = h->dist.direct_send + 4 + h->dist.direct_cap;
   }
-  a.incoming = h->incoming.p;
-  a.hist = h->hist.p;
-  a.counters = h->ctr64.p;
+  a.incoming = h->commit.incoming.p;
+  a.hist = h->commit.hist.p;
+  a.counters = h->commit.ctr64.p;
   a.sel_target = nullptr;
   a.sel_favored = nullptr;
   return a;
@@ -1345,35 +1435,35 @@ SweepArgs make_sweep_args(kmp_lp_handle *h, const RunCtx &rc) {
 
 CommitArgs make_commit_args(kmp_lp_handle *h, const RunCtx &rc) {
   CommitArgs c{};
-  c.xadj = h->xadj;
-  c.adjncy = h->adjncy;
-  c.vwgt = h->vwgt;
-  c.label = h->label.p;
-  c.labg = h->labg.p;
+  c.xadj = h->graph.xadj;
+  c.adjncy = h->graph.adjncy;
+  c.vwgt = h->graph.vwgt;
+  c.label = h->lp.label.p;
+  c.labg = h->lp.labg.p;
   c.stamp = 0;
-  c.weight = h->weight.p;
-  c.max_w = rc.mode == 1 ? h->maxw.p : nullptr;
-  c.min_w = rc.has_min ? h->minw.p : nullptr;
-  c.active = h->active.p;
+  c.weight = h->lp.weight.p;
+  c.max_w = rc.mode == 1 ? h->lp.maxw.p : nullptr;
+  c.min_w = rc.has_min ? h->lp.minw.p : nullptr;
+  c.active = h->lp.active.p;
   c.max_cluster_weight = rc.max_cluster_weight;
   c.k = rc.num_labels;
-  c.mv_u = h->mv_u.p;
-  c.mv_t = h->mv_t.p;
-  c.acc = h->acc.p;
-  c.mover_count = h->ctr32.p + (h->mover_parity ? 3 : 0);
-  c.next_mover_count = h->ctr32.p + (h->mover_parity ? 0 : 3);
-  c.also_zero = (h->world > 1 && h->comm != nullptr) ? h->dist_send.p : nullptr;
-  c.incoming = h->incoming.p;
-  c.slotmap = h->slotmap.p;
-  c.cslot = h->cslot.p;
-  c.chist = h->chist.p;
-  c.hist = h->hist.p;
-  c.jmin = h->jmin.p;
-  c.out_cur = h->out_cur.p;
-  c.out_delta = h->out_delta.p;
-  c.ohist = h->ohist.p;
-  c.ojmin = h->ojmin.p;
-  c.moved_count = h->ctr32.p + 1;
+  c.mv_u = h->commit.mv_u.p;
+  c.mv_t = h->commit.mv_t.p;
+  c.acc = h->commit.acc.p;
+  c.mover_count = h->commit.ctr32.p + (h->round.mover_parity ? 3 : 0);
+  c.next_mover_count = h->commit.ctr32.p + (h->round.mover_parity ? 0 : 3);
+  c.also_zero = (h->dist.world > 1 && h->dist.comm != nullptr) ? h->dist.send.p : nullptr;
+  c.incoming = h->commit.incoming.p;
+  c.slotmap = h->commit.slotmap.p;
+  c.cslot = h->commit.cslot.p;
+  c.chist = h->commit.chist.p;
+  c.hist = h->commit.hist.p;
+  c.jmin = h->commit.jmin.p;
+  c.out_cur = h->commit.out_cur.p;
+  c.out_delta = h->commit.out_delta.p;
+  c.ohist = h->commit.ohist.p;
+  c.ojmin = h->commit.ojmin.p;
+  c.moved_count = h->commit.ctr32.p + 1;
   return c;
 }
 
@@ -1390,22 +1480,22 @@ struct SubRound {
 };
 
 SubRound subround_of_sg(const kmp_lp_handle *h, uint32_t sg) {
-  const uint32_t S = h->lists_S;
+  const uint32_t S = h->lists.S;
   SubRound q{};
   q.group = static_cast<int>(sg / S);
   q.sr = sg % S;
   q.first_tier = first_tier_of_group(q.group);
   q.last_tier = last_tier_of_group(q.group);
   for (int t = q.first_tier; t <= q.last_tier; ++t) {
-    const uint32_t sz = h->list_off[t * S + q.sr + 1] - h->list_off[t * S + q.sr];
+    const uint32_t sz = h->lists.off[t * S + q.sr + 1] - h->lists.off[t * S + q.sr];
     q.size[t] = sz;
     q.total += sz;
     if (t == kHubTier) { // every rank sees the whole hub list and takes entries i % world == rank
       q.lo[t] = 0;
       q.hi[t] = sz;
     } else {
-      q.lo[t] = static_cast<uint32_t>(static_cast<uint64_t>(sz) * h->rank / h->world);
-      q.hi[t] = static_cast<uint32_t>(static_cast<uint64_t>(sz) * (h->rank + 1) / h->world);
+      q.lo[t] = static_cast<uint32_t>(static_cast<uint64_t>(sz) * h->dist.rank / h->dist.world);
+      q.hi[t] = static_cast<uint32_t>(static_cast<uint64_t>(sz) * (h->dist.rank + 1) / h->dist.world);
     }
   }
   return q;
@@ -1415,23 +1505,23 @@ SubRound subround_of_sg(const kmp_lp_handle *h, uint32_t sg) {
 uint32_t subround_cap(const kmp_lp_handle *h, const SubRound &q) {
   uint32_t cap = 1;
   for (int t = q.first_tier; t <= q.last_tier; ++t) {
-    cap += (q.size[t] + h->world - 1) / h->world;
+    cap += (q.size[t] + h->dist.world - 1) / h->dist.world;
   }
   return cap;
 }
 
 // sweep kernels of one sub-round over this rank's share of the lists
 int sweep_subround(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t sg, const SubRound &q) {
-  const uint32_t S = h->lists_S;
+  const uint32_t S = h->lists.S;
   SweepArgs sa = make_sweep_args(h, rc);
   sa.base_tie = sync_base(h->cfg.seed, h->call_counter, iter, SALT_TIE);
   sa.base_fav = sync_base(h->cfg.seed, h->call_counter, iter, SALT_FAV);
   sa.base_commit = sync_base(h->cfg.seed, h->call_counter, iter * 4096 + sg, SALT_COMMIT);
-  sa.accumulate = !h->stepping && rc.mode == 0; // refiner: commit_refine_fused builds the level histograms
-  sa.pull = h->pull_this;
+  sa.accumulate = !h->round.stepping && rc.mode == 0; // refiner: commit_refine_fused builds the level histograms
+  sa.pull = h->round.pull_this;
   sa.window = make_window(iter, sg);
-  h->cur_subround = q.sr;
-  h->cur_sg = sg;
+  h->round.cur_subround = q.sr;
+  h->round.cur_sg = sg;
   int live = 0;
   for (int t = q.first_tier; t <= q.last_tier; ++t) {
     live += q.size[t] != 0;
@@ -1440,7 +1530,7 @@ int sweep_subround(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t s
   // that every tier's CUDA-event time is its own)
   const bool fork = live > 1 && !h->timing;
   if (fork) {
-    KMP_CUDA(cudaEventRecord(h->ev_fork, h->stream));
+    KMP_CUDA(cudaEventRecord(h->streams.ev_fork, h->stream));
   }
   int side = 0;
   bool used[3] = {false, false, false};
@@ -1448,17 +1538,17 @@ int sweep_subround(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t s
     if (q.size[t] == 0) {
       continue;
     }
-    sa.list = h->order.p + h->list_off[t * S + q.sr] + q.lo[t];
+    sa.list = h->lists.order.p + h->lists.off[t * S + q.sr] + q.lo[t];
     sa.list_size = q.hi[t] - q.lo[t];
     h->sweep_stream = h->stream;
     if (fork && side < 3 && t != q.first_tier) {
-      h->sweep_stream = h->side_stream[side];
+      h->sweep_stream = h->streams.side[side];
       used[side] = true;
-      KMP_CUDA(cudaStreamWaitEvent(h->sweep_stream, h->ev_fork, 0));
+      KMP_CUDA(cudaStreamWaitEvent(h->sweep_stream, h->streams.ev_fork, 0));
     }
     const cudaError_t e = launch_sweep(h, rc.mode, t, sa);
     if (h->sweep_stream != h->stream) {
-      KMP_CUDA(cudaEventRecord(h->ev_join[side], h->sweep_stream));
+      KMP_CUDA(cudaEventRecord(h->streams.ev_join[side], h->sweep_stream));
       ++side;
     }
     h->sweep_stream = h->stream;
@@ -1466,7 +1556,7 @@ int sweep_subround(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t s
   }
   for (int i = 0; i < 3; ++i) {
     if (used[i]) {
-      KMP_CUDA(cudaStreamWaitEvent(h->stream, h->ev_join[i], 0));
+      KMP_CUDA(cudaStreamWaitEvent(h->stream, h->streams.ev_join[i], 0));
     }
   }
   return KMP_OK;
@@ -1483,7 +1573,7 @@ void launch_push_activation(kmp_lp_handle *h, const CommitArgs &ca, const SubRou
   default: commit_activate<256><<<capped(h, grid_for(static_cast<uint64_t>(size) * 256, 256, kSMs * 6)), 256, 0, h->stream>>>(ca); break;
   }
   timed_end(h, ev);
-  ++h->kernel_launches;
+  ++h->counts.kernel_launches;
 }
 // The refiner's ladder commit (lp_commit.cuh commit_refine_fused) in one cooperative launch, for the LP refiner and
 // both balancers. Its dynamic shared memory follows the kernel's choice of CTA-private level histograms (priv_h) and
@@ -1496,7 +1586,7 @@ int launch_commit_refine(kmp_lp_handle *h, CommitArgs ca, GatheredArgs ga, uint3
                                                        static_cast<uint32_t>(h->fused_blocks_refine)));
   GridBarrier bar{h->grid_bar.p, h->grid_bar.p + 1};
   void *args[] = {&ca, &ga, &bar, &passes};
-  if (h->p64) {
+  if (h->round.p64) {
     KMP_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void *>(commit_refine_fused<true>), dim3(blocks), dim3(256), args,
                                          smem, h->stream));
   } else {
@@ -1513,9 +1603,9 @@ int commit_subround(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t 
                     const uint32_t *gathered) {
   CommitArgs ca = make_commit_args(h, rc);
   ca.base_commit = sync_base(h->cfg.seed, h->call_counter, iter * 4096 + sg, SALT_COMMIT);
-  ca.stamp = h->stamps_ok ? make_stamp(iter, sg) : 0;
-  GatheredArgs ga{gathered, h->world, gathered != nullptr ? subround_cap(h, q) : 0u,
-                  h->ctr32.p + (h->mover_parity ? 3 : 0)};
+  ca.stamp = h->lists.stamps_ok ? make_stamp(iter, sg) : 0;
+  GatheredArgs ga{gathered, h->dist.world, gathered != nullptr ? subround_cap(h, q) : 0u,
+                  h->commit.ctr32.p + (h->round.mover_parity ? 3 : 0)};
   const int ev = timed_begin(h, kTagCommit);
   if (rc.mode == 1) {
     const int r = launch_commit_refine(h, ca, ga, std::max<uint32_t>(1, h->cfg.sync_commit_passes), q.total);
@@ -1526,7 +1616,7 @@ int commit_subround(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t 
     GridBarrier bar{h->grid_bar.p, h->grid_bar.p + 1};
     const uint32_t blocks = capped(h, std::min<uint32_t>(grid_for(q.total, 256), static_cast<uint32_t>(h->fused_blocks)));
     void *args[] = {&ca, &ga, &bar};
-    if (h->p64) {
+    if (h->round.p64) {
       KMP_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void *>(commit_cluster_fused<true>), dim3(blocks), dim3(256), args, 0,
                                            h->stream));
     } else {
@@ -1535,11 +1625,11 @@ int commit_subround(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t 
     }
   }
   timed_end(h, ev);
-  ++h->kernel_launches;
-  if (!h->pull_this || !h->pull_next) {
+  ++h->counts.kernel_launches;
+  if (!h->round.pull_this || !h->round.pull_next) {
     launch_push_activation(h, ca, q); // acc[] / mv_u[] still hold this sub-round's verdicts
   }
-  h->mover_parity ^= 1u;
+  h->round.mover_parity ^= 1u;
   return KMP_OK;
 }
 
@@ -1552,46 +1642,46 @@ int commit_subround(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t 
 // running or the next round reads flags. Both modes give the same active set as the reference's flags.
 void choose_activation(kmp_lp_handle *h, uint32_t iter) {
   // a capped neighbourhood scan cannot see all neighbours' stamps
-  const bool can_pull = h->stamps_ok && h->cfg.max_num_neighbors >= h->max_degree;
-  auto heavy = [&](uint32_t moved) { return moved == 0xFFFFFFFFu || 16ull * moved >= h->visited_total; };
+  const bool can_pull = h->lists.stamps_ok && h->cfg.max_num_neighbors >= h->graph.max_degree;
+  auto heavy = [&](uint32_t moved) { return moved == 0xFFFFFFFFu || 16ull * moved >= h->lists.visited_total; };
   if (iter == 0) {
-    h->moved_hist[0] = h->moved_hist[1] = 0xFFFFFFFFu; // [0]: round iter - 1, [1]: round iter - 2
-    h->pull_this = can_pull;
+    h->round.moved_hist[0] = h->round.moved_hist[1] = 0xFFFFFFFFu; // [0]: round iter - 1, [1]: round iter - 2
+    h->round.pull_this = can_pull;
   } else {
-    h->pull_this = h->pull_next;
+    h->round.pull_this = h->round.pull_next;
   }
-  h->pull_next = can_pull && heavy(h->moved_hist[0]);
+  h->round.pull_next = can_pull && heavy(h->round.moved_hist[0]);
   if (const char *e = std::getenv("KMP_ACTIVATION")) { // experiments / tests: force one mode
     if (e[0] == 'p' && e[1] == 'u' && e[2] == 's') {
-      h->pull_this = h->pull_next = false;
+      h->round.pull_this = h->round.pull_next = false;
     } else if (e[0] == 'p' && e[1] == 'u' && e[2] == 'l' && can_pull) {
-      h->pull_this = h->pull_next = true;
+      h->round.pull_this = h->round.pull_next = true;
     }
   }
 }
 
 int begin_iteration(kmp_lp_handle *h, uint32_t iter) {
-  KMP_CUDA(cudaMemsetAsync(h->ctr32.p, 0, kCtr32Size * sizeof(uint32_t), h->stream)); // proposal counters, moved, hub queues
-  KMP_CUDA(cudaMemsetAsync(h->queue.p, 0, h->queue.cap * sizeof(uint32_t), h->stream));
-  if (h->hub_cursor.p != nullptr) { // normally already zero (sweep_hub_select resets what it reads)
-    KMP_CUDA(cudaMemsetAsync(h->hub_cursor.p, 0, h->hub_cursor.cap * sizeof(uint32_t), h->stream));
+  KMP_CUDA(cudaMemsetAsync(h->commit.ctr32.p, 0, kCtr32Size * sizeof(uint32_t), h->stream)); // proposal counters, moved, hub queues
+  KMP_CUDA(cudaMemsetAsync(h->lists.queue.p, 0, h->lists.queue.cap * sizeof(uint32_t), h->stream));
+  if (h->hub_tmp.cursor.p != nullptr) { // normally already zero (sweep_hub_select resets what it reads)
+    KMP_CUDA(cudaMemsetAsync(h->hub_tmp.cursor.p, 0, h->hub_tmp.cursor.cap * sizeof(uint32_t), h->stream));
   }
-  if (h->world > 1 && h->comm != nullptr && h->dist_send.p != nullptr) {
-    KMP_CUDA(cudaMemsetAsync(h->dist_send.p, 0, sizeof(uint32_t), h->stream)); // proposal counter of the send buffer
+  if (h->dist.world > 1 && h->dist.comm != nullptr && h->dist.send.p != nullptr) {
+    KMP_CUDA(cudaMemsetAsync(h->dist.send.p, 0, sizeof(uint32_t), h->stream)); // proposal counter of the send buffer
   }
-  h->mover_parity = 0;
+  h->round.mover_parity = 0;
   choose_activation(h, iter);
-  h->pull_rounds += h->pull_this ? 1 : 0;
-  h->push_rounds += (!h->pull_this || !h->pull_next) ? 1 : 0;
-  if (iter >= 2 && h->stamps_ok && h->n > 0) {
+  h->counts.pull_rounds += h->round.pull_this ? 1 : 0;
+  h->counts.push_rounds += (!h->round.pull_this || !h->round.pull_next) ? 1 : 0;
+  if (iter >= 2 && h->lists.stamps_ok && h->graph.n > 0) {
     const int ev = timed_begin(h, kTagMisc);
-    if (h->p64) {
-      k_age_stamps<true><<<grid_for(h->n, 256), 256, 0, h->stream>>>(h->n, h->labg.p, iter & 1u);
+    if (h->round.p64) {
+      k_age_stamps<true><<<grid_for(h->graph.n, 256), 256, 0, h->stream>>>(h->graph.n, h->lp.labg.p, iter & 1u);
     } else {
-      k_age_stamps<false><<<grid_for(h->n, 256), 256, 0, h->stream>>>(h->n, h->labg.p, iter & 1u);
+      k_age_stamps<false><<<grid_for(h->graph.n, 256), 256, 0, h->stream>>>(h->graph.n, h->lp.labg.p, iter & 1u);
     }
     timed_end(h, ev);
-    ++h->kernel_launches;
+    ++h->counts.kernel_launches;
   }
   return KMP_OK;
 }
@@ -1599,11 +1689,11 @@ int begin_iteration(kmp_lp_handle *h, uint32_t iter) {
 // The accepted moves of the round into *moved (one host wait), and into the history choose_activation reads.
 int end_iteration(kmp_lp_handle *h, uint32_t *moved) {
   uint32_t host[2] = {0, 0};
-  KMP_CUDA(cudaMemcpyAsync(host, h->ctr32.p, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+  KMP_CUDA(cudaMemcpyAsync(host, h->commit.ctr32.p, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
   KMP_CUDA(cudaStreamSynchronize(h->stream));
   *moved = host[1];
-  h->moved_hist[1] = h->moved_hist[0];
-  h->moved_hist[0] = host[1];
+  h->round.moved_hist[1] = h->round.moved_hist[0];
+  h->round.moved_hist[0] = host[1];
   return KMP_OK;
 }
 
@@ -1660,22 +1750,22 @@ int dist_sweep_pack(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t 
   const uint32_t cap = subround_cap(h, q);
   // library path: the sweeps write their proposals straight into the send buffer (count in word 0, zeroed by the
   // previous commit / begin_iteration) -- no pack kernel
-  h->direct_send = (d_send == h->dist_send.p && h->comm != nullptr) ? d_send : nullptr;
-  h->direct_cap = cap;
-  h->stepping = true;
+  h->dist.direct_send = (d_send == h->dist.send.p && h->dist.comm != nullptr) ? d_send : nullptr;
+  h->dist.direct_cap = cap;
+  h->round.stepping = true;
   const int r = sweep_subround(h, rc, iter, sg, q);
-  h->stepping = false;
-  const bool direct = h->direct_send != nullptr;
-  h->direct_send = nullptr;
+  h->round.stepping = false;
+  const bool direct = h->dist.direct_send != nullptr;
+  h->dist.direct_send = nullptr;
   if (r != KMP_OK) {
     return r;
   }
   if (direct) {
     return KMP_OK;
   }
-  k_pack_movers<<<capped(h, grid_for(cap, 256, kSMs * 4)), 256, 0, h->stream>>>(h->mv_u.p, h->mv_t.p,
-                                                                      h->ctr32.p + (h->mover_parity ? 3 : 0), cap, d_send);
-  ++h->kernel_launches;
+  k_pack_movers<<<capped(h, grid_for(cap, 256, kSMs * 4)), 256, 0, h->stream>>>(h->commit.mv_u.p, h->commit.mv_t.p,
+                                                                      h->commit.ctr32.p + (h->round.mover_parity ? 3 : 0), cap, d_send);
+  ++h->counts.kernel_launches;
   KMP_CUDA(cudaGetLastError());
   return KMP_OK;
 }
@@ -1708,26 +1798,26 @@ bool configure_low_groups(kmp_lp_handle *h, int sms) {
 // The clusterer on one GPU; the sharded run, the refiner and the stepping API keep the per-sub-round path (a sweep
 // launch and a commit launch per sub-round).
 bool can_run_low_groups(const kmp_lp_handle *h, const RunCtx &rc) {
-  return rc.mode == 0 && h->world == 1 && !h->stepping;
+  return rc.mode == 0 && h->dist.world == 1 && !h->round.stepping;
 }
 static_assert(kMaxSubrounds <= kLowMaxSubrounds, "ensure_lists admits more sub-rounds than LowGroupArgs holds");
 // All sub-rounds of degree group `group` (0: tier 0, 1: tiers 1-2) of LP round `iter`, in sub-round order, with the
 // hashes, stamp windows, move stamps and proposal-counter parities the per-sub-round path uses.
 int run_low_group(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, int group) {
-  const uint32_t S = h->lists_S;
+  const uint32_t S = h->lists.S;
   const int ta = first_tier_of_group(group), tb = last_tier_of_group(group);
   SweepArgs sa = make_sweep_args(h, rc);
   sa.base_tie = sync_base(h->cfg.seed, h->call_counter, iter, SALT_TIE);
   sa.base_fav = sync_base(h->cfg.seed, h->call_counter, iter, SALT_FAV);
   sa.accumulate = true;
-  sa.pull = h->pull_this;
-  sa.list = h->order.p;
+  sa.pull = h->round.pull_this;
+  sa.list = h->lists.order.p;
   CommitArgs ca = make_commit_args(h, rc);
   LowGroupArgs g{};
-  g.push = !h->pull_this || !h->pull_next;
-  g.ctr32 = h->ctr32.p;
-  g.counters[0] = h->ctr64.p + ta;
-  g.counters[1] = h->ctr64.p + tb;
+  g.push = !h->round.pull_this || !h->round.pull_next;
+  g.ctr32 = h->commit.ctr32.p;
+  g.counters[0] = h->commit.ctr64.p + ta;
+  g.counters[1] = h->commit.ctr64.p + tb;
   uint32_t max_total = 0;
   for (uint32_t s = 0; s < S; ++s) {
     const uint32_t sg = static_cast<uint32_t>(group) * S + s;
@@ -1736,50 +1826,50 @@ int run_low_group(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, int group) 
       continue;
     }
     LowSubround &x = g.sub[g.num_sub++];
-    x.off[0] = h->list_off[ta * S + s];
+    x.off[0] = h->lists.off[ta * S + s];
     x.size[0] = q.size[ta];
-    x.off[1] = h->list_off[tb * S + s];
+    x.off[1] = h->lists.off[tb * S + s];
     x.size[1] = tb != ta ? q.size[tb] : 0u;
     const StampWindow w = make_window(iter, sg);
     x.window_start = w.start;
     x.window_len = w.len;
     x.base_commit = sync_base(h->cfg.seed, h->call_counter, iter * 4096 + sg, SALT_COMMIT);
-    x.stamp = h->stamps_ok ? make_stamp(iter, sg) : 0u;
-    x.parity = h->mover_parity;
-    h->mover_parity ^= 1u;
+    x.stamp = h->lists.stamps_ok ? make_stamp(iter, sg) : 0u;
+    x.parity = h->round.mover_parity;
+    h->round.mover_parity ^= 1u;
     max_total = std::max(max_total, q.total);
   }
   if (g.num_sub == 0) {
     return KMP_OK;
   }
-  const bool ew = h->adjwgt != nullptr;
-  const uint32_t blocks = capped(h, std::min<uint32_t>(grid_for(max_total, 256), h->low_blocks[group][ew][h->p64]));
+  const bool ew = h->graph.adjwgt != nullptr;
+  const uint32_t blocks = capped(h, std::min<uint32_t>(grid_for(max_total, 256), h->low_blocks[group][ew][h->round.p64]));
   GridBarrier bar{h->grid_bar.p, h->grid_bar.p + 1};
   void *args[] = {&sa, &ca, &g, &bar};
   // timing mode: the group's sweeps AND commits are this one event pair, under the group's first tier
   const int ev = timed_begin(h, ta);
-  KMP_CUDA(cudaLaunchCooperativeKernel(low_group_kernel(ew, h->p64, group), dim3(blocks), dim3(256), args, 0, h->stream));
+  KMP_CUDA(cudaLaunchCooperativeKernel(low_group_kernel(ew, h->round.p64, group), dim3(blocks), dim3(256), args, 0, h->stream));
   timed_end(h, ev);
-  ++h->kernel_launches;
-  ++h->sweep_launches;
-  ++h->group_launches[ta];
+  ++h->counts.kernel_launches;
+  ++h->counts.sweep_launches;
+  ++h->counts.group_launches[ta];
   return KMP_OK;
 }
 
 // One LP round over all (group, sub-round) lists. Returns via *moved the accepted moves.
 int run_iteration(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t *moved) {
-  const uint32_t S = h->lists_S;
+  const uint32_t S = h->lists.S;
   int rc0 = begin_iteration(h, iter);
   if (rc0 != KMP_OK) {
     return rc0;
   }
-  if (h->world > 1) { // exchange buffers for the largest sub-round, allocated once
+  if (h->dist.world > 1) { // exchange buffers for the largest sub-round, allocated once
     size_t max_words = 4;
     for (uint32_t sg = 0; sg < kNumGroups * S; ++sg) {
       max_words = std::max<size_t>(max_words, 4 + 2 * static_cast<size_t>(subround_cap(h, subround_of_sg(h, sg))));
     }
-    KMP_CUDA(h->dist_send.ensure(max_words));
-    KMP_CUDA(h->dist_recv.ensure(std::max<size_t>(max_words * h->world, h->n)));
+    KMP_CUDA(h->dist.send.ensure(max_words));
+    KMP_CUDA(h->dist.recv.ensure(std::max<size_t>(max_words * h->dist.world, h->graph.n)));
   }
   for (uint32_t sg = 0; sg < kNumGroups * S; ++sg) {
     const SubRound q = subround_of_sg(h, sg);
@@ -1787,14 +1877,14 @@ int run_iteration(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t *m
       continue;
     }
     int rc2;
-    if (h->world > 1) { // sharded: sweep the own slice, all-gather the proposals (NVLink), replicated commit
+    if (h->dist.world > 1) { // sharded: sweep the own slice, all-gather the proposals (NVLink), replicated commit
       const size_t words = 4 + 2 * static_cast<size_t>(subround_cap(h, q));
-      rc2 = dist_sweep_pack(h, rc, iter, sg, q, h->dist_send.p);
+      rc2 = dist_sweep_pack(h, rc, iter, sg, q, h->dist.send.p);
       if (rc2 != KMP_OK) {
         return rc2;
       }
-      KMP_NCCL(g_nccl.AllGather(h->dist_send.p, h->dist_recv.p, words, ncclUint32, h->comm, h->stream));
-      rc2 = commit_subround(h, rc, iter, sg, q, h->dist_recv.p);
+      KMP_NCCL(g_nccl.AllGather(h->dist.send.p, h->dist.recv.p, words, ncclUint32, h->dist.comm, h->stream));
+      rc2 = commit_subround(h, rc, iter, sg, q, h->dist.recv.p);
       if (rc2 != KMP_OK) {
         return rc2;
       }
@@ -1822,24 +1912,26 @@ int run_iteration(kmp_lp_handle *h, const RunCtx &rc, uint32_t iter, uint32_t *m
 
 // packed gather array: word width by the label range; (re)allocated grow-only
 int prepare_labg(kmp_lp_handle *h, uint32_t num_labels) {
-  h->p64 = num_labels > (1u << 24) || h->force_p64; // KMP_FORCE_P64=1: the 8-byte gather words on small test inputs
-  KMP_CUDA(h->labg.ensure(static_cast<size_t>(std::max<uint32_t>(h->n, 1)) * (h->p64 ? 8 : 4)));
+  h->round.p64 = num_labels > (1u << 24) || h->force_p64; // KMP_FORCE_P64=1: the 8-byte gather words on small test inputs
+  KMP_CUDA(h->lp.labg.ensure(static_cast<size_t>(std::max<uint32_t>(h->graph.n, 1)) * (h->round.p64 ? 8 : 4)));
   return KMP_OK;
 }
 void launch_init_cluster(kmp_lp_handle *h) {
-  if (h->p64) {
-    k_init_cluster<true><<<grid_for(h->n, 256), 256, 0, h->stream>>>(h->n, h->vwgt, h->label.p, h->labg.p, h->weight.p,
-                                                                       h->favored.p, h->active.p);
+  if (h->round.p64) {
+    k_init_cluster<true><<<grid_for(h->graph.n, 256), 256, 0, h->stream>>>(h->graph.n, h->graph.vwgt, h->lp.label.p,
+                                                                             h->lp.labg.p, h->lp.weight.p,
+                                                                             h->lp.favored.p, h->lp.active.p);
   } else {
-    k_init_cluster<false><<<grid_for(h->n, 256), 256, 0, h->stream>>>(h->n, h->vwgt, h->label.p, h->labg.p, h->weight.p,
-                                                                        h->favored.p, h->active.p);
+    k_init_cluster<false><<<grid_for(h->graph.n, 256), 256, 0, h->stream>>>(h->graph.n, h->graph.vwgt, h->lp.label.p,
+                                                                              h->lp.labg.p, h->lp.weight.p,
+                                                                              h->lp.favored.p, h->lp.active.p);
   }
 }
 void launch_pack_labels(kmp_lp_handle *h) {
-  if (h->p64) {
-    k_pack_labels<true><<<grid_for(h->n, 256), 256, 0, h->stream>>>(h->n, h->label.p, h->labg.p);
+  if (h->round.p64) {
+    k_pack_labels<true><<<grid_for(h->graph.n, 256), 256, 0, h->stream>>>(h->graph.n, h->lp.label.p, h->lp.labg.p);
   } else {
-    k_pack_labels<false><<<grid_for(h->n, 256), 256, 0, h->stream>>>(h->n, h->label.p, h->labg.p);
+    k_pack_labels<false><<<grid_for(h->graph.n, 256), 256, 0, h->stream>>>(h->graph.n, h->lp.label.p, h->lp.labg.p);
   }
 }
 
@@ -1847,10 +1939,10 @@ void launch_pack_labels(kmp_lp_handle *h) {
 // labels >= k (e.g. a clustering left on the device, or a host partition with an id >= k) are refused before any
 // kernel indexes a [k] array by a label. bad: a zeroed device counter. One n-sized read and one host wait.
 int checked_block_weights(kmp_lp_handle *h, uint32_t k, unsigned long long *bad) {
-  const uint32_t n = h->n;
+  const uint32_t n = h->graph.n;
   if (n > 0) {
-    bal_block_weights<<<capped(h, grid_for(n, 256)), 256, 0, h->stream>>>(n, k, h->vwgt, h->label.p, h->weight.p, bad);
-    ++h->kernel_launches;
+    bal_block_weights<<<capped(h, grid_for(n, 256)), 256, 0, h->stream>>>(n, k, h->graph.vwgt, h->lp.label.p, h->lp.weight.p, bad);
+    ++h->counts.kernel_launches;
   }
   unsigned long long b = 0;
   KMP_CUDA(cudaMemcpyAsync(&b, bad, sizeof(b), cudaMemcpyDeviceToHost, h->stream));
@@ -1866,25 +1958,25 @@ int checked_block_weights(kmp_lp_handle *h, uint32_t k, unsigned long long *bad)
 // caller runs last so that its host wait covers this set-up.
 int load_partition(kmp_lp_handle *h, uint32_t k, const uint32_t *partition, const int32_t *max_block_weights,
                    const int32_t *min_block_weights) {
-  const uint32_t n = h->n;
-  KMP_CUDA(h->label.ensure(n));
-  KMP_CUDA(h->weight.ensure(k));
-  KMP_CUDA(h->maxw.ensure(k));
+  const uint32_t n = h->graph.n;
+  KMP_CUDA(h->lp.label.ensure(n));
+  KMP_CUDA(h->lp.weight.ensure(k));
+  KMP_CUDA(h->lp.maxw.ensure(k));
   if (partition != nullptr) {
-    KMP_CUDA(cudaMemcpyAsync(h->label.p, partition, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, h->stream));
-    h->labels_valid = true;
+    KMP_CUDA(cudaMemcpyAsync(h->lp.label.p, partition, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, h->stream));
+    h->lp.labels_valid = true;
   }
-  KMP_CUDA(cudaMemcpyAsync(h->maxw.p, max_block_weights, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, h->stream));
+  KMP_CUDA(cudaMemcpyAsync(h->lp.maxw.p, max_block_weights, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, h->stream));
   if (min_block_weights != nullptr) {
-    KMP_CUDA(h->minw.ensure(k));
-    KMP_CUDA(cudaMemcpyAsync(h->minw.p, min_block_weights, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, h->stream));
+    KMP_CUDA(h->lp.minw.ensure(k));
+    KMP_CUDA(cudaMemcpyAsync(h->lp.minw.p, min_block_weights, static_cast<size_t>(k) * 4, cudaMemcpyHostToDevice, h->stream));
   }
-  KMP_CUDA(cudaMemsetAsync(h->weight.p, 0, static_cast<size_t>(k) * 4, h->stream));
+  KMP_CUDA(cudaMemsetAsync(h->lp.weight.p, 0, static_cast<size_t>(k) * 4, h->stream));
   return KMP_OK;
 }
 
 int refuse_without_labels(const kmp_lp_handle *h) {
-  if (!h->labels_valid) {
+  if (!h->lp.labels_valid) {
     return fail(KMP_ERR_INVALID, "no labels of the current graph on the device: cluster, pass a partition or call "
                                  "kmp_lp_upload_partition first");
   }
@@ -1893,7 +1985,7 @@ int refuse_without_labels(const kmp_lp_handle *h) {
 
 // The calls that run on one GPU only (the balancers, the overlay) refuse sharded, NCCL and open stepping handles.
 int refuse_multi_gpu(const kmp_lp_handle *h, const char *what) {
-  if (h->world > 1 || h->comm != nullptr || h->step_open) {
+  if (h->dist.world > 1 || h->dist.comm != nullptr || h->step.open) {
     return fail(KMP_ERR_UNSUPPORTED,
                 std::string(what) + " runs on one GPU: sharded, NCCL and stepping handles are refused");
   }
@@ -1901,58 +1993,52 @@ int refuse_multi_gpu(const kmp_lp_handle *h, const char *what) {
 }
 
 int begin_call(kmp_lp_handle *h, kmp_lp_stats *stats) {
-  if (h == nullptr || !h->have_graph) {
+  if (h == nullptr || !h->graph.present) {
     return fail(KMP_ERR_INVALID, "no graph set");
   }
   KMP_CUDA(cudaSetDevice(h->device));
   if (stats != nullptr) {
     std::memset(stats, 0, sizeof(*stats));
   }
-  h->kernel_launches = 0;
-  h->sweep_launches = 0;
-  h->pull_rounds = h->push_rounds = 0;
-  h->sweep_events_used = 0;
-  for (int g = 0; g < kStatTiers; ++g) {
-    h->group_launches[g] = 0;
-  }
-  KMP_CUDA(cudaEventRecord(h->ev_begin, h->stream));
+  h->counts = {};
+  KMP_CUDA(cudaEventRecord(h->streams.ev_begin, h->stream));
   return KMP_OK;
 }
 
 int end_call(kmp_lp_handle *h, kmp_lp_stats *stats) {
-  if (h->world > 1 && h->comm != nullptr && stats != nullptr) { // every rank reports the whole job's scan counters
-    KMP_NCCL(g_nccl.AllReduce(h->ctr64.p, h->ctr64.p, kCtrNodes + kStatTiers, ncclUint64, ncclSum, h->comm, h->stream));
+  if (h->dist.world > 1 && h->dist.comm != nullptr && stats != nullptr) { // every rank reports the whole job's scan counters
+    KMP_NCCL(g_nccl.AllReduce(h->commit.ctr64.p, h->commit.ctr64.p, kCtrNodes + kStatTiers, ncclUint64, ncclSum, h->dist.comm, h->stream));
   }
-  KMP_CUDA(cudaEventRecord(h->ev_end, h->stream));
+  KMP_CUDA(cudaEventRecord(h->streams.ev_end, h->stream));
   KMP_CUDA(cudaStreamSynchronize(h->stream));
   if (stats != nullptr) {
     unsigned long long c[kCtrNodes + kStatTiers] = {0};
-    KMP_CUDA(cudaMemcpy(c, h->ctr64.p, sizeof(c), cudaMemcpyDeviceToHost));
+    KMP_CUDA(cudaMemcpy(c, h->commit.ctr64.p, sizeof(c), cudaMemcpyDeviceToHost));
     for (int g = 0; g < kStatTiers; ++g) {
       stats->group_edges[g] = c[g];
       stats->group_nodes[g] = c[kCtrNodes + g];
-      stats->group_launches[g] = h->group_launches[g];
+      stats->group_launches[g] = h->counts.group_launches[g];
       stats->edges_scanned += c[g];
       stats->nodes_visited += c[kCtrNodes + g];
     }
     float ms = 0.f;
-    cudaEventElapsedTime(&ms, h->ev_begin, h->ev_end);
+    cudaEventElapsedTime(&ms, h->streams.ev_begin, h->streams.ev_end);
     stats->device_ms = ms;
     float sweep = 0.f;
-    for (size_t i = 0; i < h->sweep_events_used; ++i) {
+    for (size_t i = 0; i < h->counts.sweep_events_used; ++i) {
       float t = 0.f;
-      cudaEventElapsedTime(&t, h->sweep_events[i].first, h->sweep_events[i].second);
-      if (h->sweep_event_group[i] < kNumTiers) {
+      cudaEventElapsedTime(&t, h->streams.sweep_events[i].first, h->streams.sweep_events[i].second);
+      if (h->streams.sweep_event_group[i] < kNumTiers) {
         sweep += t;
       }
-      stats->group_sweep_ms[h->sweep_event_group[i]] += t;
+      stats->group_sweep_ms[h->streams.sweep_event_group[i]] += t;
       (void)kTagPush;
     }
     stats->sweep_ms = sweep;
-    stats->sweep_launches = h->sweep_launches;
-    stats->kernel_launches = h->kernel_launches;
-    stats->pull_rounds = h->pull_rounds;
-    stats->push_rounds = h->push_rounds;
+    stats->sweep_launches = h->counts.sweep_launches;
+    stats->kernel_launches = h->counts.kernel_launches;
+    stats->pull_rounds = h->counts.pull_rounds;
+    stats->push_rounds = h->counts.push_rounds;
   }
   return KMP_OK;
 }
@@ -1967,33 +2053,34 @@ int upload_optional_u32(kmp_lp_handle *h, DevBuf<uint32_t> &buf, const uint32_t 
 }
 
 int cluster_post_passes(kmp_lp_handle *h, int32_t max_w, uint32_t num_clusters, kmp_lp_stats *stats) {
-  const uint32_t n = h->n;
+  const uint32_t n = h->graph.n;
   const bool two_hop = (1.0 - 1.0 * num_clusters / n) <= h->cfg.two_hop_threshold; // lp_clusterer.cc:164-166
   const int iso = h->cfg.isolated_nodes_strategy;
   const bool iso_match = iso == KMP_ISOLATED_MATCH || (iso == KMP_ISOLATED_MATCH_DURING_TWO_HOP && two_hop);
   const bool iso_cluster = iso == KMP_ISOLATED_CLUSTER || (iso == KMP_ISOLATED_CLUSTER_DURING_TWO_HOP && two_hop);
   auto sort_pairs = [&](uint32_t cnt, int bits) { // pairs_a -> pairs_b, ascending
     return cub_call(h, [&](void *tmp, size_t &bytes) {
-      return cub::DeviceRadixSort::SortKeys(tmp, bytes, h->pairs_a.p, h->pairs_b.p, static_cast<int>(cnt), 0, bits,
+      return cub::DeviceRadixSort::SortKeys(tmp, bytes, h->ops.pairs_a.p, h->ops.pairs_b.p, static_cast<int>(cnt), 0, bits,
                                             h->stream);
     });
   };
-  if ((iso_match || iso_cluster) && h->num_isolated > 1) {
-    KMP_CUDA(h->pairs_a.ensure(h->num_isolated));
-    KMP_CUDA(h->pairs_b.ensure(h->num_isolated));
-    reset_u32<<<1, 1, 0, h->stream>>>(h->ctr32.p + 2);
-    k_collect_isolated<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->xadj, h->pairs_a.p, h->ctr32.p + 2);
+  if ((iso_match || iso_cluster) && h->graph.num_isolated > 1) {
+    KMP_CUDA(h->ops.pairs_a.ensure(h->graph.num_isolated));
+    KMP_CUDA(h->ops.pairs_b.ensure(h->graph.num_isolated));
+    reset_u32<<<1, 1, 0, h->stream>>>(h->commit.ctr32.p + 2);
+    k_collect_isolated<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->graph.xadj, h->ops.pairs_a.p, h->commit.ctr32.p + 2);
     uint32_t iso_cnt = 0;
-    KMP_CUDA(cudaMemcpyAsync(&iso_cnt, h->ctr32.p + 2, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+    KMP_CUDA(cudaMemcpyAsync(&iso_cnt, h->commit.ctr32.p + 2, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
     KMP_CUDA(cudaStreamSynchronize(h->stream));
     if (iso_cnt > 1) {
       KMP_CUDA(sort_pairs(iso_cnt, 32)); // key 0: ascending vertex id
       if (iso_match) {
-        k_match_isolated<<<grid_for(iso_cnt / 2 + 1, 256), 256, 0, h->stream>>>(iso_cnt, h->pairs_b.p, h->label.p, h->weight.p, max_w);
+        k_match_isolated<<<grid_for(iso_cnt / 2 + 1, 256), 256, 0, h->stream>>>(iso_cnt, h->ops.pairs_b.p, h->lp.label.p,
+                                                                                h->lp.weight.p, max_w);
       } else {
-        k_next_fit<<<1, 256, 0, h->stream>>>(iso_cnt, h->pairs_b.p, h->label.p, h->weight.p, max_w); // one group
+        k_next_fit<<<1, 256, 0, h->stream>>>(iso_cnt, h->ops.pairs_b.p, h->lp.label.p, h->lp.weight.p, max_w); // one group
       }
-      h->kernel_launches += 3;
+      h->counts.kernel_launches += 3;
       KMP_CUDA(cudaGetLastError());
     }
   }
@@ -2003,30 +2090,30 @@ int cluster_post_passes(kmp_lp_handle *h, int32_t max_w, uint32_t num_clusters, 
   if (stats != nullptr) {
     stats->two_hop_ran = 1;
   }
-  KMP_CUDA(h->pairs_a.ensure(n));
-  KMP_CUDA(h->pairs_b.ensure(n));
-  reset_u32<<<1, 1, 0, h->stream>>>(h->ctr32.p + 2);
-  k_collect_two_hop<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->xadj, h->vwgt, h->label.p, h->weight.p,
-                                                              h->favored.p, max_w, h->pairs_a.p, h->ctr32.p + 2);
+  KMP_CUDA(h->ops.pairs_a.ensure(n));
+  KMP_CUDA(h->ops.pairs_b.ensure(n));
+  reset_u32<<<1, 1, 0, h->stream>>>(h->commit.ctr32.p + 2);
+  k_collect_two_hop<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->graph.xadj, h->graph.vwgt, h->lp.label.p, h->lp.weight.p,
+                                                              h->lp.favored.p, max_w, h->ops.pairs_a.p, h->commit.ctr32.p + 2);
   uint32_t cnt = 0;
-  KMP_CUDA(cudaMemcpyAsync(&cnt, h->ctr32.p + 2, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+  KMP_CUDA(cudaMemcpyAsync(&cnt, h->commit.ctr32.p + 2, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
   KMP_CUDA(cudaStreamSynchronize(h->stream));
   if (cnt > 1) {
     KMP_CUDA(sort_pairs(cnt, 64));
     if (h->cfg.two_hop_strategy == KMP_TWO_HOP_CLUSTER_THREADWISE) {
-      k_next_fit<<<grid_for(static_cast<uint64_t>(cnt) * 32, 256, kSMs * 8), 256, 0, h->stream>>>(cnt, h->pairs_b.p, h->label.p,
-                                                                                                 h->weight.p, max_w);
-      h->kernel_launches += 3;
+      k_next_fit<<<grid_for(static_cast<uint64_t>(cnt) * 32, 256, kSMs * 8), 256, 0, h->stream>>>(cnt, h->ops.pairs_b.p, h->lp.label.p,
+                                                                                                 h->lp.weight.p, max_w);
+      h->counts.kernel_launches += 3;
     } else {
       // group heads: reuse mv-independent scratch (pairs_a is free after the sort)
-      uint32_t *head_in = reinterpret_cast<uint32_t *>(h->pairs_a.p);
+      uint32_t *head_in = reinterpret_cast<uint32_t *>(h->ops.pairs_a.p);
       uint32_t *head_out = head_in + cnt;
-      k_two_hop_heads<<<grid_for(cnt, 256), 256, 0, h->stream>>>(cnt, h->pairs_b.p, head_in);
+      k_two_hop_heads<<<grid_for(cnt, 256), 256, 0, h->stream>>>(cnt, h->ops.pairs_b.p, head_in);
       KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
         return cub::DeviceScan::InclusiveScan(tmp, bytes, head_in, head_out, MaxOp(), static_cast<int>(cnt), h->stream);
       }));
-      k_match_two_hop<<<grid_for(cnt, 256), 256, 0, h->stream>>>(cnt, h->pairs_b.p, head_out, h->label.p, h->weight.p);
-      h->kernel_launches += 5;
+      k_match_two_hop<<<grid_for(cnt, 256), 256, 0, h->stream>>>(cnt, h->ops.pairs_b.p, head_out, h->lp.label.p, h->lp.weight.p);
+      h->counts.kernel_launches += 5;
     }
     KMP_CUDA(cudaGetLastError());
   }
@@ -2039,28 +2126,28 @@ int begin_cluster_run(kmp_lp_handle *h, int32_t max_cluster_weight, const uint32
   if (h->cfg.sync_commit_passes > 1) { // the cluster commit kernels decide in one pass: no departure credit
     return fail(KMP_ERR_UNSUPPORTED, "the clusterer's sync commit is single-pass (sync_commit_passes must be 1)");
   }
-  const uint32_t n = h->n;
+  const uint32_t n = h->graph.n;
   int rc = ensure_lists(h);
   if (rc != KMP_OK) {
     return rc;
   }
-  KMP_CUDA(h->label.ensure(n));
-  KMP_CUDA(h->favored.ensure(n));
-  KMP_CUDA(h->weight.ensure(n));
+  KMP_CUDA(h->lp.label.ensure(n));
+  KMP_CUDA(h->lp.favored.ensure(n));
+  KMP_CUDA(h->lp.weight.ensure(n));
   rc = ensure_scratch(h, 0, n);
   if (rc == KMP_OK) {
     rc = prepare_labg(h, n);
   }
   if (rc == KMP_OK) {
-    rc = upload_optional_u32(h, h->communities, communities, n);
+    rc = upload_optional_u32(h, h->lp.communities, communities, n);
   }
   if (rc != KMP_OK) {
     return rc;
   }
-  KMP_CUDA(cudaMemsetAsync(h->ctr64.p, 0, kCtrSize * sizeof(unsigned long long), h->stream));
+  KMP_CUDA(cudaMemsetAsync(h->commit.ctr64.p, 0, kCtrSize * sizeof(unsigned long long), h->stream));
   if (n > 0) {
     launch_init_cluster(h);
-    ++h->kernel_launches;
+    ++h->counts.kernel_launches;
   }
   *ctx = RunCtx{0, n, max_cluster_weight, false, communities != nullptr};
   return KMP_OK;
@@ -2070,7 +2157,7 @@ int begin_cluster_run(kmp_lp_handle *h, int32_t max_cluster_weight, const uint32
 // written only when the set-up succeeds.
 int begin_refine_run(kmp_lp_handle *h, uint32_t k, const int32_t *max_block_weights, const int32_t *min_block_weights,
                      const uint32_t *communities, const uint32_t *partition, RunCtx *ctx) {
-  const uint32_t n = h->n;
+  const uint32_t n = h->graph.n;
   int rc = ensure_lists(h);
   if (rc == KMP_OK) {
     rc = ensure_scratch(h, 1, k);
@@ -2082,18 +2169,18 @@ int begin_refine_run(kmp_lp_handle *h, uint32_t k, const int32_t *max_block_weig
     rc = load_partition(h, k, partition, max_block_weights, min_block_weights);
   }
   if (rc == KMP_OK) {
-    rc = upload_optional_u32(h, h->communities, communities, n);
+    rc = upload_optional_u32(h, h->lp.communities, communities, n);
   }
   if (rc != KMP_OK) {
     return rc;
   }
-  KMP_CUDA(cudaMemsetAsync(h->ctr64.p, 0, kCtrSize * sizeof(unsigned long long), h->stream));
+  KMP_CUDA(cudaMemsetAsync(h->commit.ctr64.p, 0, kCtrSize * sizeof(unsigned long long), h->stream));
   if (n > 0) {
-    k_fill_u8<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->active.p, 1); // Base::initialize: all active
+    k_fill_u8<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->lp.active.p, 1); // Base::initialize: all active
     launch_pack_labels(h); // reads the labels without indexing by them
-    h->kernel_launches += 2;
+    h->counts.kernel_launches += 2;
   }
-  rc = checked_block_weights(h, k, h->ctr64.p + kCtrScratch); // last: its wait covers the set-up above
+  rc = checked_block_weights(h, k, h->commit.ctr64.p + kCtrScratch); // last: its wait covers the set-up above
   if (rc != KMP_OK) {
     return rc;
   }
@@ -2103,9 +2190,9 @@ int begin_refine_run(kmp_lp_handle *h, uint32_t k, const int32_t *max_block_weig
 
 // The clusters (labels of nonzero weight) of a non-empty graph: two launches, which the caller counts, and a host wait.
 int count_clusters(kmp_lp_handle *h, uint32_t *num_clusters) {
-  reset_u32<<<1, 1, 0, h->stream>>>(h->ctr32.p + 2);
-  k_count_nonzero<<<grid_for(h->n, 256), 256, 0, h->stream>>>(h->n, h->weight.p, h->ctr32.p + 2);
-  KMP_CUDA(cudaMemcpyAsync(num_clusters, h->ctr32.p + 2, 4, cudaMemcpyDeviceToHost, h->stream));
+  reset_u32<<<1, 1, 0, h->stream>>>(h->commit.ctr32.p + 2);
+  k_count_nonzero<<<grid_for(h->graph.n, 256), 256, 0, h->stream>>>(h->graph.n, h->lp.weight.p, h->commit.ctr32.p + 2);
+  KMP_CUDA(cudaMemcpyAsync(num_clusters, h->commit.ctr32.p + 2, 4, cudaMemcpyDeviceToHost, h->stream));
   KMP_CUDA(cudaStreamSynchronize(h->stream));
   return KMP_OK;
 }
@@ -2113,13 +2200,13 @@ int count_clusters(kmp_lp_handle *h, uint32_t *num_clusters) {
 // Clustering finish: the cluster count and the post passes. Every completed clustering, of an empty graph too,
 // advances the call index of the sync hashes.
 int finish_cluster_run(kmp_lp_handle *h, int32_t max_cluster_weight, kmp_lp_stats *stats) {
-  if (h->n > 0) {
+  if (h->graph.n > 0) {
     uint32_t num_clusters = 0;
     int rc = count_clusters(h, &num_clusters);
     if (rc != KMP_OK) {
       return rc;
     }
-    h->kernel_launches += 2;
+    h->counts.kernel_launches += 2;
     if (stats != nullptr) {
       stats->num_clusters = num_clusters;
     }
@@ -2129,61 +2216,61 @@ int finish_cluster_run(kmp_lp_handle *h, int32_t max_cluster_weight, kmp_lp_stat
     }
   }
   ++h->call_counter;
-  h->labels_valid = true;
+  h->lp.labels_valid = true;
   return KMP_OK;
 }
 
 // n labels into labels_out and k block weights into block_weights_out, each when non-null.
 int download_results(kmp_lp_handle *h, uint32_t *labels_out, int32_t *block_weights_out, uint32_t k) {
-  if (labels_out != nullptr && h->n > 0) {
-    KMP_CUDA(cudaMemcpyAsync(labels_out, h->label.p, static_cast<size_t>(h->n) * 4, cudaMemcpyDeviceToHost, h->stream));
+  if (labels_out != nullptr && h->graph.n > 0) {
+    KMP_CUDA(cudaMemcpyAsync(labels_out, h->lp.label.p, static_cast<size_t>(h->graph.n) * 4, cudaMemcpyDeviceToHost, h->stream));
   }
   if (block_weights_out != nullptr) {
-    KMP_CUDA(cudaMemcpyAsync(block_weights_out, h->weight.p, static_cast<size_t>(k) * 4, cudaMemcpyDeviceToHost, h->stream));
+    KMP_CUDA(cudaMemcpyAsync(block_weights_out, h->lp.weight.p, static_cast<size_t>(k) * 4, cudaMemcpyDeviceToHost, h->stream));
   }
   return KMP_OK;
 }
 
 // ---- schedule KMP_SCHEDULE_SEQ_STRICT ----------------------------------------------------------------
-// mode 0: labels are (re)initialised by the engine; mode 1: h->label holds the partition. Results stay in
-// h->label / h->weight; iteration statistics go to *stats, the scan counters to the last tier slot of ctr64.
+// mode 0: labels are (re)initialised by the engine; mode 1: h->lp.label holds the partition. Results stay in
+// h->lp.label / h->lp.weight; iteration statistics go to *stats, the scan counters to the last tier slot of ctr64.
 int run_strict(kmp_lp_handle *h, int mode, uint32_t num_keys, int32_t max_cluster_weight, uint32_t desired,
                uint32_t k, bool has_min, bool has_comm, kmp_lp_stats *stats) {
-  const size_t n = std::max<uint32_t>(h->n, 1);
+  const size_t n = std::max<uint32_t>(h->graph.n, 1);
   const size_t keys = std::max<size_t>(std::max<size_t>(num_keys, n), 1);
-  KMP_CUDA(h->favored.ensure(n));
-  KMP_CUDA(h->active.ensure(n));
-  KMP_CUDA(h->st_slot.ensure(keys));
-  KMP_CUDA(h->st_slot2.ensure(keys));
-  KMP_CUDA(h->st_concurrent.ensure(keys));
-  KMP_CUDA(h->st_used.ensure(keys));
-  KMP_CUDA(h->st_ent_key.ensure(keys + 1));
-  KMP_CUDA(h->st_ent_val.ensure(keys + 1));
-  KMP_CUDA(h->st_ent2_key.ensure(keys + 1));
-  KMP_CUDA(h->st_ent2_val.ensure(keys + 1));
-  KMP_CUDA(h->st_tie_best.ensure(keys + 1));
-  KMP_CUDA(h->st_tie_fav.ensure(keys + 1));
-  KMP_CUDA(h->st_second.ensure(n));
-  KMP_CUDA(h->st_chunks.ensure(2 * (n + 64)));
-  KMP_CUDA(h->st_sub_perm.ensure(n / 64 + 2));
-  KMP_CUDA(h->st_match.ensure(n));
-  KMP_CUDA(h->st_buckets.ensure(36));
-  KMP_CUDA(h->st_rng.ensure(1));
-  KMP_CUDA(h->st_stats.ensure(1));
-  if (!h->strict_seeded) { // Random::reseed + the RandomPermutations member of the LP object, once per object
-    kmp_strict::strict_seed_kernel<<<1, 32, 0, h->stream>>>(h->st_rng.p, h->cfg.seed);
-    h->strict_seeded = true;
-    ++h->kernel_launches;
+  KMP_CUDA(h->lp.favored.ensure(n));
+  KMP_CUDA(h->lp.active.ensure(n));
+  KMP_CUDA(h->strict.slot.ensure(keys));
+  KMP_CUDA(h->strict.slot2.ensure(keys));
+  KMP_CUDA(h->strict.concurrent.ensure(keys));
+  KMP_CUDA(h->strict.used.ensure(keys));
+  KMP_CUDA(h->strict.ent_key.ensure(keys + 1));
+  KMP_CUDA(h->strict.ent_val.ensure(keys + 1));
+  KMP_CUDA(h->strict.ent2_key.ensure(keys + 1));
+  KMP_CUDA(h->strict.ent2_val.ensure(keys + 1));
+  KMP_CUDA(h->strict.tie_best.ensure(keys + 1));
+  KMP_CUDA(h->strict.tie_fav.ensure(keys + 1));
+  KMP_CUDA(h->strict.second.ensure(n));
+  KMP_CUDA(h->strict.chunks.ensure(2 * (n + 64)));
+  KMP_CUDA(h->strict.sub_perm.ensure(n / 64 + 2));
+  KMP_CUDA(h->strict.match.ensure(n));
+  KMP_CUDA(h->strict.buckets.ensure(36));
+  KMP_CUDA(h->strict.rng.ensure(1));
+  KMP_CUDA(h->strict.stats.ensure(1));
+  if (!h->strict.seeded) { // Random::reseed + the RandomPermutations member of the LP object, once per object
+    kmp_strict::strict_seed_kernel<<<1, 32, 0, h->stream>>>(h->strict.rng.p, h->cfg.seed);
+    h->strict.seeded = true;
+    ++h->counts.kernel_launches;
   }
   kmp_strict::Args a{};
-  a.n = h->n;
-  a.m = h->m;
-  a.xadj = h->xadj;
-  a.adjncy = h->adjncy;
-  a.vwgt = h->vwgt;
-  a.adjwgt = h->adjwgt;
-  a.sorted = h->graph_sorted ? 1 : 0;
-  a.buckets = h->st_buckets.p;
+  a.n = h->graph.n;
+  a.m = h->graph.m;
+  a.xadj = h->graph.xadj;
+  a.adjncy = h->graph.adjncy;
+  a.vwgt = h->graph.vwgt;
+  a.adjwgt = h->graph.adjwgt;
+  a.sorted = h->graph.sorted ? 1 : 0;
+  a.buckets = h->strict.buckets.p;
   a.num_iterations = h->cfg.num_iterations;
   a.large_degree_threshold = h->cfg.large_degree_threshold;
   a.max_num_neighbors = h->cfg.max_num_neighbors;
@@ -2196,34 +2283,34 @@ int run_strict(kmp_lp_handle *h, int mode, uint32_t num_keys, int32_t max_cluste
   a.max_cluster_weight = max_cluster_weight;
   a.desired_num_clusters = desired;
   a.k = k;
-  a.max_bw = mode == 1 ? h->maxw.p : nullptr;
-  a.min_bw = has_min ? h->minw.p : nullptr;
-  a.communities = has_comm ? h->communities.p : nullptr;
-  a.label = h->label.p;
-  a.weight = h->weight.p;
-  a.favored = h->favored.p;
-  a.active = h->active.p;
-  a.slot = h->st_slot.p;
-  a.ent_key = h->st_ent_key.p;
-  a.ent_val = h->st_ent_val.p;
-  a.slot2 = h->st_slot2.p;
-  a.ent2_key = h->st_ent2_key.p;
-  a.ent2_val = h->st_ent2_val.p;
-  a.concurrent = h->st_concurrent.p;
-  a.used_entries = h->st_used.p;
-  a.second_phase_nodes = h->st_second.p;
-  a.tie_best = h->st_tie_best.p;
-  a.tie_fav = h->st_tie_fav.p;
-  a.chunks = h->st_chunks.p;
-  a.sub_perm = h->st_sub_perm.p;
-  a.match_map = h->st_match.p;
-  a.rng = h->st_rng.p;
-  a.stats = h->st_stats.p;
+  a.max_bw = mode == 1 ? h->lp.maxw.p : nullptr;
+  a.min_bw = has_min ? h->lp.minw.p : nullptr;
+  a.communities = has_comm ? h->lp.communities.p : nullptr;
+  a.label = h->lp.label.p;
+  a.weight = h->lp.weight.p;
+  a.favored = h->lp.favored.p;
+  a.active = h->lp.active.p;
+  a.slot = h->strict.slot.p;
+  a.ent_key = h->strict.ent_key.p;
+  a.ent_val = h->strict.ent_val.p;
+  a.slot2 = h->strict.slot2.p;
+  a.ent2_key = h->strict.ent2_key.p;
+  a.ent2_val = h->strict.ent2_val.p;
+  a.concurrent = h->strict.concurrent.p;
+  a.used_entries = h->strict.used.p;
+  a.second_phase_nodes = h->strict.second.p;
+  a.tie_best = h->strict.tie_best.p;
+  a.tie_fav = h->strict.tie_fav.p;
+  a.chunks = h->strict.chunks.p;
+  a.sub_perm = h->strict.sub_perm.p;
+  a.match_map = h->strict.match.p;
+  a.rng = h->strict.rng.p;
+  a.stats = h->strict.stats.p;
   kmp_strict::strict_kernel<<<1, 32, 0, h->stream>>>(a);
-  ++h->kernel_launches;
+  ++h->counts.kernel_launches;
   KMP_CUDA(cudaGetLastError());
   kmp_strict::Stats hs{};
-  KMP_CUDA(cudaMemcpyAsync(&hs, h->st_stats.p, sizeof(hs), cudaMemcpyDeviceToHost, h->stream));
+  KMP_CUDA(cudaMemcpyAsync(&hs, h->strict.stats.p, sizeof(hs), cudaMemcpyDeviceToHost, h->stream));
   KMP_CUDA(cudaStreamSynchronize(h->stream));
   if (stats != nullptr) {
     stats->iterations = hs.iterations;
@@ -2235,19 +2322,19 @@ int run_strict(kmp_lp_handle *h, int mode, uint32_t num_keys, int32_t max_cluste
   }
   // end_call sums the per-tier scan counters: park the engine's totals in tier slot 7
   unsigned long long c[2] = {hs.edges_scanned, hs.nodes_visited};
-  KMP_CUDA(cudaMemcpy(h->ctr64.p + (kStatTiers - 1), &c[0], 8, cudaMemcpyHostToDevice));
-  KMP_CUDA(cudaMemcpy(h->ctr64.p + kCtrNodes + (kStatTiers - 1), &c[1], 8, cudaMemcpyHostToDevice));
+  KMP_CUDA(cudaMemcpy(h->commit.ctr64.p + (kStatTiers - 1), &c[0], 8, cudaMemcpyHostToDevice));
+  KMP_CUDA(cudaMemcpy(h->commit.ctr64.p + kCtrNodes + (kStatTiers - 1), &c[1], 8, cudaMemcpyHostToDevice));
   return KMP_OK;
 }
 
 int strict_cluster(kmp_lp_handle *h, int32_t max_cluster_weight, uint32_t desired_num_clusters,
                    const uint32_t *communities, uint32_t *clustering_out, kmp_lp_stats *stats) {
-  const uint32_t n = h->n;
-  KMP_CUDA(h->label.ensure(std::max<uint32_t>(n, 1)));
-  KMP_CUDA(h->weight.ensure(std::max<uint32_t>(n, 1)));
-  KMP_CUDA(h->ctr64.ensure(kCtrSize));
-  KMP_CUDA(cudaMemsetAsync(h->ctr64.p, 0, kCtrSize * sizeof(unsigned long long), h->stream));
-  int rc = upload_optional_u32(h, h->communities, communities, n);
+  const uint32_t n = h->graph.n;
+  KMP_CUDA(h->lp.label.ensure(std::max<uint32_t>(n, 1)));
+  KMP_CUDA(h->lp.weight.ensure(std::max<uint32_t>(n, 1)));
+  KMP_CUDA(h->commit.ctr64.ensure(kCtrSize));
+  KMP_CUDA(cudaMemsetAsync(h->commit.ctr64.p, 0, kCtrSize * sizeof(unsigned long long), h->stream));
+  int rc = upload_optional_u32(h, h->lp.communities, communities, n);
   if (rc == KMP_OK) {
     rc = run_strict(h, 0, n, max_cluster_weight, desired_num_clusters, 0, false, communities != nullptr, stats);
   }
@@ -2258,25 +2345,25 @@ int strict_cluster(kmp_lp_handle *h, int32_t max_cluster_weight, uint32_t desire
     return rc;
   }
   ++h->call_counter;
-  h->labels_valid = true;
+  h->lp.labels_valid = true;
   return end_call(h, stats);
 }
 
 int strict_refine(kmp_lp_handle *h, uint32_t k, const int32_t *max_block_weights, const int32_t *min_block_weights,
                   const uint32_t *communities, uint32_t *partition_inout, int32_t *block_weights_out,
                   kmp_lp_stats *stats) {
-  const uint32_t n = h->n;
+  const uint32_t n = h->graph.n;
   // the engine's sizes, above the n labels and k weights load_partition ensures
-  KMP_CUDA(h->label.ensure(std::max<uint32_t>(n, 1)));
-  KMP_CUDA(h->weight.ensure(std::max<uint32_t>(std::max(n, k), 1)));
-  KMP_CUDA(h->ctr64.ensure(kCtrSize));
-  KMP_CUDA(cudaMemsetAsync(h->ctr64.p, 0, kCtrSize * sizeof(unsigned long long), h->stream));
+  KMP_CUDA(h->lp.label.ensure(std::max<uint32_t>(n, 1)));
+  KMP_CUDA(h->lp.weight.ensure(std::max<uint32_t>(std::max(n, k), 1)));
+  KMP_CUDA(h->commit.ctr64.ensure(kCtrSize));
+  KMP_CUDA(cudaMemsetAsync(h->commit.ctr64.p, 0, kCtrSize * sizeof(unsigned long long), h->stream));
   int rc = load_partition(h, k, partition_inout, max_block_weights, min_block_weights);
   if (rc == KMP_OK) {
-    rc = upload_optional_u32(h, h->communities, communities, n);
+    rc = upload_optional_u32(h, h->lp.communities, communities, n);
   }
   if (rc == KMP_OK) {
-    rc = checked_block_weights(h, k, h->ctr64.p + kCtrScratch); // the engine recomputes the weights itself
+    rc = checked_block_weights(h, k, h->commit.ctr64.p + kCtrScratch); // the engine recomputes the weights itself
   }
   if (rc == KMP_OK) {
     rc = run_strict(h, 1, k, 0, 0, k, min_block_weights != nullptr, communities != nullptr, stats);
@@ -2364,7 +2451,9 @@ int kmp_lp_create(const kmp_lp_config *cfg, kmp_lp_handle **out) {
       cfg->impl < KMP_LP_SINGLE_PHASE || cfg->impl > KMP_LP_GROWING_HASH_TABLES) {
     return fail(KMP_ERR_INVALID, "unknown two_hop_strategy / isolated_nodes_strategy / impl");
   }
-  kmp_lp_handle *h = new (std::nothrow) kmp_lp_handle();
+  // a refused call frees what was already created: the handle's members own their streams, events and buffers
+  std::unique_ptr<kmp_lp_handle> owner(new (std::nothrow) kmp_lp_handle());
+  kmp_lp_handle *h = owner.get();
   if (h == nullptr) {
     return fail(KMP_ERR_ALLOC, "out of host memory");
   }
@@ -2392,22 +2481,19 @@ int kmp_lp_create(const kmp_lp_config *cfg, kmp_lp_handle **out) {
     cudaGetDevice(&dev);
   }
   h->device = dev;
-  if (cudaSetDevice(dev) != cudaSuccess || cudaStreamCreateWithFlags(&h->owned_stream, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaEventCreate(&h->ev_begin) != cudaSuccess || cudaEventCreate(&h->ev_end) != cudaSuccess) {
-    delete h;
+  if (cudaSetDevice(dev) != cudaSuccess || cudaStreamCreateWithFlags(&h->streams.owned, cudaStreamNonBlocking) != cudaSuccess ||
+      cudaEventCreate(&h->streams.ev_begin) != cudaSuccess || cudaEventCreate(&h->streams.ev_end) != cudaSuccess) {
     return fail(KMP_ERR_CUDA, "failed to create stream/events");
   }
-  h->stream = h->owned_stream;
+  h->stream = h->streams.owned;
   h->sweep_stream = h->stream;
   for (int i = 0; i < 3; ++i) {
-    if (cudaStreamCreateWithFlags(&h->side_stream[i], cudaStreamNonBlocking) != cudaSuccess ||
-        cudaEventCreateWithFlags(&h->ev_join[i], cudaEventDisableTiming) != cudaSuccess) {
-      delete h;
-      return fail(KMP_ERR_CUDA, "failed to create side streams");
+    if (cudaStreamCreateWithFlags(&h->streams.side[i], cudaStreamNonBlocking) != cudaSuccess ||
+        cudaEventCreateWithFlags(&h->streams.ev_join[i], cudaEventDisableTiming) != cudaSuccess) {
+        return fail(KMP_ERR_CUDA, "failed to create side streams");
     }
   }
-  if (cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming) != cudaSuccess) {
-    delete h;
+  if (cudaEventCreateWithFlags(&h->streams.ev_fork, cudaEventDisableTiming) != cudaSuccess) {
     return fail(KMP_ERR_CUDA, "failed to create events");
   }
   if (const char *e = std::getenv("KMP_FORCE_P64")) {
@@ -2419,7 +2505,6 @@ int kmp_lp_create(const kmp_lp_config *cfg, kmp_lp_handle **out) {
   int coop = 0, per_sm = 0, per_sm_r = 0;
   cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
   if (coop == 0) {
-    delete h;
     return fail(KMP_ERR_CUDA, "this device does not support cooperative launches");
   }
   // co-resident CTAs of both commit kernels, the refiner's with its largest dynamic shared memory (kSmemPrivLimit ints)
@@ -2428,11 +2513,9 @@ int kmp_lp_create(const kmp_lp_config *cfg, kmp_lp_handle **out) {
       cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_r, commit_refine_fused<false>, 256, kSmemPrivLimit * 4) !=
           cudaSuccess ||
       per_sm_r < 1) {
-    delete h;
     return fail(KMP_ERR_CUDA, "a fused commit kernel cannot be resident on this device");
   }
   if (h->grid_bar.ensure(2) != cudaSuccess || cudaMemset(h->grid_bar.p, 0, 2 * sizeof(unsigned)) != cudaSuccess) {
-    delete h;
     return fail(KMP_ERR_CUDA, "failed to allocate the grid barrier");
   }
   // all co-resident CTAs: a sub-round of a 10^8-vertex graph commits 10^7 proposals, each a short chain of
@@ -2440,17 +2523,15 @@ int kmp_lp_create(const kmp_lp_config *cfg, kmp_lp_handle **out) {
   h->fused_blocks = sms * per_sm;
   h->fused_blocks_refine = sms * per_sm_r;
   if (!configure_low_groups(h, sms)) {
-    delete h;
     return fail(KMP_ERR_CUDA, "a persistent low-degree clustering kernel cannot be resident on this device");
   }
   if (!(configure_team_kernels<0, false, false>(h, sms) && configure_team_kernels<0, false, true>(h, sms) &&
         configure_team_kernels<0, true, false>(h, sms) && configure_team_kernels<0, true, true>(h, sms) &&
         configure_team_kernels<1, false, false>(h, sms) && configure_team_kernels<1, false, true>(h, sms) &&
         configure_team_kernels<1, true, false>(h, sms) && configure_team_kernels<1, true, true>(h, sms))) {
-    delete h;
     return fail(KMP_ERR_CUDA, "a sweep_team kernel cannot be resident on this device");
   }
-  *out = h;
+  *out = owner.release();
   return KMP_OK;
 }
 
@@ -2460,32 +2541,10 @@ int kmp_lp_destroy(kmp_lp_handle *h) {
   }
   cudaSetDevice(h->device);
   cudaStreamSynchronize(h->stream);
-  if (h->comm != nullptr) {
-    g_nccl.CommDestroy(h->comm);
-    h->comm = nullptr;
+  if (h->dist.comm != nullptr) {
+    g_nccl.CommDestroy(h->dist.comm);
   }
-  kmp_lp_free_scratch(h);
-  h->own_xadj.release();
-  h->own_adjncy.release();
-  h->own_vwgt.release();
-  h->own_adjwgt.release();
-  h->order.release();
-  for (auto &p : h->sweep_events) {
-    cudaEventDestroy(p.first);
-    cudaEventDestroy(p.second);
-  }
-  cudaEventDestroy(h->ev_begin);
-  cudaEventDestroy(h->ev_end);
-  if (h->ev_ct0 != nullptr) {
-    cudaEventDestroy(h->ev_ct0);
-    cudaEventDestroy(h->ev_ct1);
-  }
-  cudaEventDestroy(h->ev_fork);
-  for (int i = 0; i < 3; ++i) {
-    cudaEventDestroy(h->ev_join[i]);
-    cudaStreamDestroy(h->side_stream[i]);
-  }
-  cudaStreamDestroy(h->owned_stream);
+  kmp_lp_free_scratch(h); // trims the pool
   delete h;
   return KMP_OK;
 }
@@ -2502,15 +2561,15 @@ static int set_graph_common(kmp_lp_handle *h, uint32_t n, uint32_t m) {
   if (n > 0x7FFFFFFFu || m > 0x7FFFFFFFu) { // CUB scans / sorts take int counts; 32-bit EdgeID build of the reference
     return fail(KMP_ERR_UNSUPPORTED, "n and m must be below 2^31");
   }
-  h->n = n;
-  h->m = m;
-  h->have_graph = true;
-  ++h->graph_epoch;
-  h->labels_valid = false;
-  overlay_release(h, false); // stream-ordered: the stash belongs to the previous graph
-  h->lists_valid = false;
-  h->slot_state_clean = false;
-  h->graph_sorted = false;
+  h->graph.n = n;
+  h->graph.m = m;
+  h->graph.present = true;
+  ++h->graph.epoch;
+  h->lp.labels_valid = false;
+  h->ops.ov.stash.clear(); // the stash belongs to the previous graph; freed stream-ordered, after the work that reads it
+  h->lists.valid = false;
+  h->commit.slot_state_clean = false;
+  h->graph.sorted = false;
   if (h->cfg.schedule == KMP_SCHEDULE_SEQ_STRICT) {
     if (n > KMP_SEQ_STRICT_MAX_N) {
       return fail(KMP_ERR_UNSUPPORTED, "KMP_SCHEDULE_SEQ_STRICT is a one-thread-block schedule for n <= KMP_SEQ_STRICT_MAX_N");
@@ -2521,12 +2580,12 @@ static int set_graph_common(kmp_lp_handle *h, uint32_t n, uint32_t m) {
   if (rc != KMP_OK) {
     return rc;
   }
-  h->num_isolated = 0;
+  h->graph.num_isolated = 0;
   {
     // vertices in the tail bucket are either isolated or above the degree threshold; count isolated
     // ones exactly only when a post pass needs them (cheap: tail bucket size is an upper bound)
-    const uint32_t S = h->lists_S;
-    h->num_isolated = h->list_off[kNumTiers * S + 1] - h->list_off[kNumTiers * S];
+    const uint32_t S = h->lists.S;
+    h->graph.num_isolated = h->lists.off[kNumTiers * S + 1] - h->lists.off[kNumTiers * S];
   }
   return KMP_OK;
 }
@@ -2537,34 +2596,34 @@ int kmp_lp_set_graph(kmp_lp_handle *h, uint32_t n, uint32_t m, const uint32_t *x
     return fail(KMP_ERR_INVALID, "null argument");
   }
   KMP_CUDA(cudaSetDevice(h->device));
-  KMP_CUDA(h->own_xadj.ensure(static_cast<size_t>(n) + 1));
-  KMP_CUDA(h->own_adjncy.ensure(m));
+  KMP_CUDA(h->graph.own_xadj.ensure(static_cast<size_t>(n) + 1));
+  KMP_CUDA(h->graph.own_adjncy.ensure(m));
   // xadj first, on the handle's stream: the work lists only need the degrees and are built (kernels, a radix
   // pass, three small host round trips) while the m-sized arrays are still crossing PCIe on a side stream
   KMP_CUDA(cudaStreamSynchronize(h->stream)); // earlier work may still read the old arrays
-  KMP_CUDA(cudaMemcpyAsync(h->own_xadj.p, xadj, (static_cast<size_t>(n) + 1) * 4, cudaMemcpyHostToDevice, h->stream));
-  const cudaStream_t big = h->side_stream[0];
+  KMP_CUDA(cudaMemcpyAsync(h->graph.own_xadj.p, xadj, (static_cast<size_t>(n) + 1) * 4, cudaMemcpyHostToDevice, h->stream));
+  const cudaStream_t big = h->streams.side[0];
   if (m > 0) {
-    KMP_CUDA(cudaMemcpyAsync(h->own_adjncy.p, adjncy, static_cast<size_t>(m) * 4, cudaMemcpyHostToDevice, big));
+    KMP_CUDA(cudaMemcpyAsync(h->graph.own_adjncy.p, adjncy, static_cast<size_t>(m) * 4, cudaMemcpyHostToDevice, big));
   }
-  h->xadj = h->own_xadj.p;
-  h->adjncy = h->own_adjncy.p;
-  h->adjncy_16b = true; // cudaMalloc: 256-byte aligned
-  h->vwgt = nullptr;
-  h->adjwgt = nullptr;
+  h->graph.xadj = h->graph.own_xadj.p;
+  h->graph.adjncy = h->graph.own_adjncy.p;
+  h->graph.adjncy_16b = true; // cudaMalloc: 256-byte aligned
+  h->graph.vwgt = nullptr;
+  h->graph.adjwgt = nullptr;
   if (vwgt != nullptr) {
-    KMP_CUDA(h->own_vwgt.ensure(n));
-    KMP_CUDA(cudaMemcpyAsync(h->own_vwgt.p, vwgt, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, h->stream));
-    h->vwgt = h->own_vwgt.p;
+    KMP_CUDA(h->graph.own_vwgt.ensure(n));
+    KMP_CUDA(cudaMemcpyAsync(h->graph.own_vwgt.p, vwgt, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, h->stream));
+    h->graph.vwgt = h->graph.own_vwgt.p;
   }
   if (adjwgt != nullptr) {
-    KMP_CUDA(h->own_adjwgt.ensure(m));
-    KMP_CUDA(cudaMemcpyAsync(h->own_adjwgt.p, adjwgt, static_cast<size_t>(m) * 4, cudaMemcpyHostToDevice, big));
-    h->adjwgt = h->own_adjwgt.p;
+    KMP_CUDA(h->graph.own_adjwgt.ensure(m));
+    KMP_CUDA(cudaMemcpyAsync(h->graph.own_adjwgt.p, adjwgt, static_cast<size_t>(m) * 4, cudaMemcpyHostToDevice, big));
+    h->graph.adjwgt = h->graph.own_adjwgt.p;
   }
-  KMP_CUDA(cudaEventRecord(h->ev_join[0], big));
+  KMP_CUDA(cudaEventRecord(h->streams.ev_join[0], big));
   const int rc = set_graph_common(h, n, m);
-  KMP_CUDA(cudaStreamWaitEvent(h->stream, h->ev_join[0], 0)); // later work on the handle's stream sees the whole graph
+  KMP_CUDA(cudaStreamWaitEvent(h->stream, h->streams.ev_join[0], 0)); // later work on the handle's stream sees the whole graph
   return rc;
 }
 
@@ -2578,20 +2637,20 @@ int kmp_lp_set_graph_device(kmp_lp_handle *h, uint32_t n, uint32_t m, const uint
     return fail(KMP_ERR_INVALID, "device graph arrays must be 4-byte aligned");
   }
   KMP_CUDA(cudaSetDevice(h->device));
-  h->xadj = d_xadj;
-  h->adjncy = d_adjncy;
+  h->graph.xadj = d_xadj;
+  h->graph.adjncy = d_adjncy;
   // a view into a larger buffer may start anywhere: the hub tier then reads adjncy from global memory
-  h->adjncy_16b = (reinterpret_cast<uintptr_t>(d_adjncy) & 15u) == 0;
-  h->vwgt = d_vwgt;
-  h->adjwgt = d_adjwgt;
+  h->graph.adjncy_16b = (reinterpret_cast<uintptr_t>(d_adjncy) & 15u) == 0;
+  h->graph.vwgt = d_vwgt;
+  h->graph.adjwgt = d_adjwgt;
   return set_graph_common(h, n, m);
 }
 
 int kmp_lp_set_graph_sorted(kmp_lp_handle *h, int sorted) {
-  if (h == nullptr || !h->have_graph) {
+  if (h == nullptr || !h->graph.present) {
     return fail(KMP_ERR_INVALID, "no graph set");
   }
-  h->graph_sorted = sorted != 0;
+  h->graph.sorted = sorted != 0;
   return KMP_OK;
 }
 
@@ -2604,11 +2663,11 @@ int kmp_lp_cluster(kmp_lp_handle *h, int32_t max_cluster_weight, uint32_t desire
   if (h->cfg.schedule == KMP_SCHEDULE_SEQ_STRICT) {
     return strict_cluster(h, max_cluster_weight, desired_num_clusters, communities, clustering_out, stats);
   }
-  if (h->world > 1 && h->comm == nullptr) {
+  if (h->dist.world > 1 && h->dist.comm == nullptr) {
     return fail(KMP_ERR_INVALID, "sharded handle without a communicator: call kmp_lp_dist_init (or drive the "
                                  "stepping API yourself)");
   }
-  const uint32_t n = h->n;
+  const uint32_t n = h->graph.n;
   RunCtx ctx;
   rc = begin_cluster_run(h, max_cluster_weight, communities, &ctx);
   if (rc != KMP_OK) {
@@ -2638,11 +2697,11 @@ int kmp_lp_cluster(kmp_lp_handle *h, int32_t max_cluster_weight, uint32_t desire
       }
     }
   }
-  if (h->world > 1 && n > 0) { // favored[u] is only written by the rank that swept u: MAX over (favored ^ u), 0 elsewhere
-    KMP_CUDA(h->dist_recv.ensure(n));
-    k_xor_iota<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->favored.p, h->dist_recv.p);
-    KMP_NCCL(g_nccl.AllReduce(h->dist_recv.p, h->dist_recv.p, n, ncclUint32, ncclMax, h->comm, h->stream));
-    k_xor_iota<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->dist_recv.p, h->favored.p);
+  if (h->dist.world > 1 && n > 0) { // favored[u] is only written by the rank that swept u: MAX over (favored ^ u), 0 elsewhere
+    KMP_CUDA(h->dist.recv.ensure(n));
+    k_xor_iota<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->lp.favored.p, h->dist.recv.p);
+    KMP_NCCL(g_nccl.AllReduce(h->dist.recv.p, h->dist.recv.p, n, ncclUint32, ncclMax, h->dist.comm, h->stream));
+    k_xor_iota<<<grid_for(n, 256), 256, 0, h->stream>>>(n, h->dist.recv.p, h->lp.favored.p);
   }
   rc = finish_cluster_run(h, max_cluster_weight, stats);
   if (rc == KMP_OK) {
@@ -2655,28 +2714,28 @@ int kmp_lp_cluster(kmp_lp_handle *h, int32_t max_cluster_weight, uint32_t desire
 }
 
 int kmp_lp_upload_partition(kmp_lp_handle *h, const uint32_t *partition) {
-  if (h == nullptr || !h->have_graph || partition == nullptr) {
+  if (h == nullptr || !h->graph.present || partition == nullptr) {
     return fail(KMP_ERR_INVALID, "bad argument");
   }
   KMP_CUDA(cudaSetDevice(h->device));
-  KMP_CUDA(h->label.ensure(h->n));
-  KMP_CUDA(cudaMemcpyAsync(h->label.p, partition, static_cast<size_t>(h->n) * 4, cudaMemcpyHostToDevice, h->stream));
+  KMP_CUDA(h->lp.label.ensure(h->graph.n));
+  KMP_CUDA(cudaMemcpyAsync(h->lp.label.p, partition, static_cast<size_t>(h->graph.n) * 4, cudaMemcpyHostToDevice, h->stream));
   KMP_CUDA(cudaStreamSynchronize(h->stream));
-  h->labels_valid = true;
+  h->lp.labels_valid = true;
   return KMP_OK;
 }
 
 int kmp_lp_download_labels(kmp_lp_handle *h, uint32_t *labels_out) {
-  if (h == nullptr || !h->have_graph || labels_out == nullptr || h->label.p == nullptr) {
+  if (h == nullptr || !h->graph.present || labels_out == nullptr || h->lp.label.p == nullptr) {
     return fail(KMP_ERR_INVALID, "bad argument");
   }
   KMP_CUDA(cudaSetDevice(h->device));
-  KMP_CUDA(cudaMemcpyAsync(labels_out, h->label.p, static_cast<size_t>(h->n) * 4, cudaMemcpyDeviceToHost, h->stream));
+  KMP_CUDA(cudaMemcpyAsync(labels_out, h->lp.label.p, static_cast<size_t>(h->graph.n) * 4, cudaMemcpyDeviceToHost, h->stream));
   KMP_CUDA(cudaStreamSynchronize(h->stream));
   return KMP_OK;
 }
 
-const uint32_t *kmp_lp_labels_device(kmp_lp_handle *h) { return h != nullptr ? h->label.p : nullptr; }
+const uint32_t *kmp_lp_labels_device(kmp_lp_handle *h) { return h != nullptr ? h->lp.label.p : nullptr; }
 
 int kmp_lp_refine(kmp_lp_handle *h, uint32_t k, const int32_t *max_block_weights, const int32_t *min_block_weights,
                   const uint32_t *communities, uint32_t *partition_inout, int32_t *block_weights_out,
@@ -2694,11 +2753,11 @@ int kmp_lp_refine(kmp_lp_handle *h, uint32_t k, const int32_t *max_block_weights
   if (h->cfg.schedule == KMP_SCHEDULE_SEQ_STRICT) {
     return strict_refine(h, k, max_block_weights, min_block_weights, communities, partition_inout, block_weights_out, stats);
   }
-  if (h->world > 1 && h->comm == nullptr) {
+  if (h->dist.world > 1 && h->dist.comm == nullptr) {
     return fail(KMP_ERR_INVALID, "sharded handle without a communicator: call kmp_lp_dist_init (or drive the "
                                  "stepping API yourself)");
   }
-  const uint32_t n = h->n;
+  const uint32_t n = h->graph.n;
   RunCtx ctx;
   rc = begin_refine_run(h, k, max_block_weights, min_block_weights, communities, partition_inout, &ctx);
   if (rc != KMP_OK) {
@@ -2739,13 +2798,13 @@ int kmp_lp_select_all(kmp_lp_handle *h, int mode, const uint32_t *labels, const 
   if (h->cfg.schedule != KMP_SCHEDULE_SYNC) {
     return fail(KMP_ERR_UNSUPPORTED, "kmp_lp_select_all evaluates the sync selection rule");
   }
-  const uint32_t n = h->n;
+  const uint32_t n = h->graph.n;
   rc = ensure_lists(h);
   if (rc != KMP_OK) {
     return rc;
   }
-  KMP_CUDA(h->label.ensure(n));
-  KMP_CUDA(h->weight.ensure(num_labels));
+  KMP_CUDA(h->lp.label.ensure(n));
+  KMP_CUDA(h->lp.weight.ensure(num_labels));
   rc = ensure_scratch(h, mode, num_labels);
   if (rc != KMP_OK) {
     return rc;
@@ -2757,43 +2816,43 @@ int kmp_lp_select_all(kmp_lp_handle *h, int mode, const uint32_t *labels, const 
   DevBuf<uint32_t> d_target, d_fav;
   KMP_CUDA(d_target.ensure(n));
   KMP_CUDA(d_fav.ensure(n));
-  KMP_CUDA(cudaMemcpyAsync(h->label.p, labels, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, h->stream));
+  KMP_CUDA(cudaMemcpyAsync(h->lp.label.p, labels, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, h->stream));
   KMP_CUDA(cudaMemcpyAsync(d_target.p, labels, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, h->stream));
   KMP_CUDA(cudaMemsetAsync(d_fav.p, 0xFF, static_cast<size_t>(n) * 4, h->stream));
-  KMP_CUDA(cudaMemcpyAsync(h->weight.p, weights, static_cast<size_t>(num_labels) * 4, cudaMemcpyHostToDevice, h->stream));
+  KMP_CUDA(cudaMemcpyAsync(h->lp.weight.p, weights, static_cast<size_t>(num_labels) * 4, cudaMemcpyHostToDevice, h->stream));
   if (mode == 1) {
-    KMP_CUDA(h->maxw.ensure(num_labels));
-    KMP_CUDA(cudaMemcpyAsync(h->maxw.p, max_weights, static_cast<size_t>(num_labels) * 4, cudaMemcpyHostToDevice, h->stream));
+    KMP_CUDA(h->lp.maxw.ensure(num_labels));
+    KMP_CUDA(cudaMemcpyAsync(h->lp.maxw.p, max_weights, static_cast<size_t>(num_labels) * 4, cudaMemcpyHostToDevice, h->stream));
     if (min_weights != nullptr) {
-      KMP_CUDA(h->minw.ensure(num_labels));
-      KMP_CUDA(cudaMemcpyAsync(h->minw.p, min_weights, static_cast<size_t>(num_labels) * 4, cudaMemcpyHostToDevice, h->stream));
+      KMP_CUDA(h->lp.minw.ensure(num_labels));
+      KMP_CUDA(cudaMemcpyAsync(h->lp.minw.p, min_weights, static_cast<size_t>(num_labels) * 4, cudaMemcpyHostToDevice, h->stream));
     }
   }
-  KMP_CUDA(cudaMemsetAsync(h->ctr64.p, 0, kCtrSize * sizeof(unsigned long long), h->stream));
+  KMP_CUDA(cudaMemsetAsync(h->commit.ctr64.p, 0, kCtrSize * sizeof(unsigned long long), h->stream));
   if (n > 0) {
     launch_pack_labels(h);
   }
   RunCtx ctx{mode, num_labels, max_cluster_weight, mode == 1 && min_weights != nullptr, false};
   SweepArgs sa = make_sweep_args(h, ctx);
   sa.active = nullptr;
-  KMP_CUDA(cudaMemsetAsync(h->ctr32.p, 0, kCtr32Size * sizeof(uint32_t), h->stream)); // hub work-queue cursors
-  KMP_CUDA(cudaMemsetAsync(h->queue.p, 0, h->queue.cap * sizeof(uint32_t), h->stream));
-  if (h->hub_cursor.p != nullptr) {
-    KMP_CUDA(cudaMemsetAsync(h->hub_cursor.p, 0, h->hub_cursor.cap * sizeof(uint32_t), h->stream));
+  KMP_CUDA(cudaMemsetAsync(h->commit.ctr32.p, 0, kCtr32Size * sizeof(uint32_t), h->stream)); // hub work-queue cursors
+  KMP_CUDA(cudaMemsetAsync(h->lists.queue.p, 0, h->lists.queue.cap * sizeof(uint32_t), h->stream));
+  if (h->hub_tmp.cursor.p != nullptr) {
+    KMP_CUDA(cudaMemsetAsync(h->hub_tmp.cursor.p, 0, h->hub_tmp.cursor.cap * sizeof(uint32_t), h->stream));
   }
   sa.sel_target = d_target.p;
   sa.sel_favored = mode == 0 ? d_fav.p : nullptr;
   sa.base_tie = sync_base(h->cfg.seed, call_index, iteration, SALT_TIE);
   sa.base_fav = sync_base(h->cfg.seed, call_index, iteration, SALT_FAV);
-  const uint32_t S = h->lists_S;
+  const uint32_t S = h->lists.S;
   for (uint32_t ts = 0; ts < kNumTiers * S; ++ts) { // every (tier, class) list once
-    const uint32_t off = h->list_off[ts];
-    const uint32_t size = h->list_off[ts + 1] - off;
+    const uint32_t off = h->lists.off[ts];
+    const uint32_t size = h->lists.off[ts + 1] - off;
     const int tier = static_cast<int>(ts / S);
-    sa.list = h->order.p + off;
+    sa.list = h->lists.order.p + off;
     sa.list_size = size;
-    h->cur_subround = ts % S;
-    h->cur_sg = group_of_tier(tier) * S + ts % S; // one queue cursor per (tier, sub-round)
+    h->round.cur_subround = ts % S;
+    h->round.cur_sg = group_of_tier(tier) * S + ts % S; // one queue cursor per (tier, sub-round)
     KMP_CUDA(launch_sweep(h, mode, tier, sa));
   }
   KMP_CUDA(cudaMemcpyAsync(target_out, d_target.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, h->stream));
@@ -2810,77 +2869,21 @@ int kmp_lp_free_scratch(kmp_lp_handle *h) {
   }
   cudaSetDevice(h->device);
   cudaStreamSynchronize(h->stream);
-  h->label.release();
-  h->labels_valid = false;
-  h->favored.release();
-  h->communities.release();
-  h->weight.release();
-  h->maxw.release();
-  h->minw.release();
-  h->active.release();
-  h->mv_u.release();
-  h->mv_t.release();
-  h->cslot.release();
-  h->slotmap.release();
-  h->acc.release();
-  h->incoming.release();
-  h->chist.release();
-  h->hist.release();
-  h->jmin.release();
-  h->out_cur.release();
-  h->out_delta.release();
-  h->ohist.release();
-  h->ojmin.release();
-  h->ctr32.release();
-  h->ctr64.release();
-  h->hub_tab.release();
-  h->hub_cursor.release();
-  h->hub_ovf.release();
-  h->hub_lab.release();
-  h->hub_cls.release();
-  h->labg.release();
-  h->sort_keys_in.release();
-  h->sort_keys_out.release();
-  h->sort_vals_in.release();
-  h->t4_tmp_deg.release();
-  h->t4_tmp_beg.release();
-  h->t4_tmp_ids.release();
-  h->cub_tmp.release();
-  h->pairs_a.release();
-  h->pairs_b.release();
-  h->ct_vals_a.release();
-  h->ct_vals_b.release();
-  h->ct_flags.release();
-  h->ct_rank.release();
-  h->ct_cl.release();
-  h->ct_counter.release();
-  h->sp_ctl.release();
-  overlay_release(h, true);
-  for (DevBuf<uint32_t> *b : {&h->bal_cand, &h->bal_under, &h->bal_ctr32, &h->bal_target, &h->bal_lists, &h->bal_sv_a,
-                              &h->bal_sv_b, &h->bal_blk}) {
-    b->release();
+  h->lp = {};
+  h->commit = {};
+  h->hub_tmp = {};
+  h->list_tmp = {};
+  h->ops = {};
+  h->bal = {};
+  cudaMemPool_t pool = kmp_private_pool(h->device); // blocks cached for coarse graphs (kmp_contract.cuh)
+  if (pool != nullptr) {
+    cudaMemPoolTrimTo(pool, 0);
   }
-  for (DevBuf<int32_t> *b : {&h->bal_over, &h->bal_pbw, &h->bal_wt, &h->bal_prefix}) {
-    b->release();
-  }
-  h->bal_flag.release();
-  h->ubal_tmask.release();
-  h->bal_key.release();
-  h->bal_ctrl.release();
-  h->bal_sk_a.release();
-  h->bal_sk_b.release();
-  {
-    cudaMemPool_t pool = kmp_private_pool(h->device); // blocks cached for coarse graphs (kmp_contract.cuh)
-    if (pool != nullptr) {
-      cudaMemPoolTrimTo(pool, 0);
-    }
-  }
-  h->slot_state_clean = false;
   return KMP_OK;
 }
 
 int kmp_lp_edge_cut(kmp_lp_handle *h, int64_t *cut_out) {
-  if (h == nullptr || !h->have_graph || cut_out == nullptr || h->label.p == nullptr) {
+  if (h == nullptr || !h->graph.present || cut_out == nullptr || h->lp.label.p == nullptr) {
     return fail(KMP_ERR_INVALID, "bad argument");
   }
   const int rc = refuse_without_labels(h);
@@ -2888,12 +2891,12 @@ int kmp_lp_edge_cut(kmp_lp_handle *h, int64_t *cut_out) {
     return rc;
   }
   KMP_CUDA(cudaSetDevice(h->device));
-  KMP_CUDA(h->ctr64.ensure(kCtrSize));
-  KMP_CUDA(cudaMemsetAsync(h->ctr64.p + kCtrScratch, 0, sizeof(unsigned long long), h->stream));
-  k_edge_cut<<<grid_for(static_cast<uint64_t>(h->n) * 32, 256), 256, 0, h->stream>>>(h->n, h->xadj, h->adjncy, h->adjwgt,
-                                                                                      h->label.p, h->ctr64.p + kCtrScratch);
+  KMP_CUDA(h->commit.ctr64.ensure(kCtrSize));
+  KMP_CUDA(cudaMemsetAsync(h->commit.ctr64.p + kCtrScratch, 0, sizeof(unsigned long long), h->stream));
+  k_edge_cut<<<grid_for(static_cast<uint64_t>(h->graph.n) * 32, 256), 256, 0, h->stream>>>(
+      h->graph.n, h->graph.xadj, h->graph.adjncy, h->graph.adjwgt, h->lp.label.p, h->commit.ctr64.p + kCtrScratch);
   unsigned long long c = 0;
-  KMP_CUDA(cudaMemcpyAsync(&c, h->ctr64.p + kCtrScratch, sizeof(c), cudaMemcpyDeviceToHost, h->stream));
+  KMP_CUDA(cudaMemcpyAsync(&c, h->commit.ctr64.p + kCtrScratch, sizeof(c), cudaMemcpyDeviceToHost, h->stream));
   KMP_CUDA(cudaStreamSynchronize(h->stream));
   *cut_out = static_cast<int64_t>(c / 2); // metrics.cc:51-52
   return KMP_OK;
@@ -2910,8 +2913,8 @@ int kmp_lp_set_shard(kmp_lp_handle *h, uint32_t rank, uint32_t world) {
   if (h == nullptr || world == 0 || rank >= world) {
     return fail(KMP_ERR_INVALID, "bad rank/world");
   }
-  h->rank = rank;
-  h->world = world;
+  h->dist.rank = rank;
+  h->dist.world = world;
   return KMP_OK;
 }
 
@@ -2943,17 +2946,17 @@ int kmp_lp_dist_init(kmp_lp_handle *h, const void *id, uint32_t rank, uint32_t w
     return rc;
   }
   KMP_CUDA(cudaSetDevice(h->device));
-  if (h->comm != nullptr) {
-    g_nccl.CommDestroy(h->comm);
-    h->comm = nullptr;
+  if (h->dist.comm != nullptr) {
+    g_nccl.CommDestroy(h->dist.comm);
+    h->dist.comm = nullptr;
   }
   ncclUniqueId nid;
   std::memcpy(&nid, id, sizeof(nid));
   if (world > 1) {
-    KMP_NCCL(g_nccl.CommInitRank(&h->comm, static_cast<int>(world), nid, static_cast<int>(rank)));
+    KMP_NCCL(g_nccl.CommInitRank(&h->dist.comm, static_cast<int>(world), nid, static_cast<int>(rank)));
   }
-  h->rank = rank;
-  h->world = world;
+  h->dist.rank = rank;
+  h->dist.world = world;
   return KMP_OK;
 }
 
@@ -2961,13 +2964,13 @@ int kmp_lp_dist_shutdown(kmp_lp_handle *h) {
   if (h == nullptr) {
     return KMP_OK;
   }
-  if (h->comm != nullptr) {
+  if (h->dist.comm != nullptr) {
     cudaStreamSynchronize(h->stream);
-    g_nccl.CommDestroy(h->comm);
-    h->comm = nullptr;
+    g_nccl.CommDestroy(h->dist.comm);
+    h->dist.comm = nullptr;
   }
-  h->rank = 0;
-  h->world = 1;
+  h->dist.rank = 0;
+  h->dist.world = 1;
   return KMP_OK;
 }
 
@@ -2978,17 +2981,17 @@ int kmp_lp_set_stream(kmp_lp_handle *h, void *cuda_stream) {
   KMP_CUDA(cudaStreamSynchronize(h->stream));
   // 0 is a valid handle (the legacy default stream, which is what torch uses unless told otherwise);
   // (void*)-1 switches back to the handle's own stream
-  h->stream = cuda_stream == reinterpret_cast<void *>(-1) ? h->owned_stream : static_cast<cudaStream_t>(cuda_stream);
+  h->stream = cuda_stream == reinterpret_cast<void *>(-1) ? h->streams.owned : static_cast<cudaStream_t>(cuda_stream);
   h->sweep_stream = h->stream;
   return KMP_OK;
 }
 
 uint32_t kmp_lp_num_subrounds(kmp_lp_handle *h) {
-  return h != nullptr && h->lists_valid ? kNumGroups * h->lists_S : 0;
+  return h != nullptr && h->lists.valid ? kNumGroups * h->lists.S : 0;
 }
 
 int kmp_lp_subround_cap(kmp_lp_handle *h, uint32_t sg, uint32_t *cap_out, uint32_t *size_out) {
-  if (h == nullptr || !h->lists_valid || sg >= kNumGroups * h->lists_S) {
+  if (h == nullptr || !h->lists.valid || sg >= kNumGroups * h->lists.S) {
     return fail(KMP_ERR_INVALID, "bad sub-round");
   }
   const SubRound q = subround_of_sg(h, sg);
@@ -3009,12 +3012,12 @@ int kmp_lp_step_begin_cluster(kmp_lp_handle *h, int32_t max_cluster_weight, cons
   if (h->cfg.schedule != KMP_SCHEDULE_SYNC) {
     return fail(KMP_ERR_UNSUPPORTED, "the stepping API drives the sync schedule");
   }
-  rc = begin_cluster_run(h, max_cluster_weight, communities, &h->step);
+  rc = begin_cluster_run(h, max_cluster_weight, communities, &h->step.run);
   if (rc != KMP_OK) {
     return rc;
   }
-  h->step_open = true;
-  h->step_iter = 0;
+  h->step.open = true;
+  h->step.iter = 0;
   return KMP_OK;
 }
 
@@ -3030,93 +3033,93 @@ int kmp_lp_step_begin_refine(kmp_lp_handle *h, uint32_t k, const int32_t *max_bl
   if (h->cfg.schedule != KMP_SCHEDULE_SYNC) {
     return fail(KMP_ERR_UNSUPPORTED, "the stepping API drives the sync schedule");
   }
-  rc = begin_refine_run(h, k, max_block_weights, min_block_weights, communities, partition, &h->step);
+  rc = begin_refine_run(h, k, max_block_weights, min_block_weights, communities, partition, &h->step.run);
   if (rc != KMP_OK) {
     return rc;
   }
-  h->step_open = true;
-  h->step_iter = 0;
+  h->step.open = true;
+  h->step.iter = 0;
   return KMP_OK;
 }
 
 int kmp_lp_step_begin_iteration(kmp_lp_handle *h) {
-  if (h == nullptr || !h->step_open) {
+  if (h == nullptr || !h->step.open) {
     return fail(KMP_ERR_INVALID, "step_begin_* not called");
   }
-  return begin_iteration(h, h->step_iter);
+  return begin_iteration(h, h->step.iter);
 }
 
 // Sweep this rank's share of sub-round sg and pack its proposals into d_send (device memory,
 // 4 + 2 * cap words: [count, -, -, -, u[cap], t[cap]]).
 int kmp_lp_step_sweep(kmp_lp_handle *h, uint32_t iter, uint32_t sg, void *d_send) {
-  if (h == nullptr || !h->step_open || d_send == nullptr) {
+  if (h == nullptr || !h->step.open || d_send == nullptr) {
     return fail(KMP_ERR_INVALID, "bad argument");
   }
-  if (sg >= kNumGroups * h->lists_S) { // subround_of_sg indexes list_off by sg
+  if (sg >= kNumGroups * h->lists.S) { // subround_of_sg indexes lists.off by sg
     return fail(KMP_ERR_INVALID, "bad sub-round");
   }
-  return dist_sweep_pack(h, h->step, iter, sg, subround_of_sg(h, sg), static_cast<uint32_t *>(d_send));
+  return dist_sweep_pack(h, h->step.run, iter, sg, subround_of_sg(h, sg), static_cast<uint32_t *>(d_send));
 }
 
 // Commit sub-round sg from the all-gathered proposal buffers (world * (4 + 2 * cap) words).
 int kmp_lp_step_commit(kmp_lp_handle *h, uint32_t iter, uint32_t sg, const void *d_gathered) {
-  if (h == nullptr || !h->step_open || d_gathered == nullptr) {
+  if (h == nullptr || !h->step.open || d_gathered == nullptr) {
     return fail(KMP_ERR_INVALID, "bad argument");
   }
-  if (sg >= kNumGroups * h->lists_S) {
+  if (sg >= kNumGroups * h->lists.S) {
     return fail(KMP_ERR_INVALID, "bad sub-round");
   }
-  return commit_subround(h, h->step, iter, sg, subround_of_sg(h, sg), static_cast<const uint32_t *>(d_gathered));
+  return commit_subround(h, h->step.run, iter, sg, subround_of_sg(h, sg), static_cast<const uint32_t *>(d_gathered));
 }
 
 int kmp_lp_step_end_iteration(kmp_lp_handle *h, uint32_t *moved) {
-  if (h == nullptr || !h->step_open || moved == nullptr) {
+  if (h == nullptr || !h->step.open || moved == nullptr) {
     return fail(KMP_ERR_INVALID, "bad argument");
   }
   const int rc = end_iteration(h, moved);
   if (rc != KMP_OK) {
     return rc;
   }
-  ++h->step_iter;
+  ++h->step.iter;
   return KMP_OK;
 }
 
 // favored[u] ^ u into / out of a caller-provided device buffer of n words (for a MAX all-reduce:
 // only the rank that owns u ever writes favored[u]; everybody else still holds u, i.e. 0 here).
 int kmp_lp_step_favored_export(kmp_lp_handle *h, void *d_buf) {
-  if (h == nullptr || d_buf == nullptr || !h->step_open || h->step.mode != 0) {
+  if (h == nullptr || d_buf == nullptr || !h->step.open || h->step.run.mode != 0) {
     return fail(KMP_ERR_INVALID, "bad argument");
   }
-  k_xor_iota<<<grid_for(h->n, 256), 256, 0, h->stream>>>(h->n, h->favored.p, static_cast<uint32_t *>(d_buf));
+  k_xor_iota<<<grid_for(h->graph.n, 256), 256, 0, h->stream>>>(h->graph.n, h->lp.favored.p, static_cast<uint32_t *>(d_buf));
   KMP_CUDA(cudaGetLastError());
   return KMP_OK;
 }
 int kmp_lp_step_favored_import(kmp_lp_handle *h, const void *d_buf) {
-  if (h == nullptr || d_buf == nullptr || !h->step_open || h->step.mode != 0) {
+  if (h == nullptr || d_buf == nullptr || !h->step.open || h->step.run.mode != 0) {
     return fail(KMP_ERR_INVALID, "bad argument");
   }
-  k_xor_iota<<<grid_for(h->n, 256), 256, 0, h->stream>>>(h->n, static_cast<const uint32_t *>(d_buf), h->favored.p);
+  k_xor_iota<<<grid_for(h->graph.n, 256), 256, 0, h->stream>>>(h->graph.n, static_cast<const uint32_t *>(d_buf), h->lp.favored.p);
   KMP_CUDA(cudaGetLastError());
   return KMP_OK;
 }
 
 // Post passes (clusterer) and result download; stats hold THIS rank's share of the scan counters.
 int kmp_lp_step_finish(kmp_lp_handle *h, uint32_t *labels_out, int32_t *block_weights_out, kmp_lp_stats *stats) {
-  if (h == nullptr || !h->step_open) {
+  if (h == nullptr || !h->step.open) {
     return fail(KMP_ERR_INVALID, "step_begin_* not called");
   }
   if (stats != nullptr) {
     std::memset(stats, 0, sizeof(*stats));
   }
-  const bool cluster = h->step.mode == 0;
-  int rc = cluster ? finish_cluster_run(h, h->step.max_cluster_weight, stats) : KMP_OK;
+  const bool cluster = h->step.run.mode == 0;
+  int rc = cluster ? finish_cluster_run(h, h->step.run.max_cluster_weight, stats) : KMP_OK;
   if (rc == KMP_OK) {
-    rc = download_results(h, labels_out, cluster ? nullptr : block_weights_out, h->step.num_labels);
+    rc = download_results(h, labels_out, cluster ? nullptr : block_weights_out, h->step.run.num_labels);
   }
   if (rc != KMP_OK) {
     return rc;
   }
-  h->step_open = false;
+  h->step.open = false;
   return end_call(h, stats);
 }
 

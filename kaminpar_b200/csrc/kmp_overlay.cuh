@@ -22,23 +22,6 @@
 
 namespace {
 
-// handle-owned overlay state: the stashed clusterings (pool blocks, kept between calls) and the sort's values
-struct OverlayState {
-  std::vector<PoolBuf<uint32_t>> stash;
-  DevBuf<uint32_t> vals_a, vals_b;
-};
-
-void overlay_release(kmp_lp_handle *h, bool scratch) {
-  if (h->ov == nullptr) {
-    return;
-  }
-  h->ov->stash.clear(); // stream-ordered: later than any work of the handle that still reads it
-  if (scratch) {
-    delete h->ov;
-    h->ov = nullptr;
-  }
-}
-
 // key[u] = (ra(a[u]) << nb) | b[u], value u (step 2); a label >= n of either input sets *bad
 __global__ void k_overlay_keys(uint32_t n, const uint32_t *__restrict__ a, const uint32_t *__restrict__ b,
                                const uint32_t *__restrict__ rank, uint32_t nb, unsigned long long *__restrict__ keys,
@@ -84,12 +67,12 @@ struct OverlayCounts {
   uint32_t launches = 0, sort_bits = 0, num_clusters = 0;
 };
 
-// leader flags + inclusive scan of labels (n >= 1) into h->ct_flags / h->ct_rank; then one wait for the number of
+// leader flags + inclusive scan of labels (n >= 1) into h->ops.ct_flags / h->ops.ct_rank; then one wait for the number of
 // distinct labels and the out-of-range flag. `then` may enqueue more work before the wait (it sees the ranks).
 template <typename Then> int overlay_ranks(kmp_lp_handle *h, const uint32_t *labels, uint32_t *distinct, Then then) {
-  const uint32_t n = h->n;
+  const uint32_t n = h->graph.n;
   cudaStream_t st = h->stream;
-  DevBuf<uint32_t> &flags = h->ct_flags, &rank = h->ct_rank;
+  DevBuf<uint32_t> &flags = h->ops.ct_flags, &rank = h->ops.ct_rank;
   KMP_CUDA(flags.ensure(static_cast<size_t>(n) + 1)); // flags[n]: out-of-range marker
   KMP_CUDA(rank.ensure(n));
   KMP_CUDA(cudaMemsetAsync(flags.p, 0, (static_cast<size_t>(n) + 1) * 4, st));
@@ -112,12 +95,12 @@ template <typename Then> int overlay_ranks(kmp_lp_handle *h, const uint32_t *lab
   return KMP_OK;
 }
 
-// out = overlay(a, b) on the handle's graph (n >= 1); out may alias a or b. Leaves P in h->ct_flags.
+// out = overlay(a, b) on the handle's graph (n >= 1); out may alias a or b. Leaves P in h->ops.ct_flags.
 int overlay_pair(kmp_lp_handle *h, const uint32_t *a, const uint32_t *b, uint32_t *out, OverlayCounts *cnt) {
-  const uint32_t n = h->n;
+  const uint32_t n = h->graph.n;
   cudaStream_t st = h->stream;
-  OverlayState &ov = *h->ov;
-  DevBuf<unsigned long long> &keys_a = h->pairs_a, &keys_b = h->pairs_b;
+  OverlayState &ov = h->ops.ov;
+  DevBuf<unsigned long long> &keys_a = h->ops.pairs_a, &keys_b = h->ops.pairs_b;
   KMP_CUDA(keys_a.ensure(n));
   KMP_CUDA(keys_b.ensure(n));
   KMP_CUDA(ov.vals_a.ensure(n));
@@ -144,7 +127,7 @@ int overlay_pair(kmp_lp_handle *h, const uint32_t *a, const uint32_t *b, uint32_
     }));
   }
   // ---- 4. heads + scan; 5. scatter. The leader flags and ranks are dead: P reuses the flags, seg the ranks ------------
-  uint32_t *P = h->ct_flags.p, *seg = h->ct_rank.p;
+  uint32_t *P = h->ops.ct_flags.p, *seg = h->ops.ct_rank.p;
   k_overlay_heads<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, dk.Current(), nb, P, seg);
   KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
     return cub::DeviceScan::InclusiveSum(tmp, bytes, P, P, static_cast<int>(n), st);
@@ -158,9 +141,9 @@ int overlay_pair(kmp_lp_handle *h, const uint32_t *a, const uint32_t *b, uint32_
 // Reduces the first `count` (a power of two) stashed clusterings in the reference's tree order into dst (n >= 1).
 // count == 1 checks and copies C[0].
 int overlay_tree(kmp_lp_handle *h, uint32_t count, uint32_t *dst, OverlayCounts *cnt) {
-  const uint32_t n = h->n;
+  const uint32_t n = h->graph.n;
   cudaStream_t st = h->stream;
-  std::vector<PoolBuf<uint32_t>> &c = h->ov->stash;
+  std::vector<PoolBuf<uint32_t>> &c = h->ops.ov.stash;
   if (count == 1) {
     int rc = overlay_ranks(h, c[0].p, &cnt->num_clusters, [](const uint32_t *, uint32_t *) { return KMP_OK; });
     cnt->launches += 1;
@@ -179,26 +162,20 @@ int overlay_tree(kmp_lp_handle *h, uint32_t count, uint32_t *dst, OverlayCounts 
       }
     }
   }
-  KMP_CUDA(cudaMemcpyAsync(&cnt->num_clusters, h->ct_flags.p + (n - 1), 4, cudaMemcpyDeviceToHost, st));
+  KMP_CUDA(cudaMemcpyAsync(&cnt->num_clusters, h->ops.ct_flags.p + (n - 1), 4, cudaMemcpyDeviceToHost, st));
   KMP_CUDA(cudaStreamSynchronize(st));
   return KMP_OK;
 }
 
 // the stash holds at least `count` blocks of n labels
 int overlay_stash(kmp_lp_handle *h, uint32_t count) {
-  if (h->ov == nullptr) {
-    h->ov = new (std::nothrow) OverlayState();
-    if (h->ov == nullptr) {
-      return fail(KMP_ERR_ALLOC, "out of host memory");
-    }
-  }
-  std::vector<PoolBuf<uint32_t>> &c = h->ov->stash;
+  std::vector<PoolBuf<uint32_t>> &c = h->ops.ov.stash;
   if (c.size() < count) {
     c.resize(count);
   }
   for (uint32_t i = 0; i < count; ++i) {
-    if (c[i].p == nullptr || c[i].cap < h->n) {
-      KMP_CUDA(c[i].alloc(h->n, h->stream, h->device));
+    if (c[i].p == nullptr || c[i].cap < h->graph.n) {
+      KMP_CUDA(c[i].alloc(h->graph.n, h->stream, h->device));
     }
   }
   return KMP_OK;
@@ -208,7 +185,7 @@ int overlay_checks(kmp_lp_handle *h) {
   if (h == nullptr) {
     return fail(KMP_ERR_INVALID, "null handle");
   }
-  if (!h->have_graph) {
+  if (!h->graph.present) {
     return fail(KMP_ERR_INVALID, "no graph set");
   }
   return refuse_multi_gpu(h, "the overlay");
@@ -216,26 +193,26 @@ int overlay_checks(kmp_lp_handle *h) {
 
 // reduce the stash's first `count` clusterings into the handle's labels; timing and stats
 int overlay_finish(kmp_lp_handle *h, uint32_t count, uint32_t *clustering_out, kmp_overlay_stats *stats) {
-  const uint32_t n = h->n;
+  const uint32_t n = h->graph.n;
   cudaStream_t st = h->stream;
   OverlayCounts cnt;
   float ms = 0.f;
   if (n > 0) {
-    KMP_CUDA(h->label.ensure(n));
+    KMP_CUDA(h->lp.label.ensure(n));
     KMP_CUDA(call_clock_start(h, st));
-    const int rc = overlay_tree(h, count, h->label.p, &cnt);
+    const int rc = overlay_tree(h, count, h->lp.label.p, &cnt);
     if (rc != KMP_OK) {
       return rc;
     }
     KMP_CUDA(call_clock_stop(h, st));
-    KMP_CUDA(cudaEventSynchronize(h->ev_ct1));
+    KMP_CUDA(cudaEventSynchronize(h->streams.ev_ct1));
     ms = call_clock_ms(h);
     if (clustering_out != nullptr) {
-      KMP_CUDA(cudaMemcpyAsync(clustering_out, h->label.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, st));
+      KMP_CUDA(cudaMemcpyAsync(clustering_out, h->lp.label.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, st));
       KMP_CUDA(cudaStreamSynchronize(st));
     }
   }
-  h->labels_valid = true;
+  h->lp.labels_valid = true;
   if (stats != nullptr) {
     stats->num_clusterings = count;
     stats->num_clusters = cnt.num_clusters;
@@ -272,8 +249,8 @@ int kmp_lp_cluster_overlay(kmp_lp_handle *h, int num_levels, int32_t max_cluster
       return rc;
     }
     OverlayCounts cnt;
-    if (h->n > 0) {
-      rc = overlay_ranks(h, h->label.p, &cnt.num_clusters, [](const uint32_t *, uint32_t *) { return KMP_OK; });
+    if (h->graph.n > 0) {
+      rc = overlay_ranks(h, h->lp.label.p, &cnt.num_clusters, [](const uint32_t *, uint32_t *) { return KMP_OK; });
       if (rc != KMP_OK) {
         return rc;
       }
@@ -300,12 +277,12 @@ int kmp_lp_cluster_overlay(kmp_lp_handle *h, int num_levels, int32_t max_cluster
       return rc;
     }
     lp_ms += ls.device_ms;
-    if (h->n > 0) {
-      KMP_CUDA(cudaMemcpyAsync(h->ov->stash[i].p, h->label.p, static_cast<size_t>(h->n) * 4,
+    if (h->graph.n > 0) {
+      KMP_CUDA(cudaMemcpyAsync(h->ops.ov.stash[i].p, h->lp.label.p, static_cast<size_t>(h->graph.n) * 4,
                                cudaMemcpyDeviceToDevice, h->stream));
     }
   }
-  h->labels_valid = false; // until the overlay below replaces the last call's labels
+  h->lp.labels_valid = false; // until the overlay below replaces the last call's labels
   rc = overlay_finish(h, count, clustering_out, stats);
   if (stats != nullptr) {
     stats->lp_device_ms = lp_ms;
@@ -322,21 +299,21 @@ int kmp_overlay_clusterings(kmp_lp_handle *h, uint32_t count, const uint32_t *cl
   if (count == 0 || (count & (count - 1)) != 0 || count > (1u << KMP_OVERLAY_MAX_LEVELS)) {
     return fail(KMP_ERR_INVALID, "count must be a power of two in [1, 2^KMP_OVERLAY_MAX_LEVELS]");
   }
-  if (clusterings == nullptr && h->n > 0) {
+  if (clusterings == nullptr && h->graph.n > 0) {
     return fail(KMP_ERR_INVALID, "null clusterings");
   }
   KMP_CUDA(cudaSetDevice(h->device));
   if (stats != nullptr) {
     std::memset(stats, 0, sizeof(*stats));
   }
-  const uint32_t n = h->n;
+  const uint32_t n = h->graph.n;
   if (n > 0) {
     rc = overlay_stash(h, count);
     if (rc != KMP_OK) {
       return rc;
     }
     for (uint32_t i = 0; i < count; ++i) {
-      KMP_CUDA(cudaMemcpyAsync(h->ov->stash[i].p, clusterings + static_cast<size_t>(i) * n, static_cast<size_t>(n) * 4,
+      KMP_CUDA(cudaMemcpyAsync(h->ops.ov.stash[i].p, clusterings + static_cast<size_t>(i) * n, static_cast<size_t>(n) * 4,
                                cudaMemcpyHostToDevice, h->stream));
     }
   }

@@ -411,7 +411,7 @@ int finish_impl(kmp_lp_handle *h, const kmp_prepared_graph *g, uint32_t k, const
   PoolBuf<int32_t> bw, maxw, bw_out;
   PoolBuf<unsigned long long> bad;
   PoolBuf<long long> w, S;
-  const uint32_t *part = h->label.p;
+  const uint32_t *part = h->lp.label.p;
   if (partition != nullptr) {
     KMP_CUDA(d_part.alloc(np, st, dev));
     if (np > 0) {
@@ -536,8 +536,8 @@ int kmp_prepared_finish(kmp_lp_handle *h, const kmp_prepared_graph *g, uint32_t 
   }
   if (partition == nullptr) {
     // the device labels must be the handle's labels of exactly this prepared graph
-    const bool holds_g = h->have_graph && h->xadj == g->xadj.p && h->adjncy == g->adjncy.p && h->n == g->np &&
-                         h->m == g->m;
+    const bool holds_g = h->graph.present && h->graph.xadj == g->xadj.p && h->graph.adjncy == g->adjncy.p && h->graph.n == g->np &&
+                         h->graph.m == g->m;
     if (!holds_g) {
       return fail(KMP_ERR_INVALID, "the handle holds another graph than this prepared graph: pass the partition");
     }

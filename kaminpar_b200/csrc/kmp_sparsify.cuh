@@ -212,7 +212,7 @@ int sparsify_impl(kmp_lp_handle *h, const kmp_coarse_graph *g, uint32_t target_m
   } else {
     // ---- 1. radix select of the k-th smallest weight (quickselect_k_smallest(c_m - target_m + 1, ...)) ----------
     const uint32_t k = m - target_m + 1;
-    DevBuf<uint32_t> &ctl = h->sp_ctl;
+    DevBuf<uint32_t> &ctl = h->ops.sp_ctl;
     KMP_CUDA(ctl.ensure(kSpCtlWords));
     KMP_CUDA(cudaMemsetAsync(ctl.p, 0, kSpCtlWords * 4, st));
     const int32_t *w = g->adjwgt.p;
@@ -239,7 +239,7 @@ int sparsify_impl(kmp_lp_handle *h, const kmp_coarse_graph *g, uint32_t target_m
     const double p = 1.0 * static_cast<double>(target_m - larger) / static_cast<double>(equal);
     // ---- 2. keep flags -----------------------------------------------------------------------------------------
     const uint32_t tiles = (m + kTileEdges - 1) / kTileEdges;
-    DevBuf<uint32_t> &tile_lo = h->ct_flags, &pos = h->ct_rank;
+    DevBuf<uint32_t> &tile_lo = h->ops.ct_flags, &pos = h->ops.ct_rank;
     KMP_CUDA(tile_lo.ensure(static_cast<size_t>(tiles) + 1));
     KMP_CUDA(pos.ensure(static_cast<size_t>(m) + 1));
     KMP_CUDA(cudaMemsetAsync(pos.p + m, 0, 4, st));
@@ -266,8 +266,8 @@ int sparsify_impl(kmp_lp_handle *h, const kmp_coarse_graph *g, uint32_t target_m
   }
   KMP_CUDA(call_clock_stop(h, st));
   if (target_m >= 2) {
-    KMP_CUDA(cudaMemcpyAsync(&counts[0], h->ct_rank.p + m, 4, cudaMemcpyDeviceToHost, st));
-    KMP_CUDA(cudaMemcpyAsync(&counts[1], h->sp_ctl.p + kSpEqualKept, 4, cudaMemcpyDeviceToHost, st));
+    KMP_CUDA(cudaMemcpyAsync(&counts[0], h->ops.ct_rank.p + m, 4, cudaMemcpyDeviceToHost, st));
+    KMP_CUDA(cudaMemcpyAsync(&counts[1], h->ops.sp_ctl.p + kSpEqualKept, 4, cudaMemcpyDeviceToHost, st));
   }
   KMP_CUDA(cudaStreamSynchronize(st));
   kept = counts[0];

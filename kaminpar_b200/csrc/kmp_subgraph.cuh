@@ -297,8 +297,8 @@ uint32_t sub_final_k(uint32_t block, uint32_t current_k, uint32_t input_k) {
 int extract_impl(kmp_lp_handle *h, uint32_t k, kmp_subgraphs *g, kmp_subgraph_stats *stats) {
   const cudaStream_t st = h->stream;
   const int dev = h->device;
-  const uint32_t n = h->n, m = h->m;
-  const uint32_t *part = h->label.p;
+  const uint32_t n = h->graph.n, m = h->graph.m;
+  const uint32_t *part = h->lp.label.p;
   uint32_t launches = 0;
   // ---- labels >= k are refused before any [k] array is indexed by one ---------------------------------------
   {
@@ -316,13 +316,13 @@ int extract_impl(kmp_lp_handle *h, uint32_t k, kmp_subgraphs *g, kmp_subgraph_st
     KMP_CUDA(cudaMemcpyAsync(&nbad, bad.p, sizeof(nbad), cudaMemcpyDeviceToHost, st));
     KMP_CUDA(cudaStreamSynchronize(st));
     if (nbad != 0) {
-      h->labels_valid = false; // a host partition was loaded as the labels: they are not a k-way partition
+      h->lp.labels_valid = false; // a host partition was loaded as the labels: they are not a k-way partition
       return fail(KMP_ERR_INVALID, "partition holds a block id >= k");
     }
   }
   g->n = n;
   g->k = k;
-  g->graph_epoch = h->graph_epoch;
+  g->graph_epoch = h->graph.epoch;
   g->source = h;
   KMP_CUDA(g->xadj.alloc(static_cast<size_t>(n) + k, st, dev));
   KMP_CUDA(g->mapping.alloc(n, st, dev));
@@ -330,7 +330,7 @@ int extract_impl(kmp_lp_handle *h, uint32_t k, kmp_subgraphs *g, kmp_subgraph_st
   KMP_CUDA(g->blk.alloc(n, st, dev));
   KMP_CUDA(g->node_off.alloc(static_cast<size_t>(k) + 1, st, dev));
   KMP_CUDA(g->edge_off.alloc(static_cast<size_t>(k) + 1, st, dev));
-  if (h->vwgt != nullptr) {
+  if (h->graph.vwgt != nullptr) {
     KMP_CUDA(g->vwgt.alloc(n, st, dev));
   }
   const uint32_t tiles = (m + kTileEdges - 1) / kTileEdges;
@@ -342,9 +342,9 @@ int extract_impl(kmp_lp_handle *h, uint32_t k, kmp_subgraphs *g, kmp_subgraph_st
   KMP_CUDA(tile_cnt.alloc(static_cast<size_t>(tiles) + 1, st, dev));
   KMP_CUDA(tile_base.alloc(static_cast<size_t>(tiles) + 1, st, dev));
   if (m > 0) {
-    k_tile_owners<<<capped(h, grid_for(static_cast<uint64_t>(tiles) + 1, 256)), 256, 0, st>>>(n, m, h->xadj, tiles,
+    k_tile_owners<<<capped(h, grid_for(static_cast<uint64_t>(tiles) + 1, 256)), 256, 0, st>>>(n, m, h->graph.xadj, tiles,
                                                                                               tile_lo.p);
-    k_sub_count<<<capped(h, std::min<uint32_t>(tiles, kSMs * 8)), 256, 0, st>>>(m, h->xadj, h->adjncy, tile_lo.p, tiles,
+    k_sub_count<<<capped(h, std::min<uint32_t>(tiles, kSMs * 8)), 256, 0, st>>>(m, h->graph.xadj, h->graph.adjncy, tile_lo.p, tiles,
                                                                                 part, tile_cnt.p, deg.p);
     launches += 2;
     KMP_CUDA(cudaMemsetAsync(tile_cnt.p + tiles, 0, 4, st));
@@ -366,7 +366,7 @@ int extract_impl(kmp_lp_handle *h, uint32_t k, kmp_subgraphs *g, kmp_subgraph_st
     }));
     k_sub_node_off<<<capped(h, grid_for(static_cast<uint64_t>(k) + 1, 256)), 256, 0, st>>>(n, k, g->blk.p,
                                                                                             g->node_off.p);
-    k_sub_map<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, g->blk.p, g->block_nodes.p, g->node_off.p, h->vwgt, deg.p,
+    k_sub_map<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, g->blk.p, g->block_nodes.p, g->node_off.p, h->graph.vwgt, deg.p,
                                                            g->mapping.p, g->vwgt.p, deg_new.p);
     launches += 3;
     KMP_CUDA(cudaMemsetAsync(deg_new.p + n, 0, 4, st));
@@ -390,16 +390,16 @@ int extract_impl(kmp_lp_handle *h, uint32_t k, kmp_subgraphs *g, kmp_subgraph_st
   g->m = m_int;
   // ---- 3. edges ---------------------------------------------------------------------------------------------
   KMP_CUDA(g->adjncy.alloc(m_int, st, dev));
-  if (h->adjwgt != nullptr) {
+  if (h->graph.adjwgt != nullptr) {
     KMP_CUDA(g->adjwgt.alloc(m_int, st, dev));
   }
   if (m_int > 0) {
     const uint32_t grid = capped(h, std::min<uint32_t>(tiles, kSMs * 8));
-    if (h->adjwgt != nullptr) {
-      k_sub_edges<true><<<grid, 256, 0, st>>>(m, h->xadj, h->adjncy, h->adjwgt, tile_lo.p, tiles, tile_base.p, part,
+    if (h->graph.adjwgt != nullptr) {
+      k_sub_edges<true><<<grid, 256, 0, st>>>(m, h->graph.xadj, h->graph.adjncy, h->graph.adjwgt, tile_lo.p, tiles, tile_base.p, part,
                                               g->mapping.p, delta.p, g->adjncy.p, g->adjwgt.p);
     } else {
-      k_sub_edges<false><<<grid, 256, 0, st>>>(m, h->xadj, h->adjncy, nullptr, tile_lo.p, tiles, tile_base.p, part,
+      k_sub_edges<false><<<grid, 256, 0, st>>>(m, h->graph.xadj, h->graph.adjncy, nullptr, tile_lo.p, tiles, tile_base.p, part,
                                                g->mapping.p, delta.p, g->adjncy.p, nullptr);
     }
     ++launches;
@@ -464,22 +464,22 @@ int copy_back_impl(kmp_lp_handle *h, const kmp_subgraphs *g, uint32_t k_prime, u
     return fail(KMP_ERR_INVALID, "a sub-partition label is >= its block's sub-block count");
   }
   // ---- the k'-way partition becomes h's labels and block weights ---------------------------------------------
-  KMP_CUDA(h->label.ensure(n));
-  KMP_CUDA(h->weight.ensure(k_prime));
-  KMP_CUDA(cudaMemcpyAsync(h->label.p, out.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToDevice, st));
-  h->labels_valid = true;
-  KMP_CUDA(cudaMemsetAsync(h->weight.p, 0, static_cast<size_t>(k_prime) * 4, st));
+  KMP_CUDA(h->lp.label.ensure(n));
+  KMP_CUDA(h->lp.weight.ensure(k_prime));
+  KMP_CUDA(cudaMemcpyAsync(h->lp.label.p, out.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToDevice, st));
+  h->lp.labels_valid = true;
+  KMP_CUDA(cudaMemsetAsync(h->lp.weight.p, 0, static_cast<size_t>(k_prime) * 4, st));
   KMP_CUDA(cudaMemsetAsync(bad.p, 0, 8, st));
   if (n > 0) {
-    bal_block_weights<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, k_prime, h->vwgt, h->label.p, h->weight.p,
+    bal_block_weights<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, k_prime, h->graph.vwgt, h->lp.label.p, h->lp.weight.p,
                                                                    bad.p);
   }
   KMP_CUDA(cudaGetLastError());
   if (partition_out != nullptr && n > 0) {
-    KMP_CUDA(cudaMemcpyAsync(partition_out, h->label.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, st));
+    KMP_CUDA(cudaMemcpyAsync(partition_out, h->lp.label.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, st));
   }
   if (block_weights_out != nullptr) {
-    KMP_CUDA(cudaMemcpyAsync(block_weights_out, h->weight.p, static_cast<size_t>(k_prime) * 4, cudaMemcpyDeviceToHost,
+    KMP_CUDA(cudaMemcpyAsync(block_weights_out, h->lp.weight.p, static_cast<size_t>(k_prime) * 4, cudaMemcpyDeviceToHost,
                              st));
   }
   KMP_CUDA(cudaStreamSynchronize(st));
@@ -494,10 +494,10 @@ int copy_back_checked(kmp_lp_handle *h, const kmp_subgraphs *g, uint32_t k_prime
   if (!host_sub && (reinterpret_cast<uintptr_t>(sub) & 3u) != 0) {
     return fail(KMP_ERR_INVALID, "device sub-partitions must be 4-byte aligned");
   }
-  if (h->step_open) {
+  if (h->step.open) {
     return fail(KMP_ERR_INVALID, "the handle is inside a stepping call");
   }
-  if (g->source != h || !h->have_graph || h->graph_epoch != g->graph_epoch) {
+  if (g->source != h || !h->graph.present || h->graph.epoch != g->graph_epoch) {
     return fail(KMP_ERR_INVALID, "the handle holds another graph than the one the subgraphs were extracted from");
   }
   if (k_prime < g->k) {
@@ -519,16 +519,16 @@ int kmp_extract_subgraphs(kmp_lp_handle *h, uint32_t k, const uint32_t *partitio
   if (h == nullptr || out == nullptr) {
     return fail(KMP_ERR_INVALID, "null argument");
   }
-  if (!h->have_graph) {
+  if (!h->graph.present) {
     return fail(KMP_ERR_INVALID, "no graph set");
   }
-  if (h->step_open) {
+  if (h->step.open) {
     return fail(KMP_ERR_INVALID, "the handle is inside a stepping call");
   }
   if (k == 0) {
     return fail(KMP_ERR_INVALID, "k must be at least 1");
   }
-  if (static_cast<uint64_t>(h->n) + k >= (1ull << 32)) {
+  if (static_cast<uint64_t>(h->graph.n) + k >= (1ull << 32)) {
     return fail(KMP_ERR_UNSUPPORTED, "n + k must be below 2^32");
   }
   if (partition == nullptr) {
@@ -543,9 +543,9 @@ int kmp_extract_subgraphs(kmp_lp_handle *h, uint32_t k, const uint32_t *partitio
   }
   KMP_CUDA(call_clock_start(h, h->stream));
   if (partition != nullptr) { // loaded as the handle's labels, as load_partition does
-    KMP_CUDA(h->label.ensure(h->n));
-    KMP_CUDA(cudaMemcpyAsync(h->label.p, partition, static_cast<size_t>(h->n) * 4, cudaMemcpyHostToDevice, h->stream));
-    h->labels_valid = true;
+    KMP_CUDA(h->lp.label.ensure(h->graph.n));
+    KMP_CUDA(cudaMemcpyAsync(h->lp.label.p, partition, static_cast<size_t>(h->graph.n) * 4, cudaMemcpyHostToDevice, h->stream));
+    h->lp.labels_valid = true;
   }
   return make_result(h, out, [&](kmp_subgraphs *g) { return extract_impl(h, k, g, stats); });
 }

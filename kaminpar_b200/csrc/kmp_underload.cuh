@@ -7,7 +7,7 @@
 //
 // What it restates: UnderloadBalancer::refine (refinement/balancer/underload_balancer.cc:39-244) as synchronous
 // rounds (DESIGN.md §12). One round:
-//   1. block stats against the frozen weights: deficit[b] = max(0, min[b] - W[b]) (kept in bal_over), the total
+//   1. block stats against the frozen weights: deficit[b] = max(0, min[b] - W[b]) (kept in bal.over), the total
 //      underload, the underloaded flags (the target mask); the vertices that may leave their block (block not
 //      underloaded, W[b] - w(u) >= min[b]) are compacted in id order (one small read-back per round: total, count)
 //   2. candidate evaluation by the overload balancer's tiers, targets restricted to underloaded blocks
@@ -75,57 +75,57 @@ namespace {
 
 using namespace kmp;
 
-// Round start: deficit[] (in bal_over), target mask, candidates; read back {total underload, #candidates} and the
+// Round start: deficit[] (in bal.over), target mask, candidates; read back {total underload, #candidates} and the
 // number of proposals of the previous round.
 int ubal_round_begin(kmp_lp_handle *h, uint32_t k, unsigned long long *host_ctrl, uint32_t *host_proposals) {
   cudaStream_t st = h->stream;
-  const uint32_t n = h->n;
-  KMP_CUDA(cudaMemsetAsync(h->bal_ctrl.p, 0, 2 * sizeof(unsigned long long), st));
-  ubal_block_stats<<<capped(h, grid_for(k, 256)), 256, 0, st>>>(k, h->weight.p, h->minw.p, h->bal_over.p,
-                                                                h->ubal_tmask.p, h->bal_ctrl.p);
-  ubal_vertex_flags<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, h->label.p, h->vwgt, h->weight.p, h->minw.p,
-                                                                 h->ubal_tmask.p, h->bal_flag.p);
+  const uint32_t n = h->graph.n;
+  KMP_CUDA(cudaMemsetAsync(h->bal.ctrl.p, 0, 2 * sizeof(unsigned long long), st));
+  ubal_block_stats<<<capped(h, grid_for(k, 256)), 256, 0, st>>>(k, h->lp.weight.p, h->lp.minw.p, h->bal.over.p,
+                                                                h->bal.tmask.p, h->bal.ctrl.p);
+  ubal_vertex_flags<<<capped(h, grid_for(n, 256)), 256, 0, st>>>(n, h->lp.label.p, h->graph.vwgt, h->lp.weight.p, h->lp.minw.p,
+                                                                 h->bal.tmask.p, h->bal.flag.p);
   KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
-    return cub::DeviceSelect::Flagged(tmp, bytes, thrust::counting_iterator<uint32_t>(0), h->bal_flag.p, h->bal_cand.p,
-                                      h->bal_ctrl.p + 1, static_cast<int>(n), st);
+    return cub::DeviceSelect::Flagged(tmp, bytes, thrust::counting_iterator<uint32_t>(0), h->bal.flag.p, h->bal.cand.p,
+                                      h->bal.ctrl.p + 1, static_cast<int>(n), st);
   }));
-  h->kernel_launches += 3;
-  KMP_CUDA(cudaMemcpyAsync(host_ctrl, h->bal_ctrl.p, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-  KMP_CUDA(cudaMemcpyAsync(host_proposals, h->bal_ctr32.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  h->counts.kernel_launches += 3;
+  KMP_CUDA(cudaMemcpyAsync(host_ctrl, h->bal.ctrl.p, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  KMP_CUDA(cudaMemcpyAsync(host_proposals, h->bal.ctr32.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
   KMP_CUDA(cudaStreamSynchronize(st));
   return KMP_OK;
 }
 
 // Selection of a round after its read-back: evaluate the nc candidates, compact those with a target and write their
-// sort words (target << 32 | desc key bits) into bal_sk_a / bal_sv_a; *nt: their count (0: the round proposes nothing).
+// sort words (target << 32 | desc key bits) into bal.sk_a / bal.sv_a; *nt: their count (0: the round proposes nothing).
 int ubal_select(kmp_lp_handle *h, uint32_t k, uint32_t nc, uint32_t call, uint32_t r, uint32_t *nt) {
   *nt = 0;
   if (nc == 0) {
     return KMP_OK;
   }
   cudaStream_t st = h->stream;
-  int rc = bal_evaluate(h, k, nc, sync_base(h->cfg.seed, call, r, SALT_UBAL_TIE), false, h->ubal_tmask.p);
+  int rc = bal_evaluate(h, k, nc, sync_base(h->cfg.seed, call, r, SALT_UBAL_TIE), false, h->bal.tmask.p);
   if (rc != KMP_OK) {
     return rc;
   }
   // Most candidates have no underloaded neighbour block (typically few blocks are underloaded): compacting them
   // away costs one select and a read-back, where sorting them into a zero-deficit segment would cost radix passes
   // over nearly every vertex.
-  uint32_t *list = h->bal_lists.p; // free again after the evaluation
+  uint32_t *list = h->bal.lists.p; // free again after the evaluation
   KMP_CUDA(cub_call(h, [&](void *tmp, size_t &bytes) {
-    return cub::DeviceSelect::If(tmp, bytes, thrust::counting_iterator<uint32_t>(0), list, h->bal_ctrl.p + 5,
-                                 static_cast<int>(nc), UbalHasTarget{h->bal_cand.p, h->label.p, h->bal_target.p}, st);
+    return cub::DeviceSelect::If(tmp, bytes, thrust::counting_iterator<uint32_t>(0), list, h->bal.ctrl.p + 5,
+                                 static_cast<int>(nc), UbalHasTarget{h->bal.cand.p, h->lp.label.p, h->bal.target.p}, st);
   }));
   unsigned long long nt64 = 0;
-  KMP_CUDA(cudaMemcpyAsync(&nt64, h->bal_ctrl.p + 5, sizeof(nt64), cudaMemcpyDeviceToHost, st));
+  KMP_CUDA(cudaMemcpyAsync(&nt64, h->bal.ctrl.p + 5, sizeof(nt64), cudaMemcpyDeviceToHost, st));
   KMP_CUDA(cudaStreamSynchronize(st));
   *nt = static_cast<uint32_t>(nt64);
   if (*nt == 0) {
     return KMP_OK;
   }
-  ubal_sort_keys<<<capped(h, grid_for(*nt, 256)), 256, 0, st>>>(*nt, list, h->bal_target.p, h->bal_key.p, h->bal_sk_a.p,
-                                                                h->bal_sv_a.p);
-  h->kernel_launches += 2;
+  ubal_sort_keys<<<capped(h, grid_for(*nt, 256)), 256, 0, st>>>(*nt, list, h->bal.target.p, h->bal.key.p, h->bal.sk_a.p,
+                                                                h->bal.sv_a.p);
+  h->counts.kernel_launches += 2;
   KMP_CUDA(cudaGetLastError());
   return KMP_OK;
 }
@@ -172,7 +172,7 @@ int kmp_underload_balance(kmp_lp_handle *h, uint32_t k, const int32_t *max_block
     stats->underload_after = static_cast<int64_t>(res.after);
     stats->candidates = res.candidates;
     stats->edges_scanned = res.edges;
-    stats->kernel_launches = h->kernel_launches;
+    stats->kernel_launches = h->counts.kernel_launches;
     stats->device_ms = res.device_ms;
   }
   return KMP_OK;

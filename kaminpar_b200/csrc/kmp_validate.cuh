@@ -232,7 +232,7 @@ int validate_impl(kmp_lp_handle *h, uint32_t n, uint32_t m, const uint32_t *xadj
   if (m > 0) { // CUB's temporary, grown now (the query reads no data) so that the sort below allocates nothing
     size_t bytes = 0;
     KMP_CUDA(sort(nullptr, bytes));
-    KMP_CUDA(h->cub_tmp.ensure(bytes));
+    KMP_CUDA(h->commit.cub_tmp.ensure(bytes));
   }
   KMP_CUDA(call_clock_start(h, st));
   ValCtl init{};
@@ -323,7 +323,7 @@ int validate_checked(kmp_lp_handle *h, uint32_t n, uint32_t m, const uint32_t *x
   if (h == nullptr || out == nullptr || xadj == nullptr || (m > 0 && adjncy == nullptr)) {
     return fail(KMP_ERR_INVALID, "null argument");
   }
-  if (h->step_open) {
+  if (h->step.open) {
     return fail(KMP_ERR_INVALID, "the handle is inside a stepping call");
   }
   if (n > 0x7FFFFFFFu || m > 0x7FFFFFFFu) {
