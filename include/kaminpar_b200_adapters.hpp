@@ -23,6 +23,8 @@
 //                      kaminpar-shm/graphutils/permutator.cc:66-91, 236-264, kaminpar.cc:368-445 (DESIGN.md §15)
 //   Subgraphs / extract_subgraphs / copy_subgraph_partitions
 //                      kaminpar-shm/graphutils/subgraph_extractor.cc:181-324, 492-533 (DESIGN.md §16)
+//   MetisGraph / read_metis
+//                      kaminpar-io/metis_parser.cc:158-245 (csr_read on the device, DESIGN.md §18)
 //   GraphReport / validate_graph
 //                      kaminpar-shm/datastructures/csr_graph.cc:266-356 (debug::validate_graph, DESIGN.md §17)
 //
@@ -39,6 +41,7 @@
 
 #include "kaminpar_b200_balancer.h"
 #include "kaminpar_b200_contraction.h"
+#include "kaminpar_b200_io.h"
 #include "kaminpar_b200_lp.h"
 #include "kaminpar_b200_prepare.h"
 #include "kaminpar_b200_subgraph.h"
@@ -627,6 +630,85 @@ inline GraphReport validate_graph(kmp_lp_handle *h, const CSRGraphView &graph) {
   detail::check(kmp_validate_graph(h, graph.n(), graph.m(), graph.nodes.data(), graph.edges.data(),
                                    graph.edge_weights.empty() ? nullptr : graph.edge_weights.data(), &r));
   return r;
+}
+
+// The report of a METIS read (include/kaminpar_b200_io.h): for a graph, the dropped weights and the reference's
+// "ignorning extra lines" warning; for a refused file, its first violation.
+struct MetisReport : kmp_metis_report {
+  [[nodiscard]] std::string message() const {
+    const int len = kmp_metis_report_message(this, nullptr, 0);
+    std::string out(static_cast<std::size_t>(len > 0 ? len : 0) + 1, '\0');
+    kmp_metis_report_message(this, out.data(), out.size());
+    out.resize(out.size() - 1);
+    return out;
+  }
+};
+
+// A refused METIS file: what() is the report's line, report() its first violation.
+class MetisError : public std::runtime_error {
+public:
+  explicit MetisError(const MetisReport &r) : std::runtime_error("kaminpar_b200: " + r.message()), _report(r) {}
+  [[nodiscard]] const MetisReport &report() const { return _report; }
+
+private:
+  MetisReport _report;
+};
+
+// A METIS file parsed on the device of the handle that read it, in that handle's pool: destroy it before the handle.
+// device_*() go straight to kmp_lp_set_graph_device or kmp_prepare_graph_device; download() copies to host arrays
+// (the CPU parts of KaMinPar: INTEGRATION.md §2h).
+class MetisGraph {
+public:
+  struct Host {
+    std::vector<EdgeID> xadj;
+    std::vector<NodeID> adjncy;
+    std::vector<NodeWeight> vwgt;   // empty: unit weights
+    std::vector<EdgeWeight> adjwgt; // empty: unit weights
+  };
+
+  MetisGraph(kmp_metis_graph *g, const MetisReport &r) : _g(g, &kmp_metis_destroy), _report(r) {
+    detail::check(kmp_metis_device_arrays(g, &_xadj, &_adjncy, &_vwgt, &_adjwgt));
+  }
+  [[nodiscard]] NodeID n() const { return kmp_metis_n(_g.get()); }
+  [[nodiscard]] EdgeID m() const { return kmp_metis_m(_g.get()); }
+  [[nodiscard]] const MetisReport &report() const { return _report; }
+  [[nodiscard]] const EdgeID *device_xadj() const { return _xadj; }
+  [[nodiscard]] const NodeID *device_adjncy() const { return _adjncy; }
+  [[nodiscard]] const NodeWeight *device_vwgt() const { return _vwgt; } // null: unit weights
+  [[nodiscard]] const EdgeWeight *device_adjwgt() const { return _adjwgt; }
+  [[nodiscard]] Host download() const {
+    Host out;
+    out.xadj.resize(static_cast<std::size_t>(n()) + 1);
+    out.adjncy.resize(m());
+    out.vwgt.resize(_vwgt != nullptr ? n() : 0);
+    out.adjwgt.resize(_adjwgt != nullptr ? m() : 0);
+    detail::check(kmp_metis_download(_g.get(), out.xadj.data(), out.adjncy.data(),
+                                     out.vwgt.empty() ? nullptr : out.vwgt.data(),
+                                     out.adjwgt.empty() ? nullptr : out.adjwgt.data()));
+    return out;
+  }
+
+private:
+  std::unique_ptr<kmp_metis_graph, void (*)(kmp_metis_graph *)> _g;
+  MetisReport _report;
+  const EdgeID *_xadj = nullptr;
+  const NodeID *_adjncy = nullptr;
+  const NodeWeight *_vwgt = nullptr;
+  const EdgeWeight *_adjwgt = nullptr;
+};
+
+// io::metis::read_graph(path) (csr_read, kaminpar-io/metis_parser.cc:158-245) on the device, stream and pool of `h`
+// (its graph, labels and call counter are not touched). A malformed file throws MetisError with its first violation;
+// any other refusal std::runtime_error.
+inline MetisGraph read_metis(kmp_lp_handle *h, const std::string &path) {
+  MetisReport r{};
+  kmp_metis_graph *g = nullptr;
+  const int rc = kmp_read_metis(h, path.c_str(), &g, &r);
+  if (rc != KMP_OK && r.kind != KMP_METIS_OK) {
+    throw MetisError(r);
+  }
+  detail::check(rc);
+  return MetisGraph(g, r);
 }
 
 } // namespace kaminpar_b200

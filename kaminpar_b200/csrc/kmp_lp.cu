@@ -3133,6 +3133,7 @@ int kmp_lp_step_finish(kmp_lp_handle *h, uint32_t *labels_out, int32_t *block_we
 #include "kmp_prepare.cuh"
 #include "kmp_subgraph.cuh"
 #include "kmp_validate.cuh"
+#include "kmp_metis.cuh"
 
 #ifdef KMP_HUB_PHASE_STAMPS
 // scripts/hub_rate_phases.py: reads (and with reset != 0 zeroes) the rate kernel's 7 phase accumulators
