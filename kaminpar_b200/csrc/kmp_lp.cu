@@ -3151,3 +3151,20 @@ extern "C" int kmp_hub_phase_read(unsigned long long *out, int reset) {
   return 0;
 }
 #endif
+
+#ifdef KMP_TEAM_PHASE_STAMPS
+// scripts/team_phases.py: reads (and with reset != 0 zeroes) tier 3's 7 phase accumulators (lp_sweep.cuh,
+// g_team_phase). Only in a library built with -DKMP_TEAM_PHASE_STAMPS.
+extern "C" int kmp_team_phase_read(unsigned long long *out, int reset) {
+  if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpyFromSymbol(out, kmp::g_team_phase, 7 * sizeof(unsigned long long)) != cudaSuccess) {
+    return 1;
+  }
+  if (reset != 0) {
+    const unsigned long long zero[7] = {};
+    if (cudaMemcpyToSymbol(kmp::g_team_phase, zero, sizeof(zero)) != cudaSuccess) {
+      return 1;
+    }
+  }
+  return 0;
+}
+#endif

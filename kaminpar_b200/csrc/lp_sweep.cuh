@@ -40,6 +40,22 @@ __device__ __forceinline__ void emit_proposal(const SweepArgs &a, uint32_t idx, 
   }
 }
 
+// A warp's `staged` proposals, lane j holding the j-th: one atomic reserves their slots (the commit is order-free).
+template <int MODE>
+__device__ __forceinline__ void emit_staged(const SweepArgs &a, uint32_t &staged, uint32_t u, uint32_t target,
+                                            int32_t uw) {
+  uint32_t base = 0;
+  if ((threadIdx.x & 31) == 0) {
+    base = atomicAdd(a.mover_count, staged);
+  }
+  base = __shfl_sync(kFull, base, 0);
+  const uint32_t lane = threadIdx.x & 31;
+  if (lane < staged) {
+    emit_proposal<MODE>(a, base + lane, u, target, uw);
+  }
+  staged = 0;
+}
+
 __device__ __forceinline__ void block_count_flush(const SweepArgs &a, unsigned long long edges,
                                                   unsigned long long nodes) {
   // warp-level then one atomic per warp
@@ -400,6 +416,61 @@ __device__ __forceinline__ int32_t team_rating(const typename TeamVals<V16>::wor
 // lists) fit 3 with <= 40 registers, tier 6 takes a whole SM. tests/test_team_resources.py checks the build.
 template <int T> constexpr int team_ctas_per_sm() { return T == 32 ? 6 : T == 1024 ? 1 : 3; }
 
+// List entries a team claims from the work queue with one atomic. Tier 3's sub-rounds hand each SM ~300 vertices
+// within ~75 us, so one claim per vertex paces the single queue address; a batch costs at most batch - 1 vertices of
+// imbalance per team at the tail (a tier-3 warp sees ~6.5 vertices per sub-round). The larger teams claim a vertex
+// every ~6 ns or less often and keep one entry per claim. DESIGN §5 has the measured sizes.
+template <int T> __host__ __device__ constexpr uint32_t team_claim_batch() { return T == 32 ? 2 : 1; }
+
+// Per-phase device time of tier 3's vertices (one-warp teams), for scripts/team_phases.py: only a library built with
+// -DKMP_TEAM_PHASE_STAMPS takes %globaltimer stamps; otherwise they compile to nothing. Lane 0 stamps the end of each
+// phase after consuming the values the phase loaded, so their latency counts in it, and adds per warp, in ns:
+// [0] claim wait, [1] header loads, [2] gather + insert, [3] select, [4] finish (clear, active write, proposal),
+// [5] vertices claimed, [6] vertices rated.
+#ifdef KMP_TEAM_PHASE_STAMPS
+constexpr bool kTeamPhaseStamps = true;
+#else
+constexpr bool kTeamPhaseStamps = false;
+#endif
+__device__ unsigned long long g_team_phase[8];
+template <int T> struct TeamPhases {
+  static constexpr bool kOn = kTeamPhaseStamps && T == 32;
+  unsigned long long t = 0;
+  uint32_t acc[7] = {};
+  uint32_t sink = 0; // consumes each phase's loads before its stamp
+  __device__ __forceinline__ void start() {
+    if constexpr (kOn) {
+      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    }
+  }
+  __device__ __forceinline__ void lap(int i, uint32_t dep) {
+    if constexpr (kOn) {
+      sink ^= dep;
+      unsigned long long now;
+      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now) : "r"(sink));
+      acc[i] += static_cast<uint32_t>(now - t);
+      t = now;
+    }
+  }
+  __device__ __forceinline__ void count(int i) {
+    if constexpr (kOn) {
+      ++acc[i];
+    }
+  }
+  __device__ __forceinline__ void flush(int tid) {
+    if constexpr (kOn) {
+      if (tid == 0) {
+        for (int i = 0; i < 7; ++i) {
+          atomicAdd(&g_team_phase[i], static_cast<unsigned long long>(acc[i]));
+        }
+        if (sink == 0x9E3779B9u) {
+          g_team_phase[7] = 1; // keeps the consumers
+        }
+      }
+    }
+  }
+};
+
 template <int MODE, bool EW, bool P64, int T, int SLOTS, int TEAMS, bool V16 = false>
 __global__ void __launch_bounds__(T *TEAMS, team_ctas_per_sm<T>()) sweep_team(const SweepArgs a) {
   static_assert((SLOTS & (SLOTS - 1)) == 0, "table size must be a power of two");
@@ -429,11 +500,22 @@ __global__ void __launch_bounds__(T *TEAMS, team_ctas_per_sm<T>()) sweep_team(co
     keys[s] = kEmpty;
     TV::clear(vals, s);
   }
-  // work queue: the next list index is claimed one vertex ahead (by thread 0; its result is needed a vertex later)
-  uint32_t next = 0;
+  // work queue: thread 0 claims kClaim consecutive list entries per atomic, and the next batch while the team works
+  // on the last entry of the current one (its result is needed a vertex later). Every claim adds kClaim to a queue
+  // that starts at 0, so a batch ends where the index is one below a multiple of kClaim. The list is consumed in
+  // order: an index past its end means the queue is dry.
+  constexpr uint32_t kClaim = team_claim_batch<T>();
+  static_assert((kClaim & (kClaim - 1)) == 0, "claim batches are aligned powers of two");
+  uint32_t next = 0; // thread 0
   unsigned long long edges = 0, nodes = 0; // T == 32
+  // proposals of a one-warp team: lane j holds the warp's j-th unreserved proposal, and one atomic on a.mover_count
+  // reserves the slots of 32 of them (or of the rest when the queue runs dry). Larger teams propose a vertex every
+  // ~6 ns or less often and take one slot per proposal (staging measured slower there: DESIGN §5).
+  uint32_t st_u = 0, st_t = 0, staged = 0;
+  int32_t st_w = 0;
+  TeamPhases<T> ph;
   if (tid == 0) {
-    next = atomicAdd(a.queue, 1u);
+    next = atomicAdd(a.queue, kClaim);
     if (T > 32) {
       s_edges[team] = 0;
       s_nodes[team] = 0;
@@ -441,6 +523,7 @@ __global__ void __launch_bounds__(T *TEAMS, team_ctas_per_sm<T>()) sweep_team(co
   }
   TeamSync<T>::sync(bar); // the table is clear before the first inserts
   while (true) {
+    ph.start();
     uint32_t i;
     if (T == 32) {
       i = __shfl_sync(kFull, next, 0);
@@ -455,8 +538,10 @@ __global__ void __launch_bounds__(T *TEAMS, team_ctas_per_sm<T>()) sweep_team(co
     if (i >= a.list_size) {
       break;
     }
+    ph.lap(0, i);
+    ph.count(5);
     if (tid == 0) {
-      next = atomicAdd(a.queue, 1u);
+      next = (next & (kClaim - 1)) == kClaim - 1 ? atomicAdd(a.queue, kClaim) : next + 1;
     }
     const uint32_t u = a.list[i];
     const bool flag = a.active == nullptr || a.active[u] != 0;
@@ -472,6 +557,7 @@ __global__ void __launch_bounds__(T *TEAMS, team_ctas_per_sm<T>()) sweep_team(co
     const uint32_t own = a.label[u];
     const int32_t uw = a.vwgt != nullptr ? a.vwgt[u] : 1;
     const int32_t own_w = a.weight[own];
+    ph.lap(1, deg ^ own ^ static_cast<uint32_t>(uw ^ own_w));
     bool skip = false;
     if (MODE == 1) {
       const int32_t mn = a.min_w != nullptr ? a.min_w[own] : 0;
@@ -545,6 +631,7 @@ __global__ void __launch_bounds__(T *TEAMS, team_ctas_per_sm<T>()) sweep_team(co
     const bool any_hit = TeamSync<T>::any(bar, hit); // also the barrier after the inserts
     const bool act = flag || any_hit;
     const uint32_t nc = T == 32 ? claims : s_claims[team];
+    ph.lap(2, nc ^ static_cast<uint32_t>(act));
     // ---- 2. select over the listed slots: thread tid takes entries tid, tid + T, ... --------------
     const bool store_fav = (MODE == 0) && (uw == own_w) && (own_w <= a.max_cluster_weight / 2);
     Cand best = cand_none(), fav = cand_none();
@@ -626,7 +713,9 @@ __global__ void __launch_bounds__(T *TEAMS, team_ctas_per_sm<T>()) sweep_team(co
         }
         best = team_argmax<1, T>(bar, tid, c, s_red);
       }
+      ph.count(6);
     }
+    ph.lap(3, best.key ^ fav.key);
     // ---- 3. clear the listed slots, finish the vertex ---------------------------------------------
     // no barrier first: every thread clears exactly the entries it scanned
     for (uint32_t l = tid; l < nc; l += T) {
@@ -634,6 +723,8 @@ __global__ void __launch_bounds__(T *TEAMS, team_ctas_per_sm<T>()) sweep_team(co
       keys[s] = kEmpty;
       TV::clear(vals, s);
     }
+    bool proposes = false;
+    uint32_t target = 0;
     if (act && tid == 0) {
       if (T == 32) {
         edges += deg;
@@ -645,14 +736,30 @@ __global__ void __launch_bounds__(T *TEAMS, team_ctas_per_sm<T>()) sweep_team(co
       if (a.active != nullptr && flag) {
         a.active[u] = 0;
       }
-      uint32_t target;
-      if (finish_vertex<MODE>(a, u, own, store_fav, best, fav, target)) {
-        const uint32_t idx = atomicAdd(a.mover_count, 1u);
-        emit_proposal<MODE>(a, idx, u, target, uw);
+      proposes = finish_vertex<MODE>(a, u, own, store_fav, best, fav, target);
+    }
+    if (T == 32) {
+      if (__shfl_sync(kFull, proposes, 0)) {
+        target = __shfl_sync(kFull, target, 0);
+        if (lane == staged) {
+          st_u = u;
+          st_t = target;
+          st_w = uw;
+        }
+        if (++staged == 32) {
+          emit_staged<MODE>(a, staged, st_u, st_t, st_w);
+        }
       }
+    } else if (proposes) {
+      emit_proposal<MODE>(a, atomicAdd(a.mover_count, 1u), u, target, uw);
     }
     TeamSync<T>::sync(bar); // table clean
+    ph.lap(4, staged);
   }
+  if (T == 32 && staged != 0) {
+    emit_staged<MODE>(a, staged, st_u, st_t, st_w);
+  }
+  ph.flush(tid);
   if (T > 32 && tid == 0) {
     edges = s_edges[team];
     nodes = s_nodes[team];

@@ -4,6 +4,8 @@
 //   smem_cas_add      : per edge one atomicCAS + one atomicAdd on a shared-memory hash table
 //   smem_plain        : per edge plain ld/st claims on a shared-memory table (optimistic insertion)
 //   redg / atomg      : per edge one RED / one ATOM.EXCH on a random word of an L2-resident table
+//   atom_same         : atomicAdd with return on ONE address, from lane 0 of every warp of the grid, at the tier-3
+//                       team kernel's launch shape (6 x 256-thread CTAs per SM): the work-queue claim / proposal slot
 // Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -o microbench_lsu microbench_lsu.cu
 #include <cstdint>
 #include <cstdio>
@@ -253,6 +255,20 @@ template <int B, bool RET> __global__ void __launch_bounds__(256) k_gatom(const 
   }
 }
 
+// lane 0 of every warp: R atomicAdds with return on one word (the team kernels' queue claim and proposal slot)
+template <int R> __global__ void __launch_bounds__(256) k_atom_same(uint32_t *ctr, unsigned long long *out) {
+  if ((threadIdx.x & 31) != 0) {
+    return;
+  }
+  uint32_t acc = 0;
+  for (int r = 0; r < R; ++r) {
+    acc += atomicAdd(ctr, 1u);
+  }
+  if (acc == 0x1234567u) {
+    out[0] = acc;
+  }
+}
+
 template <typename F> float time_ms(F f, int reps) {
   cudaEvent_t a, b;
   cudaEventCreate(&a);
@@ -336,6 +352,16 @@ int main() {
     const size_t smem2 = (C + 2 * T * EPT) * 4;
     ms = time_ms([&] { k_smem_plain<T, EPT, C><<<kSMs * 8, T, smem2>>>(adj, m, out); }, 3);
     printf(", \"smem_plain_t128_G_s\": %.1f", m / ms * 1e-6);
+  }
+  {
+    constexpr int R = 256;
+    const uint32_t blocks = kSMs * 6;
+    uint32_t *ctr;
+    CK(cudaMalloc(&ctr, 4));
+    CK(cudaMemset(ctr, 0, 4));
+    const float ms = time_ms([&] { k_atom_same<R><<<blocks, 256>>>(ctr, out); }, 5);
+    printf(", \"atom_same_addr_per_ns\": %.3f", (double)blocks * 8 * R / (ms * 1e6));
+    cudaFree(ctr);
   }
   printf("}\n");
   return 0;
