@@ -910,8 +910,8 @@ template <int MODE, bool EW, bool P64> bool configure_team_kernels(kmp_lp_handle
   } else {
     cudaFuncSetAttribute(sweep_hub_scatter<MODE, EW, P64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kHubScatterSmem);
   }
-  bool ok = configure_team<MODE, EW, P64, 32, 512, 8, !EW>(h, sms) && configure_team<MODE, EW, P64, 128, 2048, 4>(h, sms) &&
-            configure_team<MODE, EW, P64, 512, 8192, 1>(h, sms);
+  bool ok = configure_team<MODE, EW, P64, 32, 512, 8, !EW>(h, sms) && configure_team<MODE, EW, P64, 128, 2048, 4, !EW>(h, sms) &&
+            configure_team<MODE, EW, P64, 512, 8192, 1, !EW>(h, sms);
   if constexpr (EW) {
     ok = ok && configure_team<MODE, EW, P64, 1024, 16384, 1>(h, sms);
   } else {
@@ -939,11 +939,11 @@ template <int MODE, bool EW, bool P64> cudaError_t launch_sweep_t(kmp_lp_handle 
           // 16-bit ratings with unit edge weights (a rating is at most the degree), which leaves room for the claim lists
     launch_team<MODE, EW, P64, 32, 512, 8, !EW>(h, a);
     break;
-  case 4: // deg < 1024: 128 threads per vertex, 2048 slots
-    launch_team<MODE, EW, P64, 128, 2048, 4>(h, a);
+  case 4: // deg < 1024: 128 threads per vertex, 2048 slots; 16-bit ratings with unit edge weights
+    launch_team<MODE, EW, P64, 128, 2048, 4, !EW>(h, a);
     break;
-  case 5: // deg < 4096: 512 threads per vertex, 8192 slots
-    launch_team<MODE, EW, P64, 512, 8192, 1>(h, a);
+  case 5: // deg < 4096: 512 threads per vertex, 8192 slots; 16-bit ratings with unit edge weights
+    launch_team<MODE, EW, P64, 512, 8192, 1, !EW>(h, a);
     break;
   case 6: // 1024 threads per vertex; deg < 8192: 16384 slots, or (unit edge weights) deg < 16384: 32768 slots
     if constexpr (EW) {

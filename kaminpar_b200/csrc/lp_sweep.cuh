@@ -6,6 +6,7 @@
 //   tier 3 (deg 32..255)   sweep_team<T=32>   : one warp per vertex, 512-slot shared-memory hash map
 //   tier 4 (deg 256..1023) sweep_team<T=128>  : 128 threads per vertex, 2048 slots
 //   tier 5 (deg 1024..4095) sweep_team<T=512> : one 512-thread CTA per vertex, 8192 slots
+//   (tiers 3-5 with unit edge weights: 16-bit ratings)
 //   tier 6 (deg 4096..8191, or ..16383 with unit edge weights: 16-bit ratings) sweep_team<T=1024>: one
 //                          1024-thread CTA per vertex, 16384 / 32768 slots
 //   tier 7 (deg >= 8192 / 16384) sweep_hub_*  : clusterer: staged labels rated per hash class, one CTA per class;
@@ -70,6 +71,15 @@ __device__ __forceinline__ void block_count_flush(const SweepArgs &a, unsigned l
 }
 
 // ---- neighbour access ---------------------------------------------------------------------------
+// A team reads each adjacency entry once per visit, in coalesced rows: those loads do not allocate in L1, which then
+// keeps the gathered labels -- the highest-degree vertices' labels are gathered far more often than others.
+template <typename W> __device__ __forceinline__ W load_row_entry(const W *p) {
+  static_assert(sizeof(W) == 4, "adjacency entries and edge weights are 4-byte words");
+  uint32_t x;
+  asm("ld.global.nc.L1::no_allocate.b32 %0, [%1];" : "=r"(x) : "l"(p));
+  return static_cast<W>(x);
+}
+
 template <bool P64>
 __device__ __forceinline__ typename LabG<P64>::word load_labg(const SweepArgs &a, uint32_t v) {
   return static_cast<const typename LabG<P64>::word *>(a.labg)[v];
@@ -412,8 +422,9 @@ __device__ __forceinline__ int32_t team_rating(const typename TeamVals<V16>::wor
 // CTAs per SM a team tier is built for. __launch_bounds__ caps the registers so that this many fit
 // (65536 / (threads * CTAs), allocated in steps of 8): tier 3 (256 threads) fits 6 with <= 40 registers, and with
 // edge weights it is held to 6 by shared memory too (32 KiB table + 4 KiB claim lists + the 1 KiB cuobjdump counts
-// as static + 1 KiB reserved per CTA: exactly 228 KiB for 6), tiers 4 and 5 (512 threads, 64 KiB table + 8 KiB
-// lists) fit 3 with <= 40 registers, tier 6 takes a whole SM. tests/test_team_resources.py checks the build.
+// as static + 1 KiB reserved per CTA: exactly 228 KiB for 6), tiers 4 and 5 (512 threads, 48 KiB table with 16-bit
+// ratings or 64 KiB with edge weights, 8 KiB lists) fit 3 with <= 40 registers, tier 6 takes a whole SM.
+// tests/test_team_resources.py checks the build.
 template <int T> constexpr int team_ctas_per_sm() { return T == 32 ? 6 : T == 1024 ? 1 : 3; }
 
 // List entries a team claims from the work queue with one atomic. Tier 3's sub-rounds hand each SM ~300 vertices
@@ -576,8 +587,8 @@ __global__ void __launch_bounds__(T *TEAMS, team_ctas_per_sm<T>()) sweep_team(co
 #pragma unroll
       for (int j = 0; j < B; ++j) {
         const uint32_t e = e0 + j * T + tid;
-        vb[j] = e < deg ? a.adjncy[beg + e] : kEmpty;
-        wb[j] = (EW && e < deg) ? a.adjwgt[beg + e] : 1;
+        vb[j] = e < deg ? load_row_entry(a.adjncy + beg + e) : kEmpty;
+        wb[j] = (EW && e < deg) ? load_row_entry(a.adjwgt + beg + e) : 1;
       }
 #pragma unroll
       for (int j = 0; j < B; ++j) {
