@@ -25,6 +25,8 @@
 //                      kaminpar-shm/graphutils/subgraph_extractor.cc:181-324, 492-533 (DESIGN.md §16)
 //   MetisGraph / read_metis
 //                      kaminpar-io/metis_parser.cc:158-245 (csr_read on the device, DESIGN.md §18)
+//   ParhipGraph / read_parhip
+//                      kaminpar-io/parhip_parser.cc:179-336 (read_graph without compression, DESIGN.md §19)
 //   GraphReport / validate_graph
 //                      kaminpar-shm/datastructures/csr_graph.cc:266-356 (debug::validate_graph, DESIGN.md §17)
 //
@@ -42,6 +44,7 @@
 #include "kaminpar_b200_balancer.h"
 #include "kaminpar_b200_contraction.h"
 #include "kaminpar_b200_io.h"
+#include "kaminpar_b200_parhip.h"
 #include "kaminpar_b200_lp.h"
 #include "kaminpar_b200_prepare.h"
 #include "kaminpar_b200_subgraph.h"
@@ -709,6 +712,99 @@ inline MetisGraph read_metis(kmp_lp_handle *h, const std::string &path) {
   }
   detail::check(rc);
   return MetisGraph(g, r);
+}
+
+// The report of a ParHIP read (include/kaminpar_b200_parhip.h): for a refused file, its first violation.
+struct ParhipReport : kmp_parhip_report {
+  [[nodiscard]] std::string message() const {
+    const int len = kmp_parhip_report_message(this, nullptr, 0);
+    std::string out(static_cast<std::size_t>(len > 0 ? len : 0) + 1, '\0');
+    kmp_parhip_report_message(this, out.data(), out.size());
+    out.resize(out.size() - 1);
+    return out;
+  }
+};
+
+// A refused ParHIP file: what() is the report's line, report() its first violation.
+class ParhipError : public std::runtime_error {
+public:
+  explicit ParhipError(const ParhipReport &r) : std::runtime_error("kaminpar_b200: " + r.message()), _report(r) {}
+  [[nodiscard]] const ParhipReport &report() const { return _report; }
+
+private:
+  ParhipReport _report;
+};
+
+// The node orderings of read_graph (kaminpar::shm::NodeOrdering, kaminpar.h:66-71)
+enum class ParhipOrdering : int {
+  NATURAL = KMP_PARHIP_NATURAL,
+  DEGREE_BUCKETS = KMP_PARHIP_DEGREE_BUCKETS,
+  EXTERNAL_DEGREE_BUCKETS = KMP_PARHIP_EXTERNAL_DEGREE_BUCKETS,
+  IMPLICIT_DEGREE_BUCKETS = KMP_PARHIP_IMPLICIT_DEGREE_BUCKETS
+};
+
+// A ParHIP file read on the device of the handle that read it, in that handle's pool: destroy it before the handle.
+// device_*() go straight to kmp_lp_set_graph_device, kmp_validate_graph_device or kmp_prepare_graph_device;
+// download() copies to host arrays (INTEGRATION.md §2i). sorted() and old_to_new are those of the ordering.
+class ParhipGraph {
+public:
+  struct Host {
+    std::vector<EdgeID> xadj;
+    std::vector<NodeID> adjncy;
+    std::vector<NodeWeight> vwgt;   // empty: unit weights
+    std::vector<EdgeWeight> adjwgt; // empty: unit weights
+    std::vector<NodeID> old_to_new; // empty unless EXTERNAL_DEGREE_BUCKETS
+  };
+
+  ParhipGraph(kmp_parhip_graph *g, const ParhipReport &r) : _g(g, &kmp_parhip_destroy), _report(r) {
+    detail::check(kmp_parhip_device_arrays(g, &_xadj, &_adjncy, &_vwgt, &_adjwgt, &_old_to_new));
+  }
+  [[nodiscard]] NodeID n() const { return kmp_parhip_n(_g.get()); }
+  [[nodiscard]] EdgeID m() const { return kmp_parhip_m(_g.get()); }
+  [[nodiscard]] bool sorted() const { return kmp_parhip_sorted(_g.get()) != 0; }
+  [[nodiscard]] const ParhipReport &report() const { return _report; }
+  [[nodiscard]] const EdgeID *device_xadj() const { return _xadj; }
+  [[nodiscard]] const NodeID *device_adjncy() const { return _adjncy; }
+  [[nodiscard]] const NodeWeight *device_vwgt() const { return _vwgt; } // null: unit weights
+  [[nodiscard]] const EdgeWeight *device_adjwgt() const { return _adjwgt; }
+  [[nodiscard]] const NodeID *device_old_to_new() const { return _old_to_new; }
+  [[nodiscard]] Host download() const {
+    Host out;
+    out.xadj.resize(static_cast<std::size_t>(n()) + 1);
+    out.adjncy.resize(m());
+    out.vwgt.resize(_vwgt != nullptr ? n() : 0);
+    out.adjwgt.resize(_adjwgt != nullptr ? m() : 0);
+    out.old_to_new.resize(_old_to_new != nullptr ? n() : 0);
+    detail::check(kmp_parhip_download(_g.get(), out.xadj.data(), out.adjncy.data(),
+                                      out.vwgt.empty() ? nullptr : out.vwgt.data(),
+                                      out.adjwgt.empty() ? nullptr : out.adjwgt.data(),
+                                      out.old_to_new.empty() ? nullptr : out.old_to_new.data()));
+    return out;
+  }
+
+private:
+  std::unique_ptr<kmp_parhip_graph, void (*)(kmp_parhip_graph *)> _g;
+  ParhipReport _report;
+  const EdgeID *_xadj = nullptr;
+  const NodeID *_adjncy = nullptr;
+  const NodeWeight *_vwgt = nullptr;
+  const EdgeWeight *_adjwgt = nullptr;
+  const NodeID *_old_to_new = nullptr;
+};
+
+// io::parhip::read_graph(path, false, ordering) (kaminpar-io/parhip_parser.cc:580-587) on the device, stream and pool
+// of `h` (its graph, labels and call counter are not touched). A malformed file throws ParhipError with its first
+// violation; any other refusal std::runtime_error.
+inline ParhipGraph read_parhip(kmp_lp_handle *h, const std::string &path,
+                               ParhipOrdering ordering = ParhipOrdering::NATURAL) {
+  ParhipReport r{};
+  kmp_parhip_graph *g = nullptr;
+  const int rc = kmp_read_parhip(h, path.c_str(), static_cast<int>(ordering), &g, &r);
+  if (rc != KMP_OK && r.kind != KMP_PARHIP_OK) {
+    throw ParhipError(r);
+  }
+  detail::check(rc);
+  return ParhipGraph(g, r);
 }
 
 } // namespace kaminpar_b200

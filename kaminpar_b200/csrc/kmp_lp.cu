@@ -3134,6 +3134,7 @@ int kmp_lp_step_finish(kmp_lp_handle *h, uint32_t *labels_out, int32_t *block_we
 #include "kmp_subgraph.cuh"
 #include "kmp_validate.cuh"
 #include "kmp_metis.cuh"
+#include "kmp_parhip.cuh"
 
 #ifdef KMP_HUB_PHASE_STAMPS
 // scripts/hub_rate_phases.py: reads (and with reset != 0 zeroes) the rate kernel's 7 phase accumulators

@@ -721,6 +721,40 @@ struct MetisFile {
   }
 };
 
+// Streams the file's `len` bytes into dst (device) on h's stream through the two pinned buffers of `stage` (the
+// caller's, so that they outlive the work it queues after), kMetisChunk bytes each: reading one chunk overlaps the copy
+// of the previous one. Starts h's call clock. queued(end) runs once the copy of bytes [0, end) is queued, to launch the
+// work on them; its error ends the stream.
+template <typename Queued>
+int stream_file(kmp_lp_handle *h, MetisStaging &stage, int fd, const char *path, uint64_t len, uint8_t *dst,
+                Queued &&queued) {
+  const cudaStream_t st = h->stream;
+  stage.st = st;
+  const uint64_t chunk = std::min<uint64_t>(len, kMetisChunk);
+  for (int b = 0; b < 2; ++b) {
+    KMP_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&stage.buf[b]), chunk, cudaHostAllocDefault));
+    KMP_CUDA(cudaEventCreateWithFlags(&stage.ev[b], cudaEventDisableTiming));
+  }
+  KMP_CUDA(call_clock_start(h, st));
+  for (uint64_t off = 0, idx = 0; off < len; off += chunk, ++idx) {
+    const int b = static_cast<int>(idx & 1u);
+    const uint64_t size = std::min<uint64_t>(chunk, len - off);
+    if (idx >= 2) {
+      KMP_CUDA(cudaEventSynchronize(stage.ev[b])); // the copy of chunk idx - 2 is out of this buffer
+    }
+    if (!metis_pread(fd, stage.buf[b], size, off)) {
+      return fail(KMP_ERR_INVALID, std::string("cannot read ") + path);
+    }
+    KMP_CUDA(cudaMemcpyAsync(dst + off, stage.buf[b], size, cudaMemcpyHostToDevice, st));
+    KMP_CUDA(cudaEventRecord(stage.ev[b], st));
+    const int rc = queued(off + size);
+    if (rc != KMP_OK) {
+      return rc;
+    }
+  }
+  return KMP_OK;
+}
+
 // The header from the file's first bytes, fetched by fetch(dst, size) in growing prefixes until metis_header has what
 // it needs; KMP_OK with hd filled, a refusal with r filled, or fetch's error.
 template <typename Fetch> int metis_read_header(uint64_t len, MetisHeader &hd, kmp_metis_report &r, Fetch &&fetch) {
@@ -774,32 +808,16 @@ int read_metis_impl(kmp_lp_handle *h, const char *path, kmp_metis_graph **out, k
       return rc;
     }
     MetisStaging stage;
-    stage.st = st;
-    const uint64_t chunk = std::min<uint64_t>(len, kMetisChunk);
-    for (int b = 0; b < 2; ++b) {
-      KMP_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&stage.buf[b]), chunk, cudaHostAllocDefault));
-      KMP_CUDA(cudaEventCreateWithFlags(&stage.ev[b], cudaEventDisableTiming));
-    }
-    KMP_CUDA(call_clock_start(h, st));
     uint32_t done = 0; // tiles summarised
-    for (uint64_t off = 0, idx = 0; off < len; off += chunk, ++idx) {
-      const int b = static_cast<int>(idx & 1u);
-      const uint64_t size = std::min<uint64_t>(chunk, len - off);
-      if (idx >= 2) {
-        KMP_CUDA(cudaEventSynchronize(stage.ev[b])); // the copy of chunk idx - 2 is out of this buffer
-      }
-      if (!metis_pread(f.fd, stage.buf[b], size, off)) {
-        return fail(KMP_ERR_INVALID, std::string("cannot read ") + path);
-      }
-      KMP_CUDA(cudaMemcpyAsync(g->bytes.p + off, stage.buf[b], size, cudaMemcpyHostToDevice, st));
-      KMP_CUDA(cudaEventRecord(stage.ev[b], st));
+    rc = stream_file(h, stage, f.fd, path, len, g->bytes.p, [&](uint64_t end) {
       // tiles whose bytes (and the byte before them) are all on the device
-      const uint32_t ready = off + size == len ? job.tiles : static_cast<uint32_t>((off + size) / KMP_METIS_TILE_BYTES);
-      rc = job.summarise(done, ready);
-      if (rc != KMP_OK) {
-        return rc;
-      }
+      const uint32_t ready = end == len ? job.tiles : static_cast<uint32_t>(end / KMP_METIS_TILE_BYTES);
+      const int src = job.summarise(done, ready);
       done = ready;
+      return src;
+    });
+    if (rc != KMP_OK) {
+      return rc;
     }
     rc = job.finish(g, r);
     g->bytes.release();
