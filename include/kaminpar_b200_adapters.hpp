@@ -612,17 +612,87 @@ inline void copy_subgraph_partitions(kmp_lp_handle *h, const Subgraphs &subgraph
                                               out.empty() ? nullptr : out.data(), nullptr));
 }
 
+namespace detail {
+// message() of a report: the length query of its kmp_*_report_message, then the text
+template <typename R> std::string report_message(int (*format)(const R *, char *, std::size_t), const R *r) {
+  const int len = format(r, nullptr, 0);
+  std::string out(static_cast<std::size_t>(len > 0 ? len : 0) + 1, '\0');
+  format(r, out.data(), out.size());
+  out.resize(out.size() - 1);
+  return out;
+}
+
+// A refused input file: what() is the report's line, report() its first violation.
+template <typename Report> class ReadError : public std::runtime_error {
+public:
+  explicit ReadError(const Report &r) : std::runtime_error("kaminpar_b200: " + r.message()), _report(r) {}
+  [[nodiscard]] const Report &report() const { return _report; }
+
+private:
+  Report _report;
+};
+
+// The status of a read: a refused file (a violation in its report) throws ReadError, any other refusal
+// std::runtime_error.
+template <typename Report> void check_read(int rc, const Report &r) {
+  if (rc != KMP_OK && r.kind != 0) {
+    throw ReadError<Report>(r);
+  }
+  check(rc);
+}
+
+// What MetisGraph and ParhipGraph share: the owned result G of a read on the device of the handle that read it, in
+// that handle's pool (destroy it before the handle), its report, its four device arrays and their host copy.
+template <typename G, typename Report> class ReadGraph {
+public:
+  struct Host {
+    std::vector<EdgeID> xadj;
+    std::vector<NodeID> adjncy;
+    std::vector<NodeWeight> vwgt;   // empty: unit weights
+    std::vector<EdgeWeight> adjwgt; // empty: unit weights
+  };
+
+  [[nodiscard]] NodeID n() const { return _n; }
+  [[nodiscard]] EdgeID m() const { return _m; }
+  [[nodiscard]] const Report &report() const { return _report; }
+  [[nodiscard]] const EdgeID *device_xadj() const { return _xadj; }
+  [[nodiscard]] const NodeID *device_adjncy() const { return _adjncy; }
+  [[nodiscard]] const NodeWeight *device_vwgt() const { return _vwgt; } // null: unit weights
+  [[nodiscard]] const EdgeWeight *device_adjwgt() const { return _adjwgt; }
+
+protected:
+  ReadGraph(G *g, const Report &r, void (*destroy)(G *), NodeID n, EdgeID m)
+      : _g(g, destroy), _report(r), _n(n), _m(m) {}
+  // out's arrays sized for this graph and filled by download(g, xadj, adjncy, vwgt, adjwgt, extra...)
+  template <typename... Extra>
+  void download_into(Host &out, int (*download)(const G *, EdgeID *, NodeID *, NodeWeight *, EdgeWeight *, Extra...),
+                     Extra... extra) const {
+    out.xadj.resize(static_cast<std::size_t>(_n) + 1);
+    out.adjncy.resize(_m);
+    out.vwgt.resize(_vwgt != nullptr ? _n : 0);
+    out.adjwgt.resize(_adjwgt != nullptr ? _m : 0);
+    check(download(_g.get(), out.xadj.data(), out.adjncy.data(), out.vwgt.empty() ? nullptr : out.vwgt.data(),
+                   out.adjwgt.empty() ? nullptr : out.adjwgt.data(), extra...));
+  }
+
+  std::unique_ptr<G, void (*)(G *)> _g;
+  Report _report;
+  NodeID _n;
+  EdgeID _m;
+  const EdgeID *_xadj = nullptr;
+  const NodeID *_adjncy = nullptr;
+  const NodeWeight *_vwgt = nullptr;
+  const EdgeWeight *_adjwgt = nullptr;
+};
+} // namespace detail
+
 // The report of debug::validate_graph(graph) (csr_graph.cc:266-356) with every edge counted under its first violation
 // and the duplicate neighbours beside it (include/kaminpar_b200_validate.h). valid() is the reference's verdict and
 // message() its warning line for the first violation.
 struct GraphReport : kmp_graph_report {
   [[nodiscard]] bool is_valid() const { return valid != 0; }
   [[nodiscard]] std::string message() const {
-    const int len = kmp_graph_report_message(this, nullptr, 0);
-    std::string out(static_cast<std::size_t>(len > 0 ? len : 0) + 1, '\0');
-    kmp_graph_report_message(this, out.data(), out.size());
-    out.resize(out.size() - 1);
-    return out;
+    return detail::report_message<kmp_graph_report>(&kmp_graph_report_message, this);
   }
 };
 
@@ -639,65 +709,27 @@ inline GraphReport validate_graph(kmp_lp_handle *h, const CSRGraphView &graph) {
 // "ignorning extra lines" warning; for a refused file, its first violation.
 struct MetisReport : kmp_metis_report {
   [[nodiscard]] std::string message() const {
-    const int len = kmp_metis_report_message(this, nullptr, 0);
-    std::string out(static_cast<std::size_t>(len > 0 ? len : 0) + 1, '\0');
-    kmp_metis_report_message(this, out.data(), out.size());
-    out.resize(out.size() - 1);
-    return out;
+    return detail::report_message<kmp_metis_report>(&kmp_metis_report_message, this);
   }
 };
 
 // A refused METIS file: what() is the report's line, report() its first violation.
-class MetisError : public std::runtime_error {
-public:
-  explicit MetisError(const MetisReport &r) : std::runtime_error("kaminpar_b200: " + r.message()), _report(r) {}
-  [[nodiscard]] const MetisReport &report() const { return _report; }
-
-private:
-  MetisReport _report;
-};
+using MetisError = detail::ReadError<MetisReport>;
 
 // A METIS file parsed on the device of the handle that read it, in that handle's pool: destroy it before the handle.
 // device_*() go straight to kmp_lp_set_graph_device or kmp_prepare_graph_device; download() copies to host arrays
 // (the CPU parts of KaMinPar: INTEGRATION.md §2h).
-class MetisGraph {
+class MetisGraph : public detail::ReadGraph<kmp_metis_graph, MetisReport> {
 public:
-  struct Host {
-    std::vector<EdgeID> xadj;
-    std::vector<NodeID> adjncy;
-    std::vector<NodeWeight> vwgt;   // empty: unit weights
-    std::vector<EdgeWeight> adjwgt; // empty: unit weights
-  };
-
-  MetisGraph(kmp_metis_graph *g, const MetisReport &r) : _g(g, &kmp_metis_destroy), _report(r) {
+  MetisGraph(kmp_metis_graph *g, const MetisReport &r)
+      : ReadGraph(g, r, &kmp_metis_destroy, kmp_metis_n(g), kmp_metis_m(g)) {
     detail::check(kmp_metis_device_arrays(g, &_xadj, &_adjncy, &_vwgt, &_adjwgt));
   }
-  [[nodiscard]] NodeID n() const { return kmp_metis_n(_g.get()); }
-  [[nodiscard]] EdgeID m() const { return kmp_metis_m(_g.get()); }
-  [[nodiscard]] const MetisReport &report() const { return _report; }
-  [[nodiscard]] const EdgeID *device_xadj() const { return _xadj; }
-  [[nodiscard]] const NodeID *device_adjncy() const { return _adjncy; }
-  [[nodiscard]] const NodeWeight *device_vwgt() const { return _vwgt; } // null: unit weights
-  [[nodiscard]] const EdgeWeight *device_adjwgt() const { return _adjwgt; }
   [[nodiscard]] Host download() const {
     Host out;
-    out.xadj.resize(static_cast<std::size_t>(n()) + 1);
-    out.adjncy.resize(m());
-    out.vwgt.resize(_vwgt != nullptr ? n() : 0);
-    out.adjwgt.resize(_adjwgt != nullptr ? m() : 0);
-    detail::check(kmp_metis_download(_g.get(), out.xadj.data(), out.adjncy.data(),
-                                     out.vwgt.empty() ? nullptr : out.vwgt.data(),
-                                     out.adjwgt.empty() ? nullptr : out.adjwgt.data()));
+    download_into(out, &kmp_metis_download);
     return out;
   }
-
-private:
-  std::unique_ptr<kmp_metis_graph, void (*)(kmp_metis_graph *)> _g;
-  MetisReport _report;
-  const EdgeID *_xadj = nullptr;
-  const NodeID *_adjncy = nullptr;
-  const NodeWeight *_vwgt = nullptr;
-  const EdgeWeight *_adjwgt = nullptr;
 };
 
 // io::metis::read_graph(path) (csr_read, kaminpar-io/metis_parser.cc:158-245) on the device, stream and pool of `h`
@@ -706,34 +738,19 @@ private:
 inline MetisGraph read_metis(kmp_lp_handle *h, const std::string &path) {
   MetisReport r{};
   kmp_metis_graph *g = nullptr;
-  const int rc = kmp_read_metis(h, path.c_str(), &g, &r);
-  if (rc != KMP_OK && r.kind != KMP_METIS_OK) {
-    throw MetisError(r);
-  }
-  detail::check(rc);
+  detail::check_read(kmp_read_metis(h, path.c_str(), &g, &r), r);
   return MetisGraph(g, r);
 }
 
 // The report of a ParHIP read (include/kaminpar_b200_parhip.h): for a refused file, its first violation.
 struct ParhipReport : kmp_parhip_report {
   [[nodiscard]] std::string message() const {
-    const int len = kmp_parhip_report_message(this, nullptr, 0);
-    std::string out(static_cast<std::size_t>(len > 0 ? len : 0) + 1, '\0');
-    kmp_parhip_report_message(this, out.data(), out.size());
-    out.resize(out.size() - 1);
-    return out;
+    return detail::report_message<kmp_parhip_report>(&kmp_parhip_report_message, this);
   }
 };
 
 // A refused ParHIP file: what() is the report's line, report() its first violation.
-class ParhipError : public std::runtime_error {
-public:
-  explicit ParhipError(const ParhipReport &r) : std::runtime_error("kaminpar_b200: " + r.message()), _report(r) {}
-  [[nodiscard]] const ParhipReport &report() const { return _report; }
-
-private:
-  ParhipReport _report;
-};
+using ParhipError = detail::ReadError<ParhipReport>;
 
 // The node orderings of read_graph (kaminpar::shm::NodeOrdering, kaminpar.h:66-71)
 enum class ParhipOrdering : int {
@@ -746,49 +763,26 @@ enum class ParhipOrdering : int {
 // A ParHIP file read on the device of the handle that read it, in that handle's pool: destroy it before the handle.
 // device_*() go straight to kmp_lp_set_graph_device, kmp_validate_graph_device or kmp_prepare_graph_device;
 // download() copies to host arrays (INTEGRATION.md §2i). sorted() and old_to_new are those of the ordering.
-class ParhipGraph {
+class ParhipGraph : public detail::ReadGraph<kmp_parhip_graph, ParhipReport> {
 public:
-  struct Host {
-    std::vector<EdgeID> xadj;
-    std::vector<NodeID> adjncy;
-    std::vector<NodeWeight> vwgt;   // empty: unit weights
-    std::vector<EdgeWeight> adjwgt; // empty: unit weights
+  struct Host : ReadGraph::Host {
     std::vector<NodeID> old_to_new; // empty unless EXTERNAL_DEGREE_BUCKETS
   };
 
-  ParhipGraph(kmp_parhip_graph *g, const ParhipReport &r) : _g(g, &kmp_parhip_destroy), _report(r) {
+  ParhipGraph(kmp_parhip_graph *g, const ParhipReport &r)
+      : ReadGraph(g, r, &kmp_parhip_destroy, kmp_parhip_n(g), kmp_parhip_m(g)) {
     detail::check(kmp_parhip_device_arrays(g, &_xadj, &_adjncy, &_vwgt, &_adjwgt, &_old_to_new));
   }
-  [[nodiscard]] NodeID n() const { return kmp_parhip_n(_g.get()); }
-  [[nodiscard]] EdgeID m() const { return kmp_parhip_m(_g.get()); }
   [[nodiscard]] bool sorted() const { return kmp_parhip_sorted(_g.get()) != 0; }
-  [[nodiscard]] const ParhipReport &report() const { return _report; }
-  [[nodiscard]] const EdgeID *device_xadj() const { return _xadj; }
-  [[nodiscard]] const NodeID *device_adjncy() const { return _adjncy; }
-  [[nodiscard]] const NodeWeight *device_vwgt() const { return _vwgt; } // null: unit weights
-  [[nodiscard]] const EdgeWeight *device_adjwgt() const { return _adjwgt; }
   [[nodiscard]] const NodeID *device_old_to_new() const { return _old_to_new; }
   [[nodiscard]] Host download() const {
     Host out;
-    out.xadj.resize(static_cast<std::size_t>(n()) + 1);
-    out.adjncy.resize(m());
-    out.vwgt.resize(_vwgt != nullptr ? n() : 0);
-    out.adjwgt.resize(_adjwgt != nullptr ? m() : 0);
     out.old_to_new.resize(_old_to_new != nullptr ? n() : 0);
-    detail::check(kmp_parhip_download(_g.get(), out.xadj.data(), out.adjncy.data(),
-                                      out.vwgt.empty() ? nullptr : out.vwgt.data(),
-                                      out.adjwgt.empty() ? nullptr : out.adjwgt.data(),
-                                      out.old_to_new.empty() ? nullptr : out.old_to_new.data()));
+    download_into(out, &kmp_parhip_download, out.old_to_new.empty() ? nullptr : out.old_to_new.data());
     return out;
   }
 
 private:
-  std::unique_ptr<kmp_parhip_graph, void (*)(kmp_parhip_graph *)> _g;
-  ParhipReport _report;
-  const EdgeID *_xadj = nullptr;
-  const NodeID *_adjncy = nullptr;
-  const NodeWeight *_vwgt = nullptr;
-  const EdgeWeight *_adjwgt = nullptr;
   const NodeID *_old_to_new = nullptr;
 };
 
@@ -799,11 +793,7 @@ inline ParhipGraph read_parhip(kmp_lp_handle *h, const std::string &path,
                                ParhipOrdering ordering = ParhipOrdering::NATURAL) {
   ParhipReport r{};
   kmp_parhip_graph *g = nullptr;
-  const int rc = kmp_read_parhip(h, path.c_str(), static_cast<int>(ordering), &g, &r);
-  if (rc != KMP_OK && r.kind != KMP_PARHIP_OK) {
-    throw ParhipError(r);
-  }
-  detail::check(rc);
+  detail::check_read(kmp_read_parhip(h, path.c_str(), static_cast<int>(ordering), &g, &r), r);
   return ParhipGraph(g, r);
 }
 

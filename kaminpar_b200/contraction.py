@@ -85,9 +85,7 @@ def _lib():
         lib.kmp_coarse_m.restype = C.c_uint32
         lib.kmp_coarse_fine_n.restype = C.c_uint32
         lib.kmp_coarse_destroy.restype = None
-        for sym in ("kmp_sparsification_target", "kmp_coarse_sparsify"):
-            if not hasattr(lib, sym):
-                raise RuntimeError(f"{lp.library_path()} lacks {sym}; rebuild the library")
+        lp.require_symbols(lib, "kmp_sparsification_target", "kmp_coarse_sparsify")
         lib.kmp_sparsification_target.restype = C.c_uint32
         lib.kmp_sparsification_target.argtypes = [C.c_uint32, C.c_uint32, C.c_uint32, C.c_double, C.c_double]
         lib.kmp_coarse_sparsify.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64, C.c_void_p]
@@ -116,12 +114,7 @@ class CoarseGraph(lp.DeviceResult):
 
     def get(self) -> CSRGraph:
         if self._host is None:
-            n, m = self.n, self.m
-            xadj = np.zeros(n + 1, np.uint32)
-            adj = np.zeros(m, np.uint32)
-            vw = np.zeros(n, np.int32)
-            ew = np.zeros(m, np.int32)
-            lp._check(_lib().kmp_coarse_download(self._g, lp._ptr(xadj), lp._ptr(adj), lp._ptr(vw), lp._ptr(ew), None))
+            xadj, adj, vw, ew = self._download_csr("kmp_coarse_download", self.n, self.m, True, True, None)
             self._host = CSRGraph(xadj=xadj, adjncy=adj, vwgt=vw, adjwgt=ew, sorted=False)
         return self._host
 

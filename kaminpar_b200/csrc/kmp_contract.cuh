@@ -27,11 +27,9 @@
 #include <cub/device/device_reduce.cuh>
 #include <cub/device/device_run_length_encode.cuh>
 
-struct kmp_coarse_graph {
-  int device = 0;
+struct kmp_coarse_graph : DeviceCsr {
   uint32_t fine_n = 0, c_n = 0, c_m = 0;
-  PoolBuf<uint32_t> xadj, adjncy, mapping;
-  PoolBuf<int32_t> vwgt, adjwgt;
+  PoolBuf<uint32_t> mapping;
 };
 
 namespace {
@@ -368,11 +366,10 @@ int kmp_coarse_download(const kmp_coarse_graph *g, uint32_t *xadj, uint32_t *adj
   if (g == nullptr) {
     return fail(KMP_ERR_INVALID, "null argument");
   }
-  KMP_CUDA(cudaSetDevice(g->device));
-  KMP_CUDA(copy_out(xadj, g->xadj, static_cast<size_t>(g->c_n) + 1));
-  KMP_CUDA(copy_out(adjncy, g->adjncy, g->c_m));
-  KMP_CUDA(copy_out(vwgt, g->vwgt, g->c_n));
-  KMP_CUDA(copy_out(adjwgt, g->adjwgt, g->c_m));
+  const int rc = download_csr(*g, xadj, adjncy, vwgt, adjwgt, static_cast<size_t>(g->c_n) + 1, g->c_n, g->c_m);
+  if (rc != KMP_OK) {
+    return rc;
+  }
   KMP_CUDA(copy_out(mapping, g->mapping, g->fine_n));
   return KMP_OK;
 }
@@ -382,10 +379,7 @@ int kmp_coarse_device_arrays(const kmp_coarse_graph *g, const uint32_t **d_xadj,
   if (g == nullptr) {
     return fail(KMP_ERR_INVALID, "null argument");
   }
-  hand_out(d_xadj, g->xadj);
-  hand_out(d_adjncy, g->adjncy);
-  hand_out(d_vwgt, g->vwgt);
-  hand_out(d_adjwgt, g->adjwgt);
+  hand_out_csr(*g, d_xadj, d_adjncy, d_vwgt, d_adjwgt);
   hand_out(d_mapping, g->mapping);
   return KMP_OK;
 }
@@ -427,12 +421,6 @@ int kmp_coarse_project_down(const kmp_coarse_graph *g, const uint32_t *fine, uin
   return KMP_OK;
 }
 
-void kmp_coarse_destroy(kmp_coarse_graph *g) {
-  if (g == nullptr) {
-    return;
-  }
-  cudaSetDevice(g->device); // the arrays free themselves on this device's pool
-  delete g;
-}
+void kmp_coarse_destroy(kmp_coarse_graph *g) { destroy_result(g); }
 
 } // extern "C"

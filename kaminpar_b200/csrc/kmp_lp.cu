@@ -222,6 +222,26 @@ template <typename T> void hand_out(const T **dst, const PoolBuf<T> &buf) {
   }
 }
 
+// kmp_*_destroy of a result object: its arrays free themselves on its device's pool
+template <typename T> void destroy_result(T *g) {
+  if (g == nullptr) {
+    return;
+  }
+  cudaSetDevice(g->device);
+  delete g;
+}
+
+// The buffer protocol of the *_report_message calls: the message is formatted into buf (a null or zero-size buffer
+// formats into a one-byte dummy), and its full length is returned
+template <typename... A> int format_report(char *buf, size_t size, const char *fmt, A... args) {
+  char dummy = 0;
+  if (buf == nullptr || size == 0) {
+    buf = &dummy;
+    size = 1;
+  }
+  return std::snprintf(buf, size, fmt, args...);
+}
+
 // The overlay's state on the handle (kmp_overlay.cuh): the stashed clusterings of the last overlay call (pool blocks,
 // kept between calls) and the sort's values
 struct OverlayState {
@@ -237,6 +257,40 @@ struct RunCtx {
   bool has_min;
   bool has_comm;
 };
+} // namespace
+
+// The CSR arrays of a graph result (kmp_metis_graph, kmp_parhip_graph, kmp_prepared_graph, kmp_coarse_graph) on
+// `device`'s pool; vwgt / adjwgt are unallocated for unit weights.
+struct DeviceCsr {
+  int device = 0;
+  PoolBuf<uint32_t> xadj, adjncy;
+  PoolBuf<int32_t> vwgt, adjwgt;
+
+  DeviceCsr() = default;
+  DeviceCsr(DeviceCsr &&) = default;
+  DeviceCsr &operator=(DeviceCsr &&) = default;
+  // always inlined into the result types' destructors: an out-of-line instance of one of those would be a new
+  // exported symbol of the library
+  [[gnu::always_inline]] ~DeviceCsr() = default;
+};
+
+namespace {
+// D2H copy of the arrays of g the caller asks for: xadj_len entries of xadj, n of vwgt and m of adjncy / adjwgt
+int download_csr(const DeviceCsr &g, uint32_t *x, uint32_t *a, int32_t *vw, int32_t *aw, size_t xadj_len, size_t n,
+                 size_t m) {
+  KMP_CUDA(cudaSetDevice(g.device));
+  KMP_CUDA(copy_out(x, g.xadj, xadj_len));
+  KMP_CUDA(copy_out(a, g.adjncy, m));
+  KMP_CUDA(copy_out(vw, g.vwgt, n));
+  KMP_CUDA(copy_out(aw, g.adjwgt, m));
+  return KMP_OK;
+}
+void hand_out_csr(const DeviceCsr &g, const uint32_t **x, const uint32_t **a, const int32_t **vw, const int32_t **aw) {
+  hand_out(x, g.xadj);
+  hand_out(a, g.adjncy);
+  hand_out(vw, g.vwgt);
+  hand_out(aw, g.adjwgt);
+}
 } // namespace
 
 // The handle's buffers are grouped by owner. kmp_lp_free_scratch resets the groups marked "released" (the next call
@@ -2882,6 +2936,28 @@ int kmp_lp_free_scratch(kmp_lp_handle *h) {
   return KMP_OK;
 }
 
+int kmp_pool_usage(kmp_lp_handle *h, int reset, uint64_t *used, uint64_t *used_high) {
+  if (h == nullptr || used == nullptr || used_high == nullptr) {
+    return fail(KMP_ERR_INVALID, "null argument");
+  }
+  KMP_CUDA(cudaSetDevice(h->device));
+  cudaMemPool_t pool = kmp_private_pool(h->device);
+  if (pool == nullptr) {
+    return fail(KMP_ERR_CUDA, "no device memory pool");
+  }
+  KMP_CUDA(cudaStreamSynchronize(h->stream)); // the stream-ordered frees of h's calls have happened
+  uint64_t cur = 0, high = 0;
+  KMP_CUDA(cudaMemPoolGetAttribute(pool, cudaMemPoolAttrUsedMemCurrent, &cur));
+  KMP_CUDA(cudaMemPoolGetAttribute(pool, cudaMemPoolAttrUsedMemHigh, &high));
+  *used = cur;
+  *used_high = high;
+  if (reset != 0) {
+    uint64_t zero = 0; // the only value the attribute accepts: the mark restarts at the current use
+    KMP_CUDA(cudaMemPoolSetAttribute(pool, cudaMemPoolAttrUsedMemHigh, &zero));
+  }
+  return KMP_OK;
+}
+
 int kmp_lp_edge_cut(kmp_lp_handle *h, int64_t *cut_out) {
   if (h == nullptr || !h->graph.present || cut_out == nullptr || h->lp.label.p == nullptr) {
     return fail(KMP_ERR_INVALID, "bad argument");
@@ -3133,6 +3209,7 @@ int kmp_lp_step_finish(kmp_lp_handle *h, uint32_t *labels_out, int32_t *block_we
 #include "kmp_prepare.cuh"
 #include "kmp_subgraph.cuh"
 #include "kmp_validate.cuh"
+#include "kmp_read.cuh"
 #include "kmp_metis.cuh"
 #include "kmp_parhip.cuh"
 

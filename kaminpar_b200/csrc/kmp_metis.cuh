@@ -18,20 +18,12 @@
 //   tile that holds the first violation to fill in its vertex and line.
 #pragma once
 
-#include <fcntl.h>
-#include <sys/stat.h>
-#include <unistd.h>
-
 #include <cub/block/block_scan.cuh>
 
 #include "../../include/kaminpar_b200_io.h"
 
-struct kmp_metis_graph {
-  int device = 0;
+struct kmp_metis_graph : DeviceCsr { // vwgt / adjwgt: unallocated for absent or dropped weights
   uint32_t n = 0, m = 0;
-  PoolBuf<uint32_t> xadj, adjncy;
-  PoolBuf<int32_t> vwgt, adjwgt; // unallocated for absent or dropped weights
-  PoolBuf<uint8_t> bytes;        // the file's bytes (kmp_read_metis), released when the read ends
 };
 
 namespace {
@@ -42,7 +34,6 @@ static_assert(kMetisBytesPerThread == 16, "one uint4 per thread");
 constexpr uint32_t kMLineStart = 0, kMComment = 1, kMData = 2; // line states
 constexpr unsigned long long kMetisCap = 1ull << 40;           // saturation of a token's value: above every id / weight
 constexpr unsigned long long kMetisNone = ~0ull;
-constexpr uint64_t kMetisChunk = 32ull << 20; // bytes per pinned staging buffer of kmp_read_metis
 
 // The line-state machine over a run of bytes, for each entry state s: the exit state (2 bits at 2s), the data lines
 // and tokens that begin, the tokens of the line open at the end (all tokens of the run if no data line begins), and
@@ -666,95 +657,6 @@ void metis_report_header(kmp_metis_report &r, const MetisHeader &hd) {
   r.has_edge_weights = hd.fmt % 10 != 0 ? 1 : 0;
 }
 
-int metis_begin(kmp_lp_handle *h, kmp_metis_graph **out, kmp_metis_report *report) {
-  if (h == nullptr || out == nullptr || report == nullptr) {
-    return fail(KMP_ERR_INVALID, "null argument");
-  }
-  std::memset(report, 0, sizeof(*report));
-  if (h->step.open) {
-    return fail(KMP_ERR_INVALID, "the handle is inside a stepping call");
-  }
-  KMP_CUDA(cudaSetDevice(h->device));
-  return KMP_OK;
-}
-
-// pread until `size` bytes are in or the file ends; false on a read error
-bool metis_pread(int fd, uint8_t *dst, uint64_t size, uint64_t off) {
-  while (size > 0) {
-    const ssize_t got = pread(fd, dst, size, static_cast<off_t>(off));
-    if (got <= 0) {
-      return false;
-    }
-    dst += got;
-    size -= static_cast<uint64_t>(got);
-    off += static_cast<uint64_t>(got);
-  }
-  return true;
-}
-
-// the two pinned staging buffers of kmp_read_metis and the events of the copies out of them
-struct MetisStaging {
-  cudaStream_t st = nullptr;
-  uint8_t *buf[2] = {nullptr, nullptr};
-  cudaEvent_t ev[2] = {nullptr, nullptr};
-  ~MetisStaging() {
-    if (st != nullptr) {
-      cudaStreamSynchronize(st); // no copy reads a buffer any more
-    }
-    for (int b = 0; b < 2; ++b) {
-      if (buf[b] != nullptr) {
-        cudaFreeHost(buf[b]);
-      }
-      if (ev[b] != nullptr) {
-        cudaEventDestroy(ev[b]);
-      }
-    }
-  }
-};
-
-struct MetisFile {
-  int fd = -1;
-  ~MetisFile() {
-    if (fd >= 0) {
-      close(fd);
-    }
-  }
-};
-
-// Streams the file's `len` bytes into dst (device) on h's stream through the two pinned buffers of `stage` (the
-// caller's, so that they outlive the work it queues after), kMetisChunk bytes each: reading one chunk overlaps the copy
-// of the previous one. Starts h's call clock. queued(end) runs once the copy of bytes [0, end) is queued, to launch the
-// work on them; its error ends the stream.
-template <typename Queued>
-int stream_file(kmp_lp_handle *h, MetisStaging &stage, int fd, const char *path, uint64_t len, uint8_t *dst,
-                Queued &&queued) {
-  const cudaStream_t st = h->stream;
-  stage.st = st;
-  const uint64_t chunk = std::min<uint64_t>(len, kMetisChunk);
-  for (int b = 0; b < 2; ++b) {
-    KMP_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&stage.buf[b]), chunk, cudaHostAllocDefault));
-    KMP_CUDA(cudaEventCreateWithFlags(&stage.ev[b], cudaEventDisableTiming));
-  }
-  KMP_CUDA(call_clock_start(h, st));
-  for (uint64_t off = 0, idx = 0; off < len; off += chunk, ++idx) {
-    const int b = static_cast<int>(idx & 1u);
-    const uint64_t size = std::min<uint64_t>(chunk, len - off);
-    if (idx >= 2) {
-      KMP_CUDA(cudaEventSynchronize(stage.ev[b])); // the copy of chunk idx - 2 is out of this buffer
-    }
-    if (!metis_pread(fd, stage.buf[b], size, off)) {
-      return fail(KMP_ERR_INVALID, std::string("cannot read ") + path);
-    }
-    KMP_CUDA(cudaMemcpyAsync(dst + off, stage.buf[b], size, cudaMemcpyHostToDevice, st));
-    KMP_CUDA(cudaEventRecord(stage.ev[b], st));
-    const int rc = queued(off + size);
-    if (rc != KMP_OK) {
-      return rc;
-    }
-  }
-  return KMP_OK;
-}
-
 // The header from the file's first bytes, fetched by fetch(dst, size) in growing prefixes until metis_header has what
 // it needs; KMP_OK with hd filled, a refusal with r filled, or fetch's error.
 template <typename Fetch> int metis_read_header(uint64_t len, MetisHeader &hd, kmp_metis_report &r, Fetch &&fetch) {
@@ -777,39 +679,33 @@ template <typename Fetch> int metis_read_header(uint64_t len, MetisHeader &hd, k
 }
 
 int read_metis_impl(kmp_lp_handle *h, const char *path, kmp_metis_graph **out, kmp_metis_report &r) {
-  MetisFile f;
-  f.fd = open(path, O_RDONLY);
-  struct stat info {};
-  if (f.fd < 0 || fstat(f.fd, &info) != 0) {
-    return fail(KMP_ERR_INVALID, std::string("cannot open ") + path);
-  }
-  const uint64_t len = static_cast<uint64_t>(info.st_size);
+  InputFile f;
+  int rc = f.open(path);
+  const uint64_t len = f.len;
   r.bytes = len;
+  if (rc != KMP_OK) {
+    return rc;
+  }
   if (len == 0) {
     metis_refuse(r, KMP_METIS_EMPTY, 0, 1, -1);
     return metis_fail(r);
   }
-  if (len >= (1ull << 56)) {
-    return fail(KMP_ERR_UNSUPPORTED, "files of 2^56 bytes or more are not supported");
-  }
   MetisHeader hd;
-  int rc = metis_read_header(len, hd, r, [&](uint8_t *dst, uint64_t size) -> int {
-    return metis_pread(f.fd, dst, size, 0) ? KMP_OK : fail(KMP_ERR_INVALID, std::string("cannot read ") + path);
-  });
+  rc = metis_read_header(len, hd, r, [&](uint8_t *dst, uint64_t size) { return f.read(dst, size, 0); });
   if (rc != KMP_OK) {
     return rc;
   }
+  PoolBuf<uint8_t> bytes; // released stream-ordered when the read ends
   return make_result(h, out, [&](kmp_metis_graph *g) {
-    const cudaStream_t st = h->stream;
     MetisJob job{h};
-    KMP_CUDA(g->bytes.alloc(len, st, h->device));
-    rc = job.prepare(hd, g->bytes.p, len, g);
+    KMP_CUDA(bytes.alloc(len, h->stream, h->device));
+    rc = job.prepare(hd, bytes.p, len, g);
     if (rc != KMP_OK) {
       return rc;
     }
-    MetisStaging stage;
+    FileStaging stage;
     uint32_t done = 0; // tiles summarised
-    rc = stream_file(h, stage, f.fd, path, len, g->bytes.p, [&](uint64_t end) {
+    rc = stream_file(h, stage, f, bytes.p, [&](uint64_t end) {
       // tiles whose bytes (and the byte before them) are all on the device
       const uint32_t ready = end == len ? job.tiles : static_cast<uint32_t>(end / KMP_METIS_TILE_BYTES);
       const int src = job.summarise(done, ready);
@@ -820,7 +716,6 @@ int read_metis_impl(kmp_lp_handle *h, const char *path, kmp_metis_graph **out, k
       return rc;
     }
     rc = job.finish(g, r);
-    g->bytes.release();
     return rc != KMP_OK && r.kind != KMP_METIS_OK ? metis_fail(r) : rc;
   });
 }
@@ -833,11 +728,8 @@ int parse_metis_impl(kmp_lp_handle *h, const uint8_t *d_bytes, uint64_t len, kmp
     return metis_fail(r);
   }
   MetisHeader hd;
-  const int hrc = metis_read_header(len, hd, r, [&](uint8_t *dst, uint64_t size) -> int {
-    KMP_CUDA(cudaMemcpyAsync(dst, d_bytes, size, cudaMemcpyDeviceToHost, h->stream));
-    KMP_CUDA(cudaStreamSynchronize(h->stream));
-    return KMP_OK;
-  });
+  const int hrc = metis_read_header(len, hd, r,
+                                    [&](uint8_t *dst, uint64_t size) { return fetch_device_prefix(h, dst, d_bytes, size); });
   if (hrc != KMP_OK) {
     return hrc;
   }
@@ -864,6 +756,10 @@ const char *const kMetisKindNames[KMP_METIS_NUM_KINDS] = {
     "bad byte",    "missing node weight", "missing edge weight", "zero weight",          "weight too large",
     "neighbor out of range", "self-loop", "too few lines",       "wrong edge count",     "total weight too large"};
 
+int metis_begin(kmp_lp_handle *h, kmp_metis_graph **out, kmp_metis_report *report) {
+  return reader_begin(h, out, report, [](kmp_metis_report &) {}, [] { return KMP_OK; });
+}
+
 } // namespace
 
 extern "C" {
@@ -879,29 +775,10 @@ int kmp_read_metis(kmp_lp_handle *h, const char *path, kmp_metis_graph **out, km
 int kmp_parse_metis_device(kmp_lp_handle *h, const void *d_bytes, uint64_t len, kmp_metis_graph **out,
                            kmp_metis_report *report) {
   int rc = metis_begin(h, out, report);
-  if (rc != KMP_OK) {
-    return rc;
+  if (rc == KMP_OK) {
+    rc = check_device_bytes(h, d_bytes, len);
   }
-  if (d_bytes == nullptr && len > 0) {
-    return fail(KMP_ERR_INVALID, "null argument");
-  }
-  if ((reinterpret_cast<uintptr_t>(d_bytes) & 15u) != 0) {
-    return fail(KMP_ERR_INVALID, "the device bytes must be 16-byte aligned");
-  }
-  if (len >= (1ull << 56)) {
-    return fail(KMP_ERR_UNSUPPORTED, "inputs of 2^56 bytes or more are not supported");
-  }
-  if (len > 0) { // host memory or another device's memory would reach the kernels as a raw pointer
-    cudaPointerAttributes attr{};
-    const bool on_device = cudaPointerGetAttributes(&attr, d_bytes) == cudaSuccess &&
-                           (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged) &&
-                           attr.device == h->device;
-    cudaGetLastError(); // an unregistered host pointer leaves no sticky error
-    if (!on_device) {
-      return fail(KMP_ERR_INVALID, "the bytes must be device memory on the handle's device");
-    }
-  }
-  return parse_metis_impl(h, static_cast<const uint8_t *>(d_bytes), len, out, *report);
+  return rc != KMP_OK ? rc : parse_metis_impl(h, static_cast<const uint8_t *>(d_bytes), len, out, *report);
 }
 
 uint32_t kmp_metis_n(const kmp_metis_graph *g) { return g != nullptr ? g->n : 0; }
@@ -912,10 +789,7 @@ int kmp_metis_device_arrays(const kmp_metis_graph *g, const uint32_t **d_xadj, c
   if (g == nullptr) {
     return fail(KMP_ERR_INVALID, "null argument");
   }
-  hand_out(d_xadj, g->xadj);
-  hand_out(d_adjncy, g->adjncy);
-  hand_out(d_vwgt, g->vwgt);
-  hand_out(d_adjwgt, g->adjwgt);
+  hand_out_csr(*g, d_xadj, d_adjncy, d_vwgt, d_adjwgt);
   return KMP_OK;
 }
 
@@ -923,35 +797,19 @@ int kmp_metis_download(const kmp_metis_graph *g, uint32_t *xadj, uint32_t *adjnc
   if (g == nullptr) {
     return fail(KMP_ERR_INVALID, "null argument");
   }
-  KMP_CUDA(cudaSetDevice(g->device));
-  KMP_CUDA(copy_out(xadj, g->xadj, static_cast<size_t>(g->n) + 1));
-  KMP_CUDA(copy_out(adjncy, g->adjncy, g->m));
-  KMP_CUDA(copy_out(vwgt, g->vwgt, g->n));
-  KMP_CUDA(copy_out(adjwgt, g->adjwgt, g->m));
-  return KMP_OK;
+  return download_csr(*g, xadj, adjncy, vwgt, adjwgt, static_cast<size_t>(g->n) + 1, g->n, g->m);
 }
 
-void kmp_metis_destroy(kmp_metis_graph *g) {
-  if (g == nullptr) {
-    return;
-  }
-  cudaSetDevice(g->device); // the arrays free themselves on this device's pool
-  delete g;
-}
+void kmp_metis_destroy(kmp_metis_graph *g) { destroy_result(g); }
 
 int kmp_metis_report_message(const kmp_metis_report *r, char *buf, size_t size) {
   if (r == nullptr) {
     return fail(KMP_ERR_INVALID, "null argument");
   }
-  char dummy = 0;
-  if (buf == nullptr || size == 0) {
-    buf = &dummy;
-    size = 1;
-  }
   if (r->kind <= KMP_METIS_OK || r->kind >= KMP_METIS_NUM_KINDS) {
-    return std::snprintf(buf, size, "%s", r->extra_lines ? "ignorning extra lines in input file" : ""); // :151
+    return format_report(buf, size, "%s", r->extra_lines ? "ignorning extra lines in input file" : ""); // :151
   }
-  return std::snprintf(buf, size, "%s at byte %llu (line %llu, vertex %lld)", kMetisKindNames[r->kind],
+  return format_report(buf, size, "%s at byte %llu (line %llu, vertex %lld)", kMetisKindNames[r->kind],
                        static_cast<unsigned long long>(r->offset), static_cast<unsigned long long>(r->line),
                        static_cast<long long>(r->vertex));
 }

@@ -1,7 +1,7 @@
 // kaminpar_b200: the ParHIP reader on the device + its C ABI (include/kaminpar_b200_parhip.h, DESIGN.md §19).
 // Included at the end of kmp_lp.cu after kmp_prepare.cuh and kmp_metis.cuh: the EXTERNAL ordering reuses the
 // preparation's tile histogram and stable scatter (k_prep_count, k_prep_scatter) and the contraction's tile owners
-// (k_tile_owners, owner_of_edge); kmp_read_parhip streams the file with the METIS reader's stream_file.
+// (k_tile_owners, owner_of_edge); kmp_read_parhip streams the file with kmp_read.cuh's stream_file.
 //
 // What it restates (see the header): csr_read and csr_read_deg_buckets (parhip_parser.cc:179-336).
 //   The 24-byte header is read on the host, which lays out the sections and refuses n or m >= 2^31.
@@ -21,12 +21,10 @@
 
 #include "../../include/kaminpar_b200_parhip.h"
 
-struct kmp_parhip_graph {
-  int device = 0;
+struct kmp_parhip_graph : DeviceCsr { // vwgt / adjwgt: unallocated for absent weights
   uint32_t n = 0, m = 0;
   int sorted = 0;
-  PoolBuf<uint32_t> xadj, adjncy, old_to_new; // old_to_new: EXTERNAL only
-  PoolBuf<int32_t> vwgt, adjwgt;              // unallocated for absent weights
+  PoolBuf<uint32_t> old_to_new; // EXTERNAL only
 };
 
 namespace {
@@ -548,27 +546,20 @@ int ParhipJob::finish(kmp_parhip_report &r, kmp_prepared_graph *pg) {
 }
 
 int parhip_begin(kmp_lp_handle *h, int ordering, bool prepared, void *out, kmp_parhip_report *report) {
-  if (h == nullptr || out == nullptr || report == nullptr) {
-    return fail(KMP_ERR_INVALID, "null argument");
-  }
-  std::memset(report, 0, sizeof(*report));
-  report->ordering = ordering;
-  if (h->step.open) {
-    return fail(KMP_ERR_INVALID, "the handle is inside a stepping call");
-  }
-  if ((ordering & KMP_PARHIP_COMPRESS) != 0 && (ordering & ~KMP_PARHIP_COMPRESS) >= 0 &&
-      (ordering & ~KMP_PARHIP_COMPRESS) <= KMP_PARHIP_IMPLICIT_DEGREE_BUCKETS) {
-    return fail(KMP_ERR_UNSUPPORTED, "the compressed ParHIP read is not supported");
-  }
-  if (ordering < KMP_PARHIP_NATURAL || ordering > KMP_PARHIP_IMPLICIT_DEGREE_BUCKETS) {
-    return fail(KMP_ERR_INVALID, "unknown node ordering");
-  }
-  if (prepared && ordering != KMP_PARHIP_EXTERNAL_DEGREE_BUCKETS) {
-    return fail(KMP_ERR_INVALID, "a prepared read takes the external degree-bucket ordering");
-  }
-  report->sorted = ordering == KMP_PARHIP_IMPLICIT_DEGREE_BUCKETS || ordering == KMP_PARHIP_EXTERNAL_DEGREE_BUCKETS;
-  KMP_CUDA(cudaSetDevice(h->device));
-  return KMP_OK;
+  return reader_begin(h, out, report, [&](kmp_parhip_report &r) { r.ordering = ordering; }, [&]() -> int {
+    if ((ordering & KMP_PARHIP_COMPRESS) != 0 && (ordering & ~KMP_PARHIP_COMPRESS) >= 0 &&
+        (ordering & ~KMP_PARHIP_COMPRESS) <= KMP_PARHIP_IMPLICIT_DEGREE_BUCKETS) {
+      return fail(KMP_ERR_UNSUPPORTED, "the compressed ParHIP read is not supported");
+    }
+    if (ordering < KMP_PARHIP_NATURAL || ordering > KMP_PARHIP_IMPLICIT_DEGREE_BUCKETS) {
+      return fail(KMP_ERR_INVALID, "unknown node ordering");
+    }
+    if (prepared && ordering != KMP_PARHIP_EXTERNAL_DEGREE_BUCKETS) {
+      return fail(KMP_ERR_INVALID, "a prepared read takes the external degree-bucket ordering");
+    }
+    report->sorted = ordering == KMP_PARHIP_IMPLICIT_DEGREE_BUCKETS || ordering == KMP_PARHIP_EXTERNAL_DEGREE_BUCKETS;
+    return KMP_OK;
+  });
 }
 
 // The read of one file into g (NATURAL / IMPLICIT) or pg (EXTERNAL). head: the file's first min(len, 24) bytes;
@@ -595,10 +586,7 @@ int parhip_run(kmp_lp_handle *h, const uint8_t *head, uint64_t len, int ordering
     g->m = static_cast<uint32_t>(job.L.m);
     g->sorted = r.sorted;
     if (job.ext) { // the prepared arrays become the graph's; new_to_old is freed with pg
-      g->xadj = std::move(pg->xadj);
-      g->adjncy = std::move(pg->adjncy);
-      g->vwgt = std::move(pg->vwgt);
-      g->adjwgt = std::move(pg->adjwgt);
+      static_cast<DeviceCsr &>(*g) = std::move(*pg);
       g->old_to_new = std::move(pg->old_to_new);
     }
   }
@@ -607,29 +595,25 @@ int parhip_run(kmp_lp_handle *h, const uint8_t *head, uint64_t len, int ordering
 
 int read_parhip_impl(kmp_lp_handle *h, const char *path, int ordering, kmp_parhip_graph *g, kmp_prepared_graph *pg,
                      kmp_parhip_report &r) {
-  MetisFile f;
-  f.fd = open(path, O_RDONLY);
-  struct stat info {};
-  if (f.fd < 0 || fstat(f.fd, &info) != 0) {
-    return fail(KMP_ERR_INVALID, std::string("cannot open ") + path);
-  }
-  const uint64_t len = static_cast<uint64_t>(info.st_size);
-  if (len >= (1ull << 56)) {
-    return fail(KMP_ERR_UNSUPPORTED, "files of 2^56 bytes or more are not supported");
-  }
+  InputFile f;
+  int rc = f.open(path);
+  const uint64_t len = f.len;
   uint8_t head[24] = {};
-  if (!metis_pread(f.fd, head, std::min<uint64_t>(len, 24), 0)) {
-    return fail(KMP_ERR_INVALID, std::string("cannot read ") + path);
+  if (rc == KMP_OK) {
+    rc = f.read(head, std::min<uint64_t>(len, 24), 0);
+  }
+  if (rc != KMP_OK) {
+    return rc;
   }
   PoolBuf<uint8_t> bytes; // released stream-ordered when the read ends
-  MetisStaging stage;
+  FileStaging stage;
   return parhip_run(h, head, len, ordering, g, pg, r, [&](ParhipJob &job) {
     KMP_CUDA(bytes.alloc(len, h->stream, h->device));
     int rc = job.prepare(bytes.p, g, pg);
     if (rc != KMP_OK) {
       return rc;
     }
-    return stream_file(h, stage, f.fd, path, len, bytes.p, [&](uint64_t end) { return job.ready(end); });
+    return stream_file(h, stage, f, bytes.p, [&](uint64_t end) { return job.ready(end); });
   });
 }
 
@@ -637,8 +621,10 @@ int parse_parhip_impl(kmp_lp_handle *h, const uint8_t *d_bytes, uint64_t len, in
                       kmp_prepared_graph *pg, kmp_parhip_report &r) {
   uint8_t head[24] = {};
   if (len > 0) {
-    KMP_CUDA(cudaMemcpyAsync(head, d_bytes, std::min<uint64_t>(len, 24), cudaMemcpyDeviceToHost, h->stream));
-    KMP_CUDA(cudaStreamSynchronize(h->stream));
+    const int rc = fetch_device_prefix(h, head, d_bytes, std::min<uint64_t>(len, 24));
+    if (rc != KMP_OK) {
+      return rc;
+    }
   }
   return parhip_run(h, head, len, ordering, g, pg, r, [&](ParhipJob &job) {
     int rc = job.prepare(d_bytes, g, pg);
@@ -648,29 +634,6 @@ int parse_parhip_impl(kmp_lp_handle *h, const uint8_t *d_bytes, uint64_t len, in
     KMP_CUDA(call_clock_start(h, h->stream));
     return job.ready(len);
   });
-}
-
-int parhip_check_device_bytes(const kmp_lp_handle *h, const void *d_bytes, uint64_t len) {
-  if (d_bytes == nullptr && len > 0) {
-    return fail(KMP_ERR_INVALID, "null argument");
-  }
-  if ((reinterpret_cast<uintptr_t>(d_bytes) & 15u) != 0) {
-    return fail(KMP_ERR_INVALID, "the device bytes must be 16-byte aligned");
-  }
-  if (len >= (1ull << 56)) {
-    return fail(KMP_ERR_UNSUPPORTED, "inputs of 2^56 bytes or more are not supported");
-  }
-  if (len > 0) { // host memory or another device's memory would reach the kernels as a raw pointer
-    cudaPointerAttributes attr{};
-    const bool on_device = cudaPointerGetAttributes(&attr, d_bytes) == cudaSuccess &&
-                           (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged) &&
-                           attr.device == h->device;
-    cudaGetLastError(); // an unregistered host pointer leaves no sticky error
-    if (!on_device) {
-      return fail(KMP_ERR_INVALID, "the bytes must be device memory on the handle's device");
-    }
-  }
-  return KMP_OK;
 }
 
 // the graph result of either entry point: EXTERNAL goes through a prepared graph whose arrays it takes over
@@ -704,7 +667,7 @@ int kmp_parse_parhip_device(kmp_lp_handle *h, const void *d_bytes, uint64_t len,
                             kmp_parhip_graph **out, kmp_parhip_report *report) {
   int rc = parhip_begin(h, ordering, false, out, report);
   if (rc == KMP_OK) {
-    rc = parhip_check_device_bytes(h, d_bytes, len);
+    rc = check_device_bytes(h, d_bytes, len);
   }
   if (rc != KMP_OK) {
     return rc;
@@ -732,7 +695,7 @@ int kmp_parse_parhip_device_prepared(kmp_lp_handle *h, const void *d_bytes, uint
                                      kmp_parhip_report *report) {
   int rc = parhip_begin(h, KMP_PARHIP_EXTERNAL_DEGREE_BUCKETS, true, out, report);
   if (rc == KMP_OK) {
-    rc = parhip_check_device_bytes(h, d_bytes, len);
+    rc = check_device_bytes(h, d_bytes, len);
   }
   if (rc != KMP_OK) {
     return rc;
@@ -752,10 +715,7 @@ int kmp_parhip_device_arrays(const kmp_parhip_graph *g, const uint32_t **d_xadj,
   if (g == nullptr) {
     return fail(KMP_ERR_INVALID, "null argument");
   }
-  hand_out(d_xadj, g->xadj);
-  hand_out(d_adjncy, g->adjncy);
-  hand_out(d_vwgt, g->vwgt);
-  hand_out(d_adjwgt, g->adjwgt);
+  hand_out_csr(*g, d_xadj, d_adjncy, d_vwgt, d_adjwgt);
   hand_out(d_old_to_new, g->old_to_new);
   return KMP_OK;
 }
@@ -765,59 +725,25 @@ int kmp_parhip_download(const kmp_parhip_graph *g, uint32_t *xadj, uint32_t *adj
   if (g == nullptr) {
     return fail(KMP_ERR_INVALID, "null argument");
   }
-  KMP_CUDA(cudaSetDevice(g->device));
-  KMP_CUDA(copy_out(xadj, g->xadj, static_cast<size_t>(g->n) + 1));
-  KMP_CUDA(copy_out(adjncy, g->adjncy, g->m));
-  KMP_CUDA(copy_out(vwgt, g->vwgt, g->n));
-  KMP_CUDA(copy_out(adjwgt, g->adjwgt, g->m));
+  const int rc = download_csr(*g, xadj, adjncy, vwgt, adjwgt, static_cast<size_t>(g->n) + 1, g->n, g->m);
+  if (rc != KMP_OK) {
+    return rc;
+  }
   KMP_CUDA(copy_out(old_to_new, g->old_to_new, g->n));
   return KMP_OK;
 }
 
-void kmp_parhip_destroy(kmp_parhip_graph *g) {
-  if (g == nullptr) {
-    return;
-  }
-  cudaSetDevice(g->device); // the arrays free themselves on this device's pool
-  delete g;
-}
-
-int kmp_pool_usage(kmp_lp_handle *h, int reset, uint64_t *used, uint64_t *used_high) {
-  if (h == nullptr || used == nullptr || used_high == nullptr) {
-    return fail(KMP_ERR_INVALID, "null argument");
-  }
-  KMP_CUDA(cudaSetDevice(h->device));
-  cudaMemPool_t pool = kmp_private_pool(h->device);
-  if (pool == nullptr) {
-    return fail(KMP_ERR_CUDA, "no device memory pool");
-  }
-  KMP_CUDA(cudaStreamSynchronize(h->stream)); // the stream-ordered frees of h's calls have happened
-  uint64_t cur = 0, high = 0;
-  KMP_CUDA(cudaMemPoolGetAttribute(pool, cudaMemPoolAttrUsedMemCurrent, &cur));
-  KMP_CUDA(cudaMemPoolGetAttribute(pool, cudaMemPoolAttrUsedMemHigh, &high));
-  *used = cur;
-  *used_high = high;
-  if (reset != 0) {
-    uint64_t zero = 0; // the only value the attribute accepts: the mark restarts at the current use
-    KMP_CUDA(cudaMemPoolSetAttribute(pool, cudaMemPoolAttrUsedMemHigh, &zero));
-  }
-  return KMP_OK;
-}
+void kmp_parhip_destroy(kmp_parhip_graph *g) { destroy_result(g); }
 
 int kmp_parhip_report_message(const kmp_parhip_report *r, char *buf, size_t size) {
   if (r == nullptr) {
     return fail(KMP_ERR_INVALID, "null argument");
   }
-  char dummy = 0;
-  if (buf == nullptr || size == 0) {
-    buf = &dummy;
-    size = 1;
-  }
   if (r->kind <= KMP_PARHIP_OK || r->kind >= KMP_PARHIP_NUM_KINDS) {
-    return std::snprintf(buf, size, "%s", "");
+    return format_report(buf, size, "%s", "");
   }
   const int s = r->section >= 0 && r->section <= KMP_PARHIP_SECTION_ADJWGT ? r->section : 0;
-  return std::snprintf(buf, size, "%s at byte %llu (%s entry %lld)", kParhipKindNames[r->kind],
+  return format_report(buf, size, "%s at byte %llu (%s entry %lld)", kParhipKindNames[r->kind],
                        static_cast<unsigned long long>(r->offset), kParhipSectionNames[s],
                        static_cast<long long>(r->index));
 }

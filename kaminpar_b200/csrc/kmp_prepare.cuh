@@ -266,11 +266,9 @@ __global__ void k_prep_map_back(uint32_t n, uint32_t np, uint32_t k, const uint3
 
 } // namespace
 
-struct kmp_prepared_graph {
-  int device = 0;
+struct kmp_prepared_graph : DeviceCsr {
   uint32_t n = 0, np = 0, m = 0;
-  PoolBuf<uint32_t> xadj, adjncy, old_to_new, new_to_old;
-  PoolBuf<int32_t> vwgt, adjwgt; // unallocated for unit weights
+  PoolBuf<uint32_t> old_to_new, new_to_old;
 };
 
 namespace {
@@ -489,10 +487,7 @@ int kmp_prepared_device_arrays(const kmp_prepared_graph *g, const uint32_t **d_x
   if (g == nullptr) {
     return fail(KMP_ERR_INVALID, "null argument");
   }
-  hand_out(d_xadj, g->xadj);
-  hand_out(d_adjncy, g->adjncy);
-  hand_out(d_vwgt, g->vwgt);
-  hand_out(d_adjwgt, g->adjwgt);
+  hand_out_csr(*g, d_xadj, d_adjncy, d_vwgt, d_adjwgt);
   hand_out(d_old_to_new, g->old_to_new);
   hand_out(d_new_to_old, g->new_to_old);
   return KMP_OK;
@@ -503,11 +498,10 @@ int kmp_prepared_download(const kmp_prepared_graph *g, uint32_t *xadj, uint32_t 
   if (g == nullptr) {
     return fail(KMP_ERR_INVALID, "null argument");
   }
-  KMP_CUDA(cudaSetDevice(g->device));
-  KMP_CUDA(copy_out(xadj, g->xadj, static_cast<size_t>(g->n) + 1));
-  KMP_CUDA(copy_out(adjncy, g->adjncy, g->m));
-  KMP_CUDA(copy_out(vwgt, g->vwgt, g->n));
-  KMP_CUDA(copy_out(adjwgt, g->adjwgt, g->m));
+  const int rc = download_csr(*g, xadj, adjncy, vwgt, adjwgt, static_cast<size_t>(g->n) + 1, g->n, g->m);
+  if (rc != KMP_OK) {
+    return rc;
+  }
   KMP_CUDA(copy_out(old_to_new, g->old_to_new, g->n));
   return KMP_OK;
 }
@@ -550,12 +544,6 @@ int kmp_prepared_finish(kmp_lp_handle *h, const kmp_prepared_graph *g, uint32_t 
   return finish_impl(h, g, k, max_block_weights, partition, partition_out, block_weights_out);
 }
 
-void kmp_prepared_destroy(kmp_prepared_graph *g) {
-  if (g == nullptr) {
-    return;
-  }
-  cudaSetDevice(g->device); // the arrays free themselves on this device's pool
-  delete g;
-}
+void kmp_prepared_destroy(kmp_prepared_graph *g) { destroy_result(g); }
 
 } // extern "C"

@@ -609,12 +609,6 @@ int kmp_subgraphs_copy_partitions_device(kmp_lp_handle *h, const kmp_subgraphs *
   return copy_back_checked(h, g, k_prime, input_k, d_sub_partitions, false, partition_out, block_weights_out);
 }
 
-void kmp_subgraphs_destroy(kmp_subgraphs *g) {
-  if (g == nullptr) {
-    return;
-  }
-  cudaSetDevice(g->device); // the arrays free themselves on this device's pool
-  delete g;
-}
+void kmp_subgraphs_destroy(kmp_subgraphs *g) { destroy_result(g); }
 
 } // extern "C"

@@ -368,33 +368,27 @@ int kmp_graph_report_message(const kmp_graph_report *r, char *buf, size_t size) 
   if (r == nullptr) {
     return fail(KMP_ERR_INVALID, "null argument");
   }
-  char dummy = 0;
-  if (buf == nullptr || size == 0) {
-    buf = &dummy;
-    size = 1;
-  }
   switch (r->kind) { // csr_graph.cc:276-350, word for word
   case KMP_GRAPH_XADJ_START:
-    return std::snprintf(buf, size, "xadj[0] is %u, not 0", r->e);
+    return format_report(buf, size, "xadj[0] is %u, not 0", r->e);
   case KMP_GRAPH_XADJ_END:
-    return std::snprintf(buf, size, "xadj[%u] is %u, not the number of edges %u", r->u, r->e, r->m);
+    return format_report(buf, size, "xadj[%u] is %u, not the number of edges %u", r->u, r->e, r->m);
   case KMP_GRAPH_XADJ_DECREASING:
-    return std::snprintf(buf, size, "Bad node array at position %u", r->u);
+    return format_report(buf, size, "Bad node array at position %u", r->u);
   case KMP_GRAPH_NEIGHBOR_OUT_OF_GRAPH:
-    return std::snprintf(buf, size, "Neighbor %u of %u is out-of-graph", r->v, r->u);
+    return format_report(buf, size, "Neighbor %u of %u is out-of-graph", r->v, r->u);
   case KMP_GRAPH_SELF_LOOP:
-    return std::snprintf(buf, size, "Self-loop at %u: %u --> %u", r->u, r->e, r->v);
+    return format_report(buf, size, "Self-loop at %u: %u --> %u", r->u, r->e, r->v);
   case KMP_GRAPH_NEIGHBOR_OF_NEIGHBOR_OUT_OF_GRAPH:
-    return std::snprintf(buf, size, "Neighbor %u of neighbor %u of %u is out-of-graph", r->v_rev, r->v, r->u);
+    return format_report(buf, size, "Neighbor %u of neighbor %u of %u is out-of-graph", r->v_rev, r->v, r->u);
   case KMP_GRAPH_MISSING_REVERSE:
-    return std::snprintf(buf, size, "Edge %u --> %u exists with edge %u, but the reverse edges does not exist", r->u,
+    return format_report(buf, size, "Edge %u --> %u exists with edge %u, but the reverse edges does not exist", r->u,
                          r->v, r->e);
   case KMP_GRAPH_WEIGHT_MISMATCH:
-    return std::snprintf(buf, size, "Weight of edge %u (%d) differs from the weight of its reverse edge %u (%d)", r->e,
+    return format_report(buf, size, "Weight of edge %u (%d) differs from the weight of its reverse edge %u (%d)", r->e,
                          r->w, r->e_rev, r->w_rev);
   default:
-    buf[0] = '\0';
-    return 0;
+    return format_report(buf, size, "%s", "");
   }
 }
 

@@ -142,15 +142,20 @@ def load_library():
         lib = C.CDLL(_LIB_PATH)
         lib.kmp_last_error.restype = C.c_char_p
         lib.kmp_lp_labels_device.restype = C.c_void_p
-        for sym in ("kmp_overload_balance", "kmp_balance_select_all",  # include/kaminpar_b200_balancer.h
-                    "kmp_underload_balance", "kmp_underload_select_all",
-                    "kmp_lp_cluster_overlay", "kmp_overlay_clusterings"):  # include/kaminpar_b200_contraction.h
-            if not hasattr(lib, sym):
-                raise RuntimeError(f"{_LIB_PATH} lacks {sym}; rebuild the library")
+        require_symbols(lib, "kmp_overload_balance", "kmp_balance_select_all",  # include/kaminpar_b200_balancer.h
+                        "kmp_underload_balance", "kmp_underload_select_all",
+                        "kmp_lp_cluster_overlay", "kmp_overlay_clusterings")  # include/kaminpar_b200_contraction.h
         if lib.kmp_lp_abi_version() != ABI_VERSION:  # the ctypes structs below mirror exactly this header version
             raise RuntimeError(f"{_LIB_PATH}: ABI version {lib.kmp_lp_abi_version()} != {ABI_VERSION}; rebuild the library")
         _lib = lib
     return _lib
+
+
+def require_symbols(lib, *symbols):
+    """Refuses a library built before one of `symbols` existed."""
+    for sym in symbols:
+        if not hasattr(lib, sym):
+            raise RuntimeError(f"{_LIB_PATH} lacks {sym}; rebuild the library")
 
 
 def _check(rc: int):
@@ -161,6 +166,44 @@ def _check(rc: int):
 
 def _ptr(a: Optional[np.ndarray]):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
+
+
+def report_message(fn, report) -> str:
+    """The message the C function `fn` (a kmp_*_report_message) formats for `report`."""
+    size = fn(C.byref(report), None, 0)
+    buf = C.create_string_buffer(size + 1)
+    fn(C.byref(report), buf, size + 1)
+    return buf.value.decode()
+
+
+class ReportError(RuntimeError):
+    """An input refused with a report; `report` holds its first violation, `code` the library's error code."""
+
+    def __init__(self, code: int, report):
+        super().__init__(f"kaminpar_b200 error {code}: {report.message()}")
+        self.code = code
+        self.report = report
+
+
+def check_report(rc: int, report, error):
+    """_check, except that a call refused with a violation in `report` raises error(rc, report)."""
+    if rc != 0 and report.kind != 0:
+        raise error(rc, report)
+    _check(rc)
+
+
+def device_bytes(tensor):
+    """(pointer, length) of the bytes of a contiguous torch CUDA tensor, for a reader that parses them on the
+    device. The library reads them on its handle's stream, so the work torch has queued on its current stream is
+    waited for first: a tensor just written by a kernel is read whole."""
+    import torch
+
+    if tensor.dtype.itemsize != 1 or not tensor.is_contiguous():
+        raise ValueError("a device read needs a contiguous tensor of bytes")
+    if not tensor.is_cuda:  # the library refuses device memory of another device than the handle's
+        raise ValueError("a device read needs a CUDA tensor")
+    torch.cuda.current_stream(tensor.device).synchronize()
+    return C.c_void_p(tensor.data_ptr() or None), C.c_uint64(tensor.numel())
 
 
 # --------------------------------------------------------------------------------------------
@@ -563,6 +606,14 @@ class LPHandle:
         _check(self._lib.kmp_lp_free_scratch(self._h))
 
 
+def pool_usage(handle: LPHandle, reset: bool = False):
+    """(bytes in use, most bytes in use since the last reset) of the device pool the handle and its results allocate
+    from; reset restarts the high-water mark at the current use."""
+    used, high = C.c_uint64(), C.c_uint64()
+    _check(load_library().kmp_pool_usage(handle._h, C.c_int(int(reset)), C.byref(used), C.byref(high)))
+    return int(used.value), int(high.value)
+
+
 class DeviceResult:
     """A result object of a graph operation on an LPHandle (a coarse graph, a prepared graph, extracted subgraphs).
     It owns device memory of the handle's pool, freed on the handle's stream when it closes, so the handle stays open
@@ -581,6 +632,17 @@ class DeviceResult:
         ptrs = [C.c_void_p() for _ in range(count)]
         _check(getattr(load_library(), symbol)(self._g, *[C.byref(p) for p in ptrs]))
         return tuple(int(p.value or 0) for p in ptrs)
+
+    def _download_csr(self, symbol: str, n: int, m: int, vwgt: bool, adjwgt: bool, *extra):
+        """(xadj, adjncy, vwgt, adjwgt) of n vertices and m edges copied to the host by `symbol`, the weights None
+        unless present; `extra` are the host arrays (or None) that `symbol` fills after adjwgt."""
+        xadj = np.zeros(n + 1, np.uint32)
+        adj = np.zeros(m, np.uint32)
+        vw = np.zeros(n, np.int32) if vwgt else None
+        ew = np.zeros(m, np.int32) if adjwgt else None
+        _check(getattr(load_library(), symbol)(self._g, _ptr(xadj), _ptr(adj), _ptr(vw), _ptr(ew),
+                                               *[_ptr(a) for a in extra]))
+        return xadj, adj, vw, ew
 
     def close(self):
         if getattr(self, "_g", None):

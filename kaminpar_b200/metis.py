@@ -15,8 +15,6 @@ from __future__ import annotations
 
 import ctypes as C
 
-import numpy as np
-
 from . import lp
 from .graph import CSRGraph
 
@@ -55,32 +53,22 @@ class MetisReport(C.Structure):
     def message(self) -> str:
         """'<kind> at byte <offset> (line <line>, vertex <vertex>)' for a refusal; for a graph the reference's
         warning line when extra lines were ignored, else ''."""
-        lib = _lib()
-        size = lib.kmp_metis_report_message(C.byref(self), None, 0)
-        buf = C.create_string_buffer(size + 1)
-        lib.kmp_metis_report_message(C.byref(self), buf, size + 1)
-        return buf.value.decode()
+        return lp.report_message(_lib().kmp_metis_report_message, self)
 
     def __repr__(self) -> str:
         return (f"MetisReport({self.kind_name}, offset={self.offset}, line={self.line}, vertex={self.vertex}, "
                 f"n={self.n}, m={self.m}, bytes={self.bytes})")
 
 
-class MetisError(RuntimeError):
-    """A refused METIS input; `report` holds its first violation, `code` the library's error code."""
-
-    def __init__(self, code: int, report: MetisReport):
-        super().__init__(f"kaminpar_b200 error {code}: {report.message()}")
-        self.code = code
-        self.report = report
+class MetisError(lp.ReportError):
+    """A refused METIS input; `report` (a MetisReport) holds its first violation, `code` the library's error code."""
 
 
 def _lib():
     lib = lp.load_library()
     if not getattr(lib, "_metis_ready", False):
-        for sym in ("kmp_read_metis", "kmp_parse_metis_device", "kmp_metis_download", "kmp_metis_report_message"):
-            if not hasattr(lib, sym):
-                raise RuntimeError(f"{lp.library_path()} lacks {sym}; rebuild the library")
+        lp.require_symbols(lib, "kmp_read_metis", "kmp_parse_metis_device", "kmp_metis_download",
+                           "kmp_metis_report_message")
         for sym in ("kmp_metis_n", "kmp_metis_m"):
             getattr(lib, sym).restype = C.c_uint32
             getattr(lib, sym).argtypes = [C.c_void_p]
@@ -118,12 +106,8 @@ class MetisGraph(lp.DeviceResult):
     def get(self) -> CSRGraph:
         """The graph, copied to the host."""
         if self._host is None:
-            n, m = self.n, self.m
-            xadj = np.zeros(n + 1, np.uint32)
-            adj = np.zeros(m, np.uint32)
-            vw = np.zeros(n, np.int32) if self._has_vwgt else None
-            ew = np.zeros(m, np.int32) if self._has_adjwgt else None
-            lp._check(_lib().kmp_metis_download(self._g, lp._ptr(xadj), lp._ptr(adj), lp._ptr(vw), lp._ptr(ew)))
+            xadj, adj, vw, ew = self._download_csr("kmp_metis_download", self.n, self.m, self._has_vwgt,
+                                                   self._has_adjwgt)
             self._host = CSRGraph(xadj=xadj, adjncy=adj, vwgt=vw, adjwgt=ew)
         return self._host
 
@@ -137,10 +121,7 @@ class MetisGraph(lp.DeviceResult):
 
 
 def _finish(rc: int, out, report: MetisReport, handle: lp.LPHandle) -> MetisGraph:
-    if rc != 0:
-        if report.kind != 0:
-            raise MetisError(rc, report)
-        lp._check(rc)
+    lp.check_report(rc, report, MetisError)
     return MetisGraph(out, report, handle)
 
 
@@ -153,13 +134,10 @@ def read_metis_device(handle: lp.LPHandle, path: str) -> MetisGraph:
 
 
 def parse_metis_device(handle: lp.LPHandle, tensor) -> MetisGraph:
-    """The same on the bytes of a contiguous torch uint8 CUDA tensor (16-byte aligned) on the handle's device."""
-    if tensor.dtype.itemsize != 1 or not tensor.is_contiguous():
-        raise ValueError("parse_metis_device needs a contiguous tensor of bytes")
-    if not tensor.is_cuda:  # the library refuses device memory of another device than the handle's
-        raise ValueError("parse_metis_device needs a CUDA tensor")
+    """The same on the bytes of a contiguous torch uint8 CUDA tensor (16-byte aligned) on the handle's device. Work
+    queued on torch's current stream is waited for first, so a tensor just written by a kernel is read whole."""
+    ptr, size = lp.device_bytes(tensor)
     out = C.c_void_p()
     report = MetisReport()
-    rc = _lib().kmp_parse_metis_device(handle._h, C.c_void_p(tensor.data_ptr() or None), C.c_uint64(tensor.numel()),
-                                       C.byref(out), C.byref(report))
+    rc = _lib().kmp_parse_metis_device(handle._h, ptr, size, C.byref(out), C.byref(report))
     return _finish(rc, out, report, handle)

@@ -58,34 +58,22 @@ class ParhipReport(C.Structure):
 
     def message(self) -> str:
         """'<kind> at byte <offset> (<section> entry <index>)' for a refusal, '' for a graph."""
-        lib = _lib()
-        size = lib.kmp_parhip_report_message(C.byref(self), None, 0)
-        buf = C.create_string_buffer(size + 1)
-        lib.kmp_parhip_report_message(C.byref(self), buf, size + 1)
-        return buf.value.decode()
+        return lp.report_message(_lib().kmp_parhip_report_message, self)
 
     def __repr__(self) -> str:
         return (f"ParhipReport({self.kind_name}, offset={self.offset}, section={SECTIONS[self.section]}, "
                 f"index={self.index}, n={self.n}, m={self.m}, bytes={self.bytes})")
 
 
-class ParhipError(RuntimeError):
-    """A refused ParHIP input; `report` holds its first violation, `code` the library's error code."""
-
-    def __init__(self, code: int, report: ParhipReport):
-        super().__init__(f"kaminpar_b200 error {code}: {report.message()}")
-        self.code = code
-        self.report = report
+class ParhipError(lp.ReportError):
+    """A refused ParHIP input; `report` (a ParhipReport) holds its first violation, `code` the library's error code."""
 
 
 def _lib():
     lib = lp.load_library()
     if not getattr(lib, "_parhip_ready", False):
-        for sym in ("kmp_read_parhip", "kmp_parse_parhip_device", "kmp_read_parhip_prepared",
-                    "kmp_parse_parhip_device_prepared", "kmp_parhip_download", "kmp_parhip_report_message",
-                    "kmp_pool_usage"):
-            if not hasattr(lib, sym):
-                raise RuntimeError(f"{lp.library_path()} lacks {sym}; rebuild the library")
+        lp.require_symbols(lib, "kmp_read_parhip", "kmp_parse_parhip_device", "kmp_read_parhip_prepared",
+                           "kmp_parse_parhip_device_prepared", "kmp_parhip_download", "kmp_parhip_report_message")
         for sym in ("kmp_parhip_n", "kmp_parhip_m"):
             getattr(lib, sym).restype = C.c_uint32
             getattr(lib, sym).argtypes = [C.c_void_p]
@@ -98,7 +86,6 @@ def _lib():
         lib.kmp_parse_parhip_device_prepared.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]
         lib.kmp_parhip_download.argtypes = [C.c_void_p] * 6
         lib.kmp_parhip_report_message.argtypes = [C.c_void_p, C.c_char_p, C.c_size_t]
-        lib.kmp_pool_usage.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
         lib._parhip_ready = True
     return lib
 
@@ -131,14 +118,10 @@ class ParhipGraph(lp.DeviceResult):
 
     def _download(self):
         if self._host is None:
-            n, m = self.n, self.m
-            xadj = np.zeros(n + 1, np.uint32)
-            adj = np.zeros(m, np.uint32)
-            vw = np.zeros(n, np.int32) if self._has_vwgt else None
-            ew = np.zeros(m, np.int32) if self._has_adjwgt else None
+            n = self.n
             perm = np.zeros(n, np.uint32) if self._has_perm else None
-            lp._check(_lib().kmp_parhip_download(self._g, lp._ptr(xadj), lp._ptr(adj), lp._ptr(vw), lp._ptr(ew),
-                                                 lp._ptr(perm)))
+            xadj, adj, vw, ew = self._download_csr("kmp_parhip_download", n, self.m, self._has_vwgt,
+                                                   self._has_adjwgt, perm)
             self._host = (CSRGraph(xadj=xadj, adjncy=adj, vwgt=vw, adjwgt=ew, sorted=self.sorted), perm)
         return self._host
 
@@ -163,57 +146,28 @@ def _ordering(ordering) -> int:
     return ORDERINGS[ordering] if isinstance(ordering, str) else int(ordering)
 
 
-def _raise(rc: int, report: ParhipReport):
-    if report.kind != 0:
-        raise ParhipError(rc, report)
-    lp._check(rc)
-
-
-def _device_bytes(tensor):
-    import torch
-
-    if tensor.dtype.itemsize != 1 or not tensor.is_contiguous():
-        raise ValueError("the ParHIP reader needs a contiguous tensor of bytes")
-    if not tensor.is_cuda:  # the library refuses device memory of another device than the handle's
-        raise ValueError("the ParHIP reader needs a CUDA tensor")
-    # the handle reads the bytes on its own stream: whatever torch queued to write them must have finished
-    torch.cuda.current_stream(tensor.device).synchronize()
-    return C.c_void_p(tensor.data_ptr() or None), C.c_uint64(tensor.numel())
-
-
-def pool_usage(handle: lp.LPHandle, reset: bool = False):
-    """(bytes in use, most bytes in use since the last reset) of the device pool the handle and its results allocate
-    from; reset restarts the high-water mark at the current use."""
-    used, high = C.c_uint64(), C.c_uint64()
-    lp._check(_lib().kmp_pool_usage(handle._h, int(reset), C.byref(used), C.byref(high)))
-    return int(used.value), int(high.value)
-
-
 def read_parhip_device(handle: lp.LPHandle, path: str, ordering="natural") -> ParhipGraph:
     """read_graph of the ParHIP file at `path` on the device of `handle` (its graph and state are not touched)."""
     out = C.c_void_p()
     report = ParhipReport()
     rc = _lib().kmp_read_parhip(handle._h, str(path).encode(), _ordering(ordering), C.byref(out), C.byref(report))
-    if rc != 0:
-        _raise(rc, report)
+    lp.check_report(rc, report, ParhipError)
     return ParhipGraph(out, report, handle)
 
 
 def parse_parhip_device(handle: lp.LPHandle, tensor, ordering="natural") -> ParhipGraph:
     """The same on the bytes of a contiguous torch uint8 CUDA tensor (16-byte aligned) on the handle's device. Work
     queued on torch's current stream is waited for first, so a tensor just written by a kernel is read whole."""
-    ptr, size = _device_bytes(tensor)
+    ptr, size = lp.device_bytes(tensor)
     out = C.c_void_p()
     report = ParhipReport()
     rc = _lib().kmp_parse_parhip_device(handle._h, ptr, size, _ordering(ordering), C.byref(out), C.byref(report))
-    if rc != 0:
-        _raise(rc, report)
+    lp.check_report(rc, report, ParhipError)
     return ParhipGraph(out, report, handle)
 
 
 def _prepared(rc: int, out, report: ParhipReport, handle: lp.LPHandle) -> prepare.PreparedGraph:
-    if rc != 0:
-        _raise(rc, report)
+    lp.check_report(rc, report, ParhipError)
     prepare._lib()
     pg = prepare.PreparedGraph(out, prepare.PrepareStats(), handle)
     pg.report = report
@@ -231,7 +185,7 @@ def read_parhip_prepared(handle: lp.LPHandle, path: str) -> prepare.PreparedGrap
 
 def parse_parhip_prepared(handle: lp.LPHandle, tensor) -> prepare.PreparedGraph:
     """The same on bytes already on the device."""
-    ptr, size = _device_bytes(tensor)
+    ptr, size = lp.device_bytes(tensor)
     out = C.c_void_p()
     report = ParhipReport()
     rc = _lib().kmp_parse_parhip_device_prepared(handle._h, ptr, size, C.byref(out), C.byref(report))

@@ -39,9 +39,8 @@ class PrepareStats(C.Structure):
 def _lib():
     lib = lp.load_library()
     if not getattr(lib, "_prepare_ready", False):
-        for sym in ("kmp_prepare_graph", "kmp_prepare_graph_device", "kmp_prepared_finish", "kmp_lp_set_graph_prepared"):
-            if not hasattr(lib, sym):
-                raise RuntimeError(f"{lp.library_path()} lacks {sym}; rebuild the library")
+        lp.require_symbols(lib, "kmp_prepare_graph", "kmp_prepare_graph_device", "kmp_prepared_finish",
+                           "kmp_lp_set_graph_prepared")
         for sym in ("kmp_prepared_n", "kmp_prepared_num_isolated", "kmp_prepared_m"):
             getattr(lib, sym).restype = C.c_uint32
             getattr(lib, sym).argtypes = [C.c_void_p]
@@ -82,15 +81,10 @@ class PreparedGraph(lp.DeviceResult):
 
     def _download(self):
         if self._host is None:
-            n_all, m = self.n + self.num_isolated, self.m
-            xadj = np.zeros(n_all + 1, np.uint32)
-            adj = np.zeros(m, np.uint32)
-            vw = np.zeros(n_all, np.int32) if self._has_vwgt else None
-            ew = np.zeros(m, np.int32) if self._has_adjwgt else None
+            n_all = self.n + self.num_isolated
             o2n = np.zeros(n_all, np.uint32)
-            lp._check(_lib().kmp_prepared_download(self._g, lp._ptr(xadj), lp._ptr(adj), lp._ptr(vw), lp._ptr(ew),
-                                                   lp._ptr(o2n)))
-            self._host = (xadj, adj, vw, ew, o2n)
+            self._host = self._download_csr("kmp_prepared_download", n_all, self.m, self._has_vwgt, self._has_adjwgt,
+                                            o2n) + (o2n,)
         return self._host
 
     def old_to_new(self) -> np.ndarray:

@@ -39,9 +39,8 @@ class SubgraphStats(C.Structure):
 def _lib():
     lib = lp.load_library()
     if not getattr(lib, "_subgraph_ready", False):
-        for sym in ("kmp_extract_subgraphs", "kmp_subgraphs_copy_partitions", "kmp_subgraphs_copy_partitions_device"):
-            if not hasattr(lib, sym):
-                raise RuntimeError(f"{lp.library_path()} lacks {sym}; rebuild the library")
+        lp.require_symbols(lib, "kmp_extract_subgraphs", "kmp_subgraphs_copy_partitions",
+                           "kmp_subgraphs_copy_partitions_device")
         for sym in ("kmp_subgraphs_k", "kmp_subgraphs_n", "kmp_subgraphs_m"):
             getattr(lib, sym).restype = C.c_uint32
             getattr(lib, sym).argtypes = [C.c_void_p]

@@ -52,11 +52,7 @@ class GraphReport(C.Structure):
 
     def message(self) -> str:
         """The reference's warning line for the first violation ("" when valid)."""
-        lib = _lib()
-        size = lib.kmp_graph_report_message(C.byref(self), None, 0)
-        buf = C.create_string_buffer(size + 1)
-        lib.kmp_graph_report_message(C.byref(self), buf, size + 1)
-        return buf.value.decode()
+        return lp.report_message(_lib().kmp_graph_report_message, self)
 
     def __repr__(self) -> str:
         return (f"GraphReport({self.kind_name}, u={self.u}, e={self.e}, v={self.v}, e_rev={self.e_rev}, "
@@ -66,9 +62,7 @@ class GraphReport(C.Structure):
 def _lib():
     lib = lp.load_library()
     if not getattr(lib, "_validate_ready", False):
-        for sym in ("kmp_validate_graph", "kmp_validate_graph_device", "kmp_graph_report_message"):
-            if not hasattr(lib, sym):
-                raise RuntimeError(f"{lp.library_path()} lacks {sym}; rebuild the library")
+        lp.require_symbols(lib, "kmp_validate_graph", "kmp_validate_graph_device", "kmp_graph_report_message")
         lib.kmp_validate_graph.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32] + [C.c_void_p] * 4
         lib.kmp_validate_graph_device.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32] + [C.c_void_p] * 4
         lib.kmp_graph_report_message.argtypes = [C.c_void_p, C.c_char_p, C.c_size_t]

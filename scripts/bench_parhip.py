@@ -91,28 +91,29 @@ def pool_peaks(h, data, path):
     before a step and the use before the first step is subtracted. From a file the bytes are staged in the pool and
     counted there. From resident bytes the caller's tensor is added where it must stay alive: through the whole fused
     parse, but only through the natural parse of the two-step path."""
+    from kaminpar_b200 import lp
     from kaminpar_b200 import parhip as PH
     from kaminpar_b200 import prepare as PR
 
     length = data.numel()
     res = {}
-    base, _ = PH.pool_usage(h, reset=True)
+    base, _ = lp.pool_usage(h, reset=True)
     PH.read_parhip_prepared(h, path).close()
-    res["read_fused"] = PH.pool_usage(h)[1] - base
-    base, _ = PH.pool_usage(h, reset=True)
+    res["read_fused"] = lp.pool_usage(h)[1] - base
+    base, _ = lp.pool_usage(h, reset=True)
     g = PH.read_parhip_device(h, path, "natural")
     pg = PR.rearrange_by_degree_buckets_device(h, g.n, g.m, *g.device_arrays()[:4])
-    res["read_then_prepare"] = PH.pool_usage(h)[1] - base
+    res["read_then_prepare"] = lp.pool_usage(h)[1] - base
     pg.close()
     g.close()
-    base, _ = PH.pool_usage(h, reset=True)
+    base, _ = lp.pool_usage(h, reset=True)
     PH.parse_parhip_prepared(h, data).close()
-    res["parse_fused"] = PH.pool_usage(h)[1] - base + length
-    base, _ = PH.pool_usage(h, reset=True)
+    res["parse_fused"] = lp.pool_usage(h)[1] - base + length
+    base, _ = lp.pool_usage(h, reset=True)
     g = PH.parse_parhip_device(h, data, "natural")
-    p1 = PH.pool_usage(h, reset=True)[1] - base
+    p1 = lp.pool_usage(h, reset=True)[1] - base
     pg = PR.rearrange_by_degree_buckets_device(h, g.n, g.m, *g.device_arrays()[:4])
-    p2 = PH.pool_usage(h)[1] - base
+    p2 = lp.pool_usage(h)[1] - base
     res["parse_then_prepare"] = max(p1 + length, p2)
     pg.close()
     g.close()
