@@ -23,6 +23,8 @@
 //                      kaminpar-shm/graphutils/permutator.cc:66-91, 236-264, kaminpar.cc:368-445 (DESIGN.md §15)
 //   Subgraphs / extract_subgraphs / copy_subgraph_partitions
 //                      kaminpar-shm/graphutils/subgraph_extractor.cc:181-324, 492-533 (DESIGN.md §16)
+//   bipartition_subgraphs
+//                      kaminpar-shm/initial_partitioning/ (InitialBipartitionerWorkerPool::bipartition, DESIGN.md §20)
 //   MetisGraph / read_metis
 //                      kaminpar-io/metis_parser.cc:158-245 (csr_read on the device, DESIGN.md §18)
 //   ParhipGraph / read_parhip
@@ -42,6 +44,7 @@
 #include <vector>
 
 #include "kaminpar_b200_balancer.h"
+#include "kaminpar_b200_bipartition.h"
 #include "kaminpar_b200_contraction.h"
 #include "kaminpar_b200_io.h"
 #include "kaminpar_b200_parhip.h"
@@ -610,6 +613,25 @@ inline void copy_subgraph_partitions(kmp_lp_handle *h, const Subgraphs &subgraph
   }
   detail::check(kmp_subgraphs_copy_partitions(h, subgraphs.device(), k_prime, input_k, sub_partitions.data(),
                                               out.empty() ? nullptr : out.data(), nullptr));
+}
+
+// InitialBipartitionerWorkerPool::bipartition on every block of `subgraphs` that is split in two, on the device
+// (kmp_bipartition_subgraphs): d_sub_partitions (n entries of device memory) receives the block-major sub-partitions
+// that copy_subgraph_partitions' device form takes. input_max_block_weights: the input partition context's input_k
+// maximum block weights.
+inline kmp_bipartition_stats bipartition_subgraphs(kmp_lp_handle *h, const Subgraphs &subgraphs, BlockID k_prime,
+                                                   BlockID input_k, std::span<const BlockWeight> input_max_block_weights,
+                                                   bool uniform_block_weights, std::int64_t input_total_node_weight,
+                                                   double input_epsilon, const kmp_ip_config &cfg, std::int32_t seed,
+                                                   std::uint32_t *d_sub_partitions) {
+  if (input_max_block_weights.size() != input_k) {
+    throw std::invalid_argument("bipartition_subgraphs: input_max_block_weights needs input_k entries");
+  }
+  kmp_bipartition_stats stats{};
+  detail::check(kmp_bipartition_subgraphs(h, subgraphs.device(), k_prime, input_k, input_max_block_weights.data(),
+                                          uniform_block_weights ? 1 : 0, input_total_node_weight, input_epsilon, &cfg,
+                                          seed, d_sub_partitions, &stats));
+  return stats;
 }
 
 namespace detail {

@@ -3208,6 +3208,7 @@ int kmp_lp_step_finish(kmp_lp_handle *h, uint32_t *labels_out, int32_t *block_we
 #include "kmp_underload.cuh"
 #include "kmp_prepare.cuh"
 #include "kmp_subgraph.cuh"
+#include "kmp_bipartition_dev.cuh"
 #include "kmp_validate.cuh"
 #include "kmp_read.cuh"
 #include "kmp_metis.cuh"

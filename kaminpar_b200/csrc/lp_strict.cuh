@@ -25,105 +25,24 @@
 
 #include <cstdint>
 
-#if defined(__CUDACC__)
-#define KMP_HD __host__ __device__
-#else
-#define KMP_HD
-#endif
+#include "kmp_rng.cuh"
 
 namespace kmp_strict {
+
+using namespace kmp_rng;
 
 constexpr uint32_t kInvalid = 0xFFFFFFFFu;
 constexpr uint32_t kRatingMapThreshold = 10000; // label_propagation.h:62
 constexpr uint32_t kPermSize = 64, kNumPerms = 64; // RandomPermutations<NodeID, 64, 64>
-constexpr uint32_t kBools = 1024;
 
-// ---- std::mt19937 + the libstdc++ distributions ------------------------------------------------
-struct Rng {
-  uint32_t mt[624];
-  uint32_t idx;
-  uint8_t bools[kBools];
-  uint32_t next_bool;
+// ---- Random / RandomPermutations<NodeID, 64, 64> -------------------------------------------------
+struct Rng : RngCore {
   uint32_t perms[kNumPerms][kPermSize];
 };
 
-KMP_HD inline void mt_seed(Rng &r, uint32_t seed) {
-  r.mt[0] = seed;
-  for (uint32_t i = 1; i < 624; ++i) {
-    r.mt[i] = 1812433253u * (r.mt[i - 1] ^ (r.mt[i - 1] >> 30)) + i;
-  }
-  r.idx = 624;
-}
-KMP_HD inline uint32_t mt_next(Rng &r) {
-  if (r.idx >= 624) {
-    for (uint32_t i = 0; i < 624; ++i) {
-      const uint32_t y = (r.mt[i] & 0x80000000u) | (r.mt[(i + 1) % 624] & 0x7FFFFFFFu);
-      r.mt[i] = r.mt[(i + 397) % 624] ^ (y >> 1) ^ ((y & 1u) ? 0x9908B0DFu : 0u);
-    }
-    r.idx = 0;
-  }
-  uint32_t y = r.mt[r.idx++];
-  y ^= y >> 11;
-  y ^= (y << 7) & 0x9D2C5680u;
-  y ^= (y << 15) & 0xEFC60000u;
-  y ^= y >> 18;
-  return y;
-}
-// uniform_int_distribution<T>(0, range - 1) on a 32-bit generator, 1 <= range <= 2^32 - 1 (_S_nd<uint64_t>)
-KMP_HD inline uint32_t uniform_below(Rng &r, uint32_t range) {
-  uint64_t product = static_cast<uint64_t>(mt_next(r)) * range;
-  uint32_t low = static_cast<uint32_t>(product);
-  if (low < range) {
-    const uint32_t threshold = (0u - range) % range;
-    while (low < threshold) {
-      product = static_cast<uint64_t>(mt_next(r)) * range;
-      low = static_cast<uint32_t>(product);
-    }
-  }
-  return static_cast<uint32_t>(product >> 32);
-}
-// std::shuffle(first, first + size, gen) over 32-bit elements; stride: elements are `stride` words wide
-// (chunks are {start, end} pairs) -- the index sequence does not depend on the element type
-KMP_HD inline void swap_elems(uint32_t *a, uint64_t i, uint64_t j, uint32_t stride) {
-  for (uint32_t q = 0; q < stride; ++q) {
-    const uint32_t t = a[i * stride + q];
-    a[i * stride + q] = a[j * stride + q];
-    a[j * stride + q] = t;
-  }
-}
-KMP_HD inline void shuffle(Rng &r, uint32_t *a, uint64_t size, uint32_t stride = 1) {
-  if (size == 0) {
-    return;
-  }
-  const uint64_t urngrange = 0xFFFFFFFFull;
-  if (urngrange / size >= size) {
-    uint64_t i = 1;
-    if ((size % 2) == 0) {
-      swap_elems(a, i, uniform_below(r, 2), stride);
-      ++i;
-    }
-    while (i != size) {
-      const uint64_t swap_range = i + 1;
-      const uint32_t x = uniform_below(r, static_cast<uint32_t>(swap_range * (swap_range + 1)));
-      const uint64_t p0 = x / (swap_range + 1), p1 = x % (swap_range + 1);
-      swap_elems(a, i, p0, stride);
-      ++i;
-      swap_elems(a, i, p1, stride);
-      ++i;
-    }
-    return;
-  }
-  for (uint64_t i = 1; i != size; ++i) {
-    swap_elems(a, i, uniform_below(r, static_cast<uint32_t>(i + 1)), stride);
-  }
-}
 // Random::reseed (random.cc:45-56) with thread index 0 + RandomPermutations ctor (random.h:138-143)
 KMP_HD inline void rng_init(Rng &r, int seed) {
-  mt_seed(r, static_cast<uint32_t>(seed));
-  r.next_bool = 0;
-  for (uint32_t i = 0; i < kBools; ++i) {
-    r.bools[i] = static_cast<uint8_t>(uniform_below(r, 2));
-  }
+  rng_seed(r, seed);
   for (uint32_t p = 0; p < kNumPerms; ++p) {
     for (uint32_t i = 0; i < kPermSize; ++i) {
       r.perms[p][i] = i;
@@ -131,8 +50,6 @@ KMP_HD inline void rng_init(Rng &r, int seed) {
     shuffle(r, r.perms[p], kPermSize);
   }
 }
-KMP_HD inline uint32_t random_index(Rng &r, uint32_t lo, uint32_t hi) { return lo + uniform_below(r, hi - lo); } // random.h:64-68
-KMP_HD inline bool random_bool(Rng &r) { return r.bools[r.next_bool++ % kBools] != 0; }                          // random.h:70-72
 
 // ---- engine state (device memory, owned by the handle) ----------------------------------------
 struct Stats {

@@ -6,6 +6,8 @@
         (graphutils/subgraph_extractor.cc:181-324)
     Subgraphs.copy_partitions(handle, sub_partitions, k_prime, input_k)
         graph::copy_subgraph_partitions (subgraph_extractor.cc:492-533)
+    Subgraphs.bipartition(handle, k_prime, input_k, max_block_weights, seed=...)
+        InitialBipartitionerWorkerPool::bipartition on every block split in two (kaminpar_b200/bipartition.py)
 
 Between the two, a caller bipartitions each block (on the host: `block(b)`, or on another handle: `device_view(b)`)
 and lays the sub-partitions out block-major, block b's at [node_off[b], node_off[b + 1]).
@@ -157,6 +159,18 @@ class Subgraphs(lp.DeviceResult):
             lp._check(lib.kmp_subgraphs_copy_partitions(handle._h, self._g, C.c_uint32(k_prime), C.c_uint32(input_k),
                                                         lp._ptr(sub), lp._ptr(out), lp._ptr(bw)))
         return out, bw
+
+    def bipartition(self, handle: lp.LPHandle, k_prime: int, input_k: int, max_block_weights, *, seed: int,
+                    total_node_weight: int, ip_config=None, uniform: bool = True, epsilon: float = 0.03):
+        """KaMinPar's initial bipartitioner on every block split in two (kaminpar_b200.bipartition, DESIGN.md §20):
+        a torch tensor of n sub-block ids on the device, block-major; its data_ptr() goes straight into
+        copy_partitions. max_block_weights / total_node_weight / uniform / epsilon: the input graph's partition
+        context at input_k."""
+        from . import bipartition as BP
+
+        out, _ = BP.bipartition(self, handle, k_prime, input_k, max_block_weights, seed=seed, ip_config=ip_config,
+                                uniform=uniform, total_node_weight=total_node_weight, epsilon=epsilon)
+        return out
 
 
 def extract_subgraphs(handle: lp.LPHandle, k: int, partition: Optional[np.ndarray] = None) -> Subgraphs:
